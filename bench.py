@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py — the contract benchmark of the batched TinyMPC solve path on B200.
+"""bench.py — the contract benchmark of the batched TinyMPC solve path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -23,6 +23,10 @@ configs: the other BASELINE configs, each timed the same way (device events, L2 
            C5  three corners of the random-LTI sweep at 2^20/8 = 131072 instances per GPU, fixed work (50 iterations)
          Under --gpus N every config runs sharded the same way (weak: fixed instances per GPU).
 roofline, cpu_baseline, clocks: see DESIGN.md §7.
+
+--dump-outputs DIR writes, after the timed steps, what the headline's timed path returned in its last step (rank 0):
+sol_x, sol_u, residuals (float32) and iter, solved (float64) as DIR/<name>.npy, for a fixed sample of DUMP_INSTANCES
+instances drawn with a fixed seed (the inputs are seeded too), so that two builds can be compared output for output.
 
 --impl reference times the reference's own CPU implementation (oracle/_ref = the unmodified reference compiled
 here; falls back to the oracle port when the prebuilt library is absent) on the host cores, same metric/config:
@@ -47,6 +51,7 @@ sys.path.insert(0, ROOT)
 WORKLOAD = "quadrotor_hovering nx=12 nu=4 N=50 box batch=65536/GPU identical instances fp32 cold-start max_iter=100 (BASELINE configs[1])"
 METRIC = "MPC instances solved/sec (terminated by the reference rule; ADMM iters/sec/GPU alongside)"
 B_PER_GPU = 65536
+DUMP_INSTANCES = 4096  # sample of the headline batch written by --dump-outputs (~13 MB)
 N_HORIZON = 50
 KERNEL_NAMES = {1: "tpi", 2: "gpi", 4: "gps"}
 # `config` is the same dict in both arms (the driver compares them); arm-specific details go to `plan` / `arm`
@@ -66,6 +71,7 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the `configs` block (C3/C4/C5)")
     ap.add_argument("--extra-steps", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (a seeded sample) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -362,7 +368,7 @@ class Gpu:
         self.torch, self.dist = torch, dist
         self.args, self.local, self.world = args, local, world
         self.dev = torch.device("cuda", local)
-        self.flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=self.dev)  # > 126 MB L2
+        self.flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=self.dev)  # > 50 MB L2
         self.stream = torch.cuda.current_stream(self.dev)
 
     def barrier(self):
@@ -457,6 +463,15 @@ def plan_of(st):
             "tmem_cols_per_cta": st["tmem_cols_per_cta"], "instances_per_cta": st["instances_per_cta"]}
 
 
+def dump_outputs(d, out, B):
+    """the arrays a caller of the timed path receives, restricted to a seeded sample of instances"""
+    os.makedirs(d, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(B, size=min(B, DUMP_INSTANCES), replace=False))
+    for name in ("sol_x", "sol_u", "residuals", "iter", "solved"):
+        a = out[name].cpu().numpy()[idx]
+        np.save(os.path.join(d, name + ".npy"), a if a.dtype.kind == "f" else a.astype(np.float64))
+
+
 def main():
     args = parse()
     rank = int(os.environ.get("RANK", "0"))
@@ -491,7 +506,7 @@ def main():
     if os.path.exists(peaks_path):
         peak, peak_src = float(json.load(open(peaks_path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
     # ---- headline: C2 ----
     case = make_case("C2")
@@ -503,6 +518,8 @@ def main():
     time.sleep(0.25)
     t_wall0 = time.perf_counter()
     batch, out, step_ms = g.device_arm(solver, case, K, W)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out, B)
     total_ms = float(sum(step_ms))
     st = solver.stats()
     iters_step = int(out["iter"].sum().item())
@@ -517,17 +534,9 @@ def main():
     e2e_ok = bool(np.array_equal(hb.sol_u.view(np.uint8), out["sol_u"].cpu().numpy().view(np.uint8)))
     k_ms = float(np.mean(step_ms))  # one launch per step: the step IS the kernel
     roof = roofline(case, st, k_ms, iters_step, peak, peak_src)
-    traffic_table = {}
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        try:
-            traffic_table = json.load(open(tpath))  # DRAM bytes per launch from the committed ncu captures
-        except Exception:
-            traffic_table = {}
-    roof["traffic"] = traffic_table.get(f"family{st['kernel_family']}_{args.mode}")
-    roof["note"] = ("compute-bound by construction (SURVEY §8d: ~2000 flop per compulsory byte); the fp32-pipe / issue-slot "
-                    "utilisation from ncu is the quality figure (profiles/r02_ncu_summary.md)")
-    roof["flops_frac_of_74.5_tflops_fp32"] = roof["flops_achieved_tflops"] / 74.5
+    roof["note"] = ("compute-bound by construction (SURVEY §8d: ~2000 flop per compulsory byte); the achieved fp32 rate "
+                    "against the data sheet's is the quality figure")
+    roof["flops_frac_of_67_tflops_fp32"] = roof["flops_achieved_tflops"] / 67.0  # H100 SXM data sheet, dense FP32
     del batch, out, hb
     solver.close()
     torch.cuda.empty_cache()
@@ -556,7 +565,6 @@ def main():
                      "iter_histogram_rank0": {str(i): n for i, n in enumerate(hist) if n},
                      "plan": plan_of(sx), "gpu_launches": Kx * sx["kernel_launches"],
                      "roofline": roofline(c, sx, kx, iters_x, peak, peak_src)}
-            entry["roofline"]["traffic"] = traffic_table.get(f"{name.split('_')[0].lower()}_family{sx['kernel_family']}_{args.mode}")
             extra_launches += Kx * sx["kernel_launches"]
             del b_, o_
             if name in ("C3", "C4"):

@@ -1,10 +1,10 @@
 /*
- * tinympc_b200.h — C ABI of the B200-native batched TinyMPC solve path.
+ * tinympc_b200.h — C ABI of the H100-native (sm_90a) batched TinyMPC solve path.
  *
  * This is the drop-in boundary for the hot path of TinyMPC/TinyMPC:
  *     tiny_solve()  (reference src/tinympc/tiny_api.cpp:384-386)
  *       -> solve()  (reference src/tinympc/admm.cpp:331-455)
- * run for B independent MPC instances per call on one B200.
+ * run for B independent MPC instances per call on one H100.
  *
  * Plain C: POD structs, raw pointers, sizes.  No Eigen, no torch types.
  * The reference's own "C" API (src/tinympc/tiny_api.hpp:10-62) passes Eigen
@@ -45,9 +45,9 @@ extern "C" {
 /* kernel family selection (TINYMPC_KERNEL_AUTO picks the fastest that fits) */
 #define TINYMPC_KERNEL_AUTO 0
 #define TINYMPC_KERNEL_TPI 1 /* thread-per-instance, state streamed through HBM/L2 (any feature set)   */
-#define TINYMPC_KERNEL_GPI 2 /* lane-group-per-instance: state resident on chip (shared + tensor memory) when the   */
+#define TINYMPC_KERNEL_GPI 2 /* lane-group-per-instance: state resident on chip (shared memory) when the            */
                              /* problem is box-constrained and fits, else the streamed variant below               */
-/* 3 was an experimental split of a batch between the GPI and TPI kernels; removed (it never won, see profiles/) */
+/* 3 was an experimental split of a batch between the GPI and TPI kernels; removed (it never won) */
 #define TINYMPC_KERNEL_GPS 4 /* lane-group-per-instance, state streamed through an L2/HBM workspace by TMA bulk     */
                              /* copies (any feature set: box, cones, hyperplanes; fp32 and fp64)                   */
 
@@ -189,7 +189,7 @@ typedef struct tinympc_b200_stats {
     int32_t ctas;
     int32_t threads_per_cta;
     int64_t gpi_instances; /* instances of the batch solved by a lane-group kernel (GPI or GPS) */
-    int32_t tmem_cols_per_cta; /* GPI: tensor-memory columns holding the dual variables and d (0 = all in shared memory) */
+    int32_t tmem_cols_per_cta; /* always 0: the state of every kernel family lives in shared / global memory on sm_90   */
     int32_t reserved0;
     int64_t workspace_bytes; /* GPS / TPI: bytes of streamed-state workspace behind the last solve (0 = state on chip) */
 } tinympc_b200_stats_t;

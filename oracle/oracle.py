@@ -29,7 +29,8 @@ _libs = {}
 
 
 def build(verbose=False):
-    """Build the C restatement and, when /root/reference is present, the reference libraries."""
+    """Build the C restatement and, when the TinyMPC checkout (TINYMPC_REFERENCE, default /root/reference) is present,
+    the reference libraries."""
     r = subprocess.run(["make", "-C", _HERE, "-j8", "all"], capture_output=True, text=True)
     if verbose or r.returncode:
         print(r.stdout[-4000:], r.stderr[-4000:])

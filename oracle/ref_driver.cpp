@@ -1,7 +1,7 @@
 // oracle/ref_driver.cpp — TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 //
 // A raw-pointer batched driver around the UNMODIFIED reference (TinyMPC/TinyMPC).  It is compiled
-// together with the reference's own sources where they lie under /root/reference
+// together with the reference's own sources where they lie in a TinyMPC checkout
 // (src/tinympc/{admm,tiny_api,rho_benchmark}.cpp + the vendored Eigen) by oracle/Makefile, with outputs
 // only into oracle/_ref/ (git-ignored).  Nothing from the reference is copied into this repository.
 //

@@ -3,7 +3,7 @@
  *
  * Plain-C CPU restatement of the reference's solve path, included twice by tinympc_oracle.c
  * (once with T = double, once with T = float).  Each function cites the reference lines it follows
- * (paths relative to /root/reference).  Arithmetic contract (SURVEY Appendix A/B.2, validated there
+ * (paths relative to the TinyMPC checkout).  Arithmetic contract (SURVEY Appendix A/B.2, validated there
  * and re-validated by tests/test_oracle_vs_reference.py against oracle/_ref):
  *   - every dot product is  s = a0*b0; s = s + ak*bk  for k ascending, separate multiply and add
  *     (compile with -ffp-contract=off);

@@ -1,5 +1,7 @@
 #!/usr/bin/env python3
-"""Generate the golden fixtures from the UNMODIFIED reference (run in the build container only).
+"""Generate the golden fixtures from the UNMODIFIED reference (needs the compiled reference under oracle/_ref,
+see oracle/Makefile: make -C oracle REF=<TinyMPC checkout>, and for the example outputs the binaries the shim Makefile
+builds from the same checkout).
 
     python tests/golden/make_golden.py
 
@@ -10,9 +12,19 @@ per case, one compressed .npz with
   * the settings, the inputs of every step (x0 sequence, Xref, Uref),
   * the reference's outputs of every step (solution, iter, solved, residuals, and every state array).
 The fixtures pin the oracle restatement (tests/test_oracle_golden.py, runs anywhere) and the CUDA path
-(tests/test_gpu_parity.py) to the reference bit-for-bit without /root/reference being present.
+(tests/test_gpu_parity.py) to the reference bit-for-bit without the reference being present.
+
+tests/golden/reference/ holds what the other reference comparisons check against:
+  * lti_sweep_{f32,f64}.npz   the randomised (nx, nu) sweep of tests/test_oracle_vs_reference.py (the cache tiny_setup
+                              derives, x0 sequence and the SHA-256 digest of every output array of every step),
+  * precompute_{f32,f64}.npz  the cache tiny_setup derives for the models of the device-precompute test,
+  * sensitivity_tables.npz    tiny_initialize_sensitivity_matrices' tables,
+  * examples.json             per example program of the reference: how many lines its stdout has, how many of them are
+                              result lines (helpers.example_key_lines) and the SHA-256 digest of those.
 """
+import json
 import os
+import subprocess
 import sys
 
 import numpy as np
@@ -30,7 +42,63 @@ PROBLEM_FIELDS = ["A", "B", "f", "Q", "R", "Kinf", "Pinf", "Quu_inv", "AmBKt", "
                   "tv_blin_x", "tv_Alin_u", "tv_blin_u"]
 
 
+def save_problem(out, prefix, prob):
+    for f in PROBLEM_FIELDS:
+        v = getattr(prob, f)
+        if v is not None:
+            out[prefix + "prob_" + f] = v
+
+
+def ref_fn(prob, settings, x0, Xref, Uref, state, cold, want):
+    return oracle.solve_batch(prob, settings, x0, Xref, Uref, state=state, cold_start=cold, want_state=want, impl="reference")
+
+
+def make_reference_checks():
+    os.makedirs(H.REFERENCE_DIR, exist_ok=True)
+    for dt in (np.float32, np.float64):
+        tag = "f32" if dt == np.float32 else "f64"
+        out = {}
+        for n, (nx, nu, N, spec, inst) in enumerate(H.lti_sweep_cases(dt)):
+            prob = H.problem_from_spec(spec, dt, oracle.ref_setup)
+            res, x0s = H.closed_loop(prob, spec.settings, inst, 3, False, H.BOX_STATE, ref_fn)
+            for f in H.CACHE_FIELDS:
+                out[f"d{n}_{f}"] = getattr(prob, f)
+            out[f"d{n}_x0_seq"] = np.stack(x0s)
+            out[f"d{n}_digests"] = np.array([[H.digest(r[key]) for key in H.OUT_KEYS + H.BOX_STATE] for r in res])
+        path = os.path.join(H.REFERENCE_DIR, f"lti_sweep_{tag}.npz")
+        np.savez_compressed(path, **out)
+        print(f"{path}: {os.path.getsize(path)} bytes")
+        out = {}
+        for n, (nx, nu, spec) in enumerate(H.precompute_models()):
+            prob = H.problem_from_spec(spec, dt, oracle.ref_setup)
+            for f in H.CACHE_FIELDS:
+                out[f"m{n}_{f}"] = getattr(prob, f)
+        path = os.path.join(H.REFERENCE_DIR, f"precompute_{tag}.npz")
+        np.savez_compressed(path, **out)
+        print(f"{path}: {os.path.getsize(path)} bytes")
+    import ctypes as C
+    shapes = [(4, 12), (12, 12), (4, 4), (12, 12)]
+    ref = [np.zeros(s, np.float64, order="F") for s in shapes]
+    assert oracle.ref_lib(np.float64).tinympc_ref_sensitivity_tables(*[C.c_void_p(a.ctypes.data) for a in ref]) == 0
+    np.savez_compressed(os.path.join(H.REFERENCE_DIR, "sensitivity_tables.npz"), **{f"t{i}": a for i, a in enumerate(ref)})
+    make_example_digests()
+
+
+def make_example_digests():
+    exdir = os.path.join(os.path.dirname(os.path.dirname(HERE)), "oracle", "_ref", "examples_ref")
+    ex = {}
+    for name in sorted(os.listdir(exdir)):
+        r = subprocess.run([os.path.join(exdir, name)], capture_output=True, text=True, timeout=600, cwd=exdir, check=True)
+        key = H.example_key_lines(r.stdout.splitlines())
+        ex[name] = {"lines": len(key), "sha256": H.text_digest(key), "stdout_lines": len(r.stdout.splitlines())}
+    with open(os.path.join(H.REFERENCE_DIR, "examples.json"), "w") as fh:
+        json.dump(ex, fh, indent=1, sort_keys=True)
+        fh.write("\n")
+    print(ex)
+
+
 def main():
+    make_reference_checks()
     cases = H.make_cases()
     for name in sorted(cases):
         c = cases[name]
@@ -44,10 +112,7 @@ def main():
         res, x0s = H.closed_loop(prob, st, c["inst"], c["steps"], c["reset_duals"], c["state"], fn)
         out = dict(nx=prob.nx, nu=prob.nu, N=prob.N, rho=prob.rho, dtype=np.dtype(prob.dtype).name, steps=c["steps"],
                    reset_duals=int(c["reset_duals"]), state_names=np.array(c["state"]))
-        for f in PROBLEM_FIELDS:
-            v = getattr(prob, f)
-            if v is not None:
-                out["prob_" + f] = v
+        save_problem(out, "", prob)
         for n, _ in abi.Settings._fields_:
             out["set_" + n] = getattr(st, n)
         out["Xref"] = np.asarray(c["inst"]["Xref"], dtype=prob.dtype)

@@ -2,6 +2,7 @@
 workloads) and a closed-loop runner that feeds warm-start state back the way the reference's examples do."""
 from __future__ import annotations
 
+import hashlib
 import os
 
 import numpy as np
@@ -10,12 +11,32 @@ from tinympc_b200 import abi, workloads as wl
 from tinympc_b200.problem import MPCProblem, copy_settings
 
 GOLDEN_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+REFERENCE_DIR = os.path.join(GOLDEN_DIR, "reference")  # stored outputs of the unmodified reference (golden/make_golden.py)
+CACHE_FIELDS = ("Q", "R", "Kinf", "Pinf", "Quu_inv", "AmBKt", "APf", "BPf")
 BOX_STATE = ["x", "u", "v", "z", "vnew", "znew", "g", "y"]
 SOC_STATE = BOX_STATE + ["vcnew", "zcnew", "gc", "yc"]
 LIN_STATE = BOX_STATE + ["vlnew", "zlnew", "gl", "yl"]
 TVLIN_STATE = BOX_STATE + ["vlnew_tv", "zlnew_tv", "gl_tv", "yl_tv"]
 ALL_STATE = list(abi.STATE_FIELDS)
 OUT_KEYS = ["sol_x", "sol_u", "iter", "solved", "residuals"]
+
+
+def digest(a):
+    """Bit-exact fingerprint of an array (bytes, shape and dtype): stored in place of large reference outputs."""
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(a.tobytes() + repr((a.shape, a.dtype.str)).encode()).hexdigest()
+
+
+def text_digest(lines):
+    return hashlib.sha256("\n".join(lines).encode()).hexdigest()
+
+
+EXAMPLE_KEYS = ("tracking error", "terations", "converged", "Tracking", "Average")
+
+
+def example_key_lines(lines):
+    """The lines of an example program's output that carry results (errors, iteration counts, convergence)."""
+    return [ln for ln in lines if any(t in ln for t in EXAMPLE_KEYS)]
 
 
 def bits_equal(a, b):
@@ -130,12 +151,42 @@ def closed_loop(prob: MPCProblem, settings, inst, steps, reset_duals, state_name
     return results, x0s
 
 
+def lti_sweep_cases(dt):
+    """Randomised sweep over the compiled (nx, nu) pairs and short horizons (BASELINE config 5's generator):
+    -> [(nx, nu, N, spec, inst)], the state pushed into the bounds."""
+    dims = [(4, 1), (4, 2), (4, 8), (6, 3), (8, 4), (12, 2), (12, 8), (16, 4), (16, 8)]
+    out = []
+    for n, (nx, nu) in enumerate(dims):
+        N = (3, 7, 12)[n % 3]
+        sp = wl.random_lti(nx, nu, N, seed=40 + n)
+        sp.settings.max_iter = 25
+        sp.settings.check_termination = 1 + n % 3
+        inst = wl.random_instances(5, nx, N, seed=70 + n, dtype=dt)
+        inst["x0"] = (3.0 * inst["x0"]).astype(dt)
+        out.append((nx, nu, N, sp, inst))
+    return out
+
+
+def precompute_models():
+    """The models whose cache the device precompute is compared on: -> [(nx, nu, spec)]"""
+    groups = ((12, 4, [wl.quadrotor(N=10), wl.quadrotor(N=10, hz=50)] + [wl.random_lti(12, 4, 10, seed=i) for i in range(6)]),
+              (6, 3, [wl.rocket(N=10)] + [wl.random_lti(6, 3, 10, seed=i) for i in range(5)]),
+              (16, 8, [wl.random_lti(16, 8, 10, seed=i) for i in range(6)]))
+    return [(nx, nu, sp) for nx, nu, specs in groups for sp in specs]
+
+
+def load_problem(d, prefix, nx, nu, N, dt, rho):
+    """MPCProblem from the prob_* arrays a golden file stores under `prefix`"""
+    p = prefix + "prob_"
+    kw = {k[len(p):]: d[k] for k in d.files if k.startswith(p)}
+    return MPCProblem(nx=nx, nu=nu, N=N, dtype=dt, rho=float(dt(rho)), **kw)
+
+
 def load_golden(name):
     """-> (MPCProblem, Settings, inst, meta, steps[list of dict]) from tests/golden/<name>.npz"""
     d = np.load(os.path.join(GOLDEN_DIR, name + ".npz"))
     dt = np.dtype(str(d["dtype"])).type
-    kw = {k[5:]: d[k] for k in d.files if k.startswith("prob_")}
-    prob = MPCProblem(nx=int(d["nx"]), nu=int(d["nu"]), N=int(d["N"]), dtype=dt, rho=float(d["rho"]), **kw)
+    prob = load_problem(d, "", int(d["nx"]), int(d["nu"]), int(d["N"]), dt, float(d["rho"]))
     st = abi.Settings()
     for n, _ in abi.Settings._fields_:
         setattr(st, n, type(getattr(st, n))(d["set_" + n]))

@@ -22,7 +22,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(abi.EXPORTS), declared ^ set(abi.EXPORTS)
     for n in declared:
         assert hasattr(lib, n), n
-    assert b"sm_100a" in lib.tinympc_b200_version()
+    assert b"sm_90a" in lib.tinympc_b200_version()
 
 
 def test_struct_layout_matches_header():

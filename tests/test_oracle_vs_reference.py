@@ -1,14 +1,14 @@
-"""The C restatement (oracle/tinympc_oracle.c) must be BIT-IDENTICAL to the unmodified reference compiled
-with the pinned flags (oracle/_ref/libtinympc_ref_{f64,f32}.so) on every parity case, through warm-started
-closed loops.  Runs only where the reference library exists (the build container; it is prebuilt and travels
-to the GPU box too)."""
+"""The C restatement (oracle/tinympc_oracle.c) against the unmodified reference compiled with the pinned flags: its
+precompute, and a randomised sweep of warm-started closed loops over the compiled (nx, nu) pairs, bit for bit.  The
+reference's outputs are stored under tests/golden (tests/golden/make_golden.py), so these checks run anywhere; the
+parity cases themselves are replayed by tests/test_oracle_golden.py."""
+import os
+
 import numpy as np
 import pytest
 
 import helpers as H
 from oracle import oracle
-
-CASES = H.make_cases()
 
 
 def _solve(impl):
@@ -17,30 +17,12 @@ def _solve(impl):
     return fn
 
 
-@pytest.mark.parametrize("name", sorted(CASES))
-def test_port_bit_identical_to_reference(name):
-    c = CASES[name]
-    if not oracle.ref_available(c["dtype"]):
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
-    prob = H.problem_from_spec(c["spec"], c["dtype"], oracle.ref_setup)
-    st = c["spec"].settings
-    ref, x0s = H.closed_loop(prob, st, c["inst"], c["steps"], c["reset_duals"], c["state"], _solve("reference"))
-    port, _ = H.closed_loop(prob, st, c["inst"], c["steps"], c["reset_duals"], c["state"], _solve("port"), x0_seq=x0s)
-    moved = 0
-    for k, (r, p) in enumerate(zip(ref, port)):
-        for key in H.OUT_KEYS + c["state"]:
-            assert H.bits_equal(r[key], p[key]), f"{name} step {k}: {key} differs"
-        moved += int(r["iter"].sum())
-    assert moved > 0
-
-
 def test_precompute_port_close_to_reference():
+    """The restated precompute vs the cache the reference's tiny_setup derived (stored with the golden cases)."""
+    cases = H.make_cases()
     for name in ("cartpole_f64", "quad_hover_N10_f64", "rocket_soc_N10_f64", "lti_8_2_f64"):
-        c = CASES[name]
-        if not oracle.ref_available(np.float64):
-            pytest.skip("oracle/_ref not built")
-        pr = H.problem_from_spec(c["spec"], np.float64, oracle.ref_setup)
-        pp = H.problem_from_spec(c["spec"], np.float64, oracle.port_setup)
+        pr = H.load_golden(name)[0]
+        pp = H.problem_from_spec(cases[name]["spec"], np.float64, oracle.port_setup)
         for f in ("Kinf", "Pinf", "Quu_inv", "AmBKt", "APf", "BPf", "Q", "R"):
             a, b = getattr(pr, f), getattr(pp, f)
             assert np.allclose(a, b, rtol=1e-9, atol=1e-9 * max(1.0, np.abs(a).max())), (name, f)
@@ -49,22 +31,15 @@ def test_precompute_port_close_to_reference():
 @pytest.mark.parametrize("dt", [np.float32, np.float64])
 def test_port_bit_identical_to_reference_random_lti_sweep(dt):
     """Randomised sweep over the compiled (nx, nu) pairs and short horizons (BASELINE config 5's generator): warm-started
-    three-step loops with active box bounds, restatement vs the unmodified reference, bit for bit."""
-    from tinympc_b200 import workloads as wl
-
-    if not oracle.ref_available(dt):
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
-    dims = [(4, 1), (4, 2), (4, 8), (6, 3), (8, 4), (12, 2), (12, 8), (16, 4), (16, 8)]
-    for n, (nx, nu) in enumerate(dims):
-        N = (3, 7, 12)[n % 3]
-        sp = wl.random_lti(nx, nu, N, seed=40 + n)
-        sp.settings.max_iter = 25
-        sp.settings.check_termination = 1 + n % 3
-        inst = wl.random_instances(5, nx, N, seed=70 + n, dtype=dt)
-        inst["x0"] = (3.0 * inst["x0"]).astype(dt)  # push the rollout into the bounds
-        prob = H.problem_from_spec(sp, dt, oracle.ref_setup)
-        ref, x0s = H.closed_loop(prob, sp.settings, inst, 3, False, H.BOX_STATE, _solve("reference"))
-        port, _ = H.closed_loop(prob, sp.settings, inst, 3, False, H.BOX_STATE, _solve("port"), x0_seq=x0s)
-        for k, (r, p) in enumerate(zip(ref, port)):
-            for key in H.OUT_KEYS + H.BOX_STATE:
-                assert H.bits_equal(r[key], p[key]), f"({nx},{nu},{N}) step {k}: {key} differs"
+    three-step loops with active box bounds, restatement vs the unmodified reference (its cache, measured states and the
+    digest of every output array stored in tests/golden/reference), bit for bit."""
+    tag = "f32" if dt == np.float32 else "f64"
+    d = np.load(os.path.join(H.REFERENCE_DIR, f"lti_sweep_{tag}.npz"))
+    for n, (nx, nu, N, sp, inst) in enumerate(H.lti_sweep_cases(dt)):
+        prob = H.problem_from_spec(sp, dt, oracle.port_setup)
+        for f in H.CACHE_FIELDS:
+            setattr(prob, f, d[f"d{n}_{f}"])
+        port, _ = H.closed_loop(prob, sp.settings, inst, 3, False, H.BOX_STATE, _solve("port"), x0_seq=d[f"d{n}_x0_seq"])
+        for k, p in enumerate(port):
+            for key, want in zip(H.OUT_KEYS + H.BOX_STATE, d[f"d{n}_digests"][k]):
+                assert H.digest(p[key]) == str(want), f"({nx},{nu},{N}) step {k}: {key} differs"

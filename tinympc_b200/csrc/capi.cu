@@ -188,8 +188,7 @@ int check_ready(const tinympc_b200_solver *s) {
     return 0;
 }
 
-// Which kernel family serves a solve.  GPI = lane groups, state on chip (box constraints, horizon fits in shared + tensor
-// memory); GPS = lane groups, state streamed (everything else the lane mapping covers); TPI = one thread per instance.
+// Which kernel family serves a solve.  GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane mapping covers); TPI = one thread per instance.
 // `smem_out`: shared-memory bytes of the on-chip plan (0 = not available).  Returns -1 when an explicit request cannot
 // be honoured.
 int resolve_family(const tinympc_b200_solver *s, const Features &ft, int *smem_out, int64_t B = 0) {
@@ -204,34 +203,26 @@ int resolve_family(const tinympc_b200_solver *s, const Features &ft, int *smem_o
     if (s->family == TINYMPC_KERNEL_GPI) return gpi_ok ? TINYMPC_KERNEL_GPI : (gps_ok ? TINYMPC_KERNEL_GPS : -1);
     if (s->family == TINYMPC_KERNEL_GPS) return gps_ok ? TINYMPC_KERNEL_GPS : -1;
     if (s->family == TINYMPC_KERNEL_TPI) return TINYMPC_KERNEL_TPI;
-    // AUTO (measured rules; evidence: profiles/r02_auto_rule_sweep.md, profiles/r01_sweep_1gpu.md)
-    const int gps_plan = gps_ok ? s->dim->gps_lanes(s->dtype) : 0;
-    const bool gps_two = ((gps_plan >> 8) & 0xff) == 2;  // two instances per lane group: the small shapes
+    // AUTO (measured rules; evidence: tools/auto_rule_sweep.py, DESIGN.md §5)
     const bool big_batch = B >= (int64_t)s->sm_count * 384;  // one thread per instance fills the GPU
-    // cones / hyperplanes: streamed lane groups (rocket landing, fp64: 3.3x the thread-per-instance kernel)
+    // cones / hyperplanes: streamed lane groups
     if (ft.ext) return gps_ok ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI;
-    // box constraints, streamed alternative when the state does not stay on chip: for big batches the streamed lane groups
-    // beat one thread per instance on the small fp64 shapes ((6,3,100): 28.1 vs 36.7 ms, (4,2,50): 9.1 vs 11.6 ms) and lose
-    // on the wide ones ((12,4,50) fp64: 61.6 vs 35.8 ms; fp32 N = 100: 41-113 vs 36-71 ms); small batches cannot fill the
-    // GPU with one thread per instance
-    const int streamed = !gps_ok ? TINYMPC_KERNEL_TPI
-                                 : ((!big_batch || (s->dtype == TINYMPC_F64 && gps_two)) ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI);
+    // box constraints, streamed alternative when the state does not stay on chip: one thread per instance for big batches
+    // (it beats the streamed lane groups on every measured shape, fp64 (6,3,100) included: 60.0 vs 63.9 ms); small batches
+    // cannot fill the GPU with one thread per instance
+    const int streamed = (gps_ok && !big_batch) ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI;
     if (!gpi_ok) return streamed;
-    // fp32: on chip (GPI) unless shared + tensor memory hold fewer than 32 instances per SM (long horizons with wide inputs)
-    // AND the batch is large.  Measured on B200 (B = 131 072, N = 100): at 16 instances/SM the streamed kernels win by 10-35 %
-    // for every shape except (16,8), where the thread-per-instance register footprint costs more than the low on-chip
-    // occupancy; at >= 32 instances/SM GPI always wins.
+    // Big batches leave the chip when shared memory holds too few instances per SM, except for (16,8), where the
+    // thread-per-instance register footprint costs more than the low on-chip occupancy.  Measured on H100 (B = 131 072 fp32 /
+    // 65 536 fp64, 50 iterations): fp32 on chip wins from 16 instances per SM on ((12,8,50): 45 vs 69 ms thread per instance;
+    // (12,4,100): 85 vs 94 ms) and loses at 8 ((4,8,100): 128 vs 78 ms); fp64 (rows re-read per sweep) on chip wins with three
+    // warps per SM ((4,2,50): 13 vs 19 ms; (16,8,50): 80 vs 197 ms) unless they hold only 6 instances ((12,4,50): 73 vs 60 ms),
+    // and loses badly with one warp ((6,3,100): 143 vs 60 ms thread per instance).
     const int plan = s->dim->gpi_instances_per_cta ? s->dim->gpi_instances_per_cta(s->dtype, s->N, s->max_smem_optin) : 0;
     const int ipc = plan & 0xffff, gpi_warps = plan >> 16;
-    if (s->dtype == TINYMPC_F64) {
-        // fp64 (rows re-read per sweep, duals in tensor memory): on chip wins as soon as four warps per SM are resident
-        // ((12,4,50): 29.6 vs 35.9 ms TPI at 16 instances/SM; (16,8,50): 57.3 vs 88.4 ms at 8/SM), and loses badly with one
-        // warp per SM ((6,3,100): 83 vs 28.4 ms on the streamed lane groups)
-        if (gpi_warps > 0 && gpi_warps < 4 && big_batch) return streamed;
-        return TINYMPC_KERNEL_GPI;
-    }
     const bool tpi_heavy = s->nx >= 16 && s->nu >= 8;
-    if (ipc > 0 && ipc < 32 && !tpi_heavy && big_batch) return streamed;
+    const bool few = s->dtype == TINYMPC_F64 ? (gpi_warps < 2 || ipc < 8) : ipc < 16;
+    if (ipc > 0 && few && !tpi_heavy && big_batch) return streamed;
     return TINYMPC_KERNEL_GPI;
 }
 
@@ -335,7 +326,7 @@ int64_t tpi_chunk_instances(const tinympc_b200_solver *s, const Features &ft, in
         if (v < 0) return B;  // chunking off
     }
     (void)ft;
-    return B;  // measured on B200 (profiles/r01_tpi_chunk_sweep.txt): sub-batching only lowers occupancy; TPI is latency-, not L2-, limited
+    return B;  // sub-batching only lowers occupancy: TPI is latency-, not L2-, limited
 }
 
 // enqueue one batched solve on `stream` (device pointers); fills stats
@@ -411,7 +402,6 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     s->stats.instances_per_cta = d.out_instances_per_cta;
     s->stats.smem_bytes_per_cta = d.out_smem;
     s->stats.threads_per_cta = d.out_threads;
-    s->stats.tmem_cols_per_cta = d.out_tmem_cols;
     if (timed) CUDA_TRY(cudaEventRecord(s->ev1, stream));
     CUDA_TRY(cudaEventRecord(s->ev_last, stream));
     s->last_stream = stream;
@@ -475,7 +465,7 @@ int precompute_batch_T(int nx, int nu, int64_t B, const T *A, const T *Bm, const
 extern "C" {
 
 const char *tinympc_b200_last_error(void) { return g_err.c_str(); }
-const char *tinympc_b200_version(void) { return "tinympc_b200 0.1 (sm_100a)"; }
+const char *tinympc_b200_version(void) { return "tinympc_b200 0.1 (sm_90a)"; }
 
 int tinympc_b200_supported(int32_t dtype, int32_t nx, int32_t nu) {
     return (dtype == TINYMPC_F32 || dtype == TINYMPC_F64) && find_dim(nx, nu) != nullptr;
@@ -581,7 +571,7 @@ int tinympc_b200_create(const tinympc_problem_t *p, int32_t device, tinympc_b200
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(TINYMPC_ERR_UNSUPPORTED, "this library is built for sm_100a (B200) only");
+    if (prop.major != 9 || prop.minor != 0) return fail(TINYMPC_ERR_UNSUPPORTED, "this library is built for sm_90a (H100) only");
 
     tinympc_b200_solver *s = new tinympc_b200_solver();
     s->device = device;

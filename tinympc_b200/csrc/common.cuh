@@ -28,93 +28,25 @@ __device__ __forceinline__ T nmac(T acc, T a, T b) {  // acc - a*b
     }
 }
 // ---- several ascending-k dot products against the same vector -------------------------------------------------
-// out[r] = M[r][0]*v[0]; out[r] = out[r] + M[r][k]*v[k]   (k ascending; STRICT: separate multiply and add).
-// fp32: rows are processed in pairs with PACKED adds (add.rn.f32x2 -> FADD2: two IEEE fp32 additions per issued
-// instruction, bit-identical to two FADDs) while the multiplies stay scalar FMULs, so ptxas cannot contract them
-// into FFMA2 (it fuses mul.f32x2+add.f32x2 even under -fmad=false, see profiles/r01_f32x2_microbench.txt).
-// FAST fp32 uses fma.rn.f32x2 (FFMA2).  fp64 has no packed form.
-__device__ __forceinline__ unsigned long long pack2(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void unpack2(unsigned long long v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ unsigned long long add2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ unsigned long long fma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-
-__device__ __forceinline__ unsigned long long sub2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-// element-wise o = a + b / o = a - b on short vectors.  fp32, even length: packed FADD2 (two IEEE additions per issued
-// instruction, bit-identical to two FADDs); anything else: scalar.
+// out[r] = M[r][0]*v[0]; out[r] = out[r] + M[r][k]*v[k]   (k ascending; STRICT: separate multiply and add, never
+// contracted under -fmad=false; FAST: fma with the same order of terms).
+// element-wise o = a + b / o = a - b on short vectors
 template <typename T, int NV>
 __device__ __forceinline__ void vadd(const T (&a)[NV], const T (&b)[NV], T (&o)[NV]) {
-    constexpr int NP = (sizeof(T) == 4) ? NV / 2 * 2 : 0;  // elements handled as packed pairs
-    if constexpr (sizeof(T) == 4) {
 #pragma unroll
-        for (int e = 0; e < NP; e += 2) {
-            float lo, hi;
-            unpack2(add2(pack2((float)a[e], (float)a[e + 1]), pack2((float)b[e], (float)b[e + 1])), lo, hi);
-            o[e] = lo;
-            o[e + 1] = hi;
-        }
-    }
-#pragma unroll
-    for (int e = NP; e < NV; ++e) o[e] = a[e] + b[e];
+    for (int e = 0; e < NV; ++e) o[e] = a[e] + b[e];
 }
 template <typename T, int NV>
 __device__ __forceinline__ void vsub(const T (&a)[NV], const T (&b)[NV], T (&o)[NV]) {
-    constexpr int NP = (sizeof(T) == 4) ? NV / 2 * 2 : 0;
-    if constexpr (sizeof(T) == 4) {
 #pragma unroll
-        for (int e = 0; e < NP; e += 2) {
-            float lo, hi;
-            unpack2(sub2(pack2((float)a[e], (float)a[e + 1]), pack2((float)b[e], (float)b[e + 1])), lo, hi);
-            o[e] = lo;
-            o[e + 1] = hi;
-        }
-    }
-#pragma unroll
-    for (int e = NP; e < NV; ++e) o[e] = a[e] - b[e];
+    for (int e = 0; e < NV; ++e) o[e] = a[e] - b[e];
 }
 
-template <bool FAST, int NR, int NE>
-__device__ __forceinline__ void dots(const float (&M)[NR][NE], const float (&v)[NE], float (&out)[NR]) {
-#pragma unroll
-    for (int r = 0; r + 1 < NR; r += 2) {
-        unsigned long long acc = pack2(M[r][0] * v[0], M[r + 1][0] * v[0]);
-#pragma unroll
-        for (int k = 1; k < NE; ++k) {
-            if constexpr (FAST) {
-                acc = fma2(pack2(M[r][k], M[r + 1][k]), pack2(v[k], v[k]), acc);
-            } else {
-                acc = add2(acc, pack2(M[r][k] * v[k], M[r + 1][k] * v[k]));
-            }
-        }
-        unpack2(acc, out[r], out[r + 1]);
-    }
-    if constexpr (NR % 2 == 1) {
-        float s = M[NR - 1][0] * v[0];
-#pragma unroll
-        for (int k = 1; k < NE; ++k) s = mac<FAST>(s, M[NR - 1][k], v[k]);
-        out[NR - 1] = s;
-    }
-}
-template <bool FAST, int NR, int NE>
-__device__ __forceinline__ void dots(const double (&M)[NR][NE], const double (&v)[NE], double (&out)[NR]) {
+template <bool FAST, int NR, int NE, typename T>
+__device__ __forceinline__ void dots(const T (&M)[NR][NE], const T (&v)[NE], T (&out)[NR]) {
 #pragma unroll
     for (int r = 0; r < NR; ++r) {
-        double s = M[r][0] * v[0];
+        T s = M[r][0] * v[0];
 #pragma unroll
         for (int k = 1; k < NE; ++k) s = mac<FAST>(s, M[r][k], v[k]);
         out[r] = s;
@@ -122,33 +54,11 @@ __device__ __forceinline__ void dots(const double (&M)[NR][NE], const double (&v
 }
 
 // same, with the coefficients supplied by a callable coef(r, k) (e.g. constant-bank matrix entries in the TPI kernel)
-template <bool FAST, int NR, int NE, typename F>
-__device__ __forceinline__ void dots_f(F coef, const float (&v)[NE], float (&out)[NR]) {
-#pragma unroll
-    for (int r = 0; r + 1 < NR; r += 2) {
-        unsigned long long acc = pack2(coef(r, 0) * v[0], coef(r + 1, 0) * v[0]);
-#pragma unroll
-        for (int k = 1; k < NE; ++k) {
-            if constexpr (FAST) {
-                acc = fma2(pack2(coef(r, k), coef(r + 1, k)), pack2(v[k], v[k]), acc);
-            } else {
-                acc = add2(acc, pack2(coef(r, k) * v[k], coef(r + 1, k) * v[k]));
-            }
-        }
-        unpack2(acc, out[r], out[r + 1]);
-    }
-    if constexpr (NR % 2 == 1) {
-        float s = coef(NR - 1, 0) * v[0];
-#pragma unroll
-        for (int k = 1; k < NE; ++k) s = mac<FAST>(s, coef(NR - 1, k), v[k]);
-        out[NR - 1] = s;
-    }
-}
-template <bool FAST, int NR, int NE, typename F>
-__device__ __forceinline__ void dots_f(F coef, const double (&v)[NE], double (&out)[NR]) {
+template <bool FAST, int NR, int NE, typename F, typename T>
+__device__ __forceinline__ void dots_f(F coef, const T (&v)[NE], T (&out)[NR]) {
 #pragma unroll
     for (int r = 0; r < NR; ++r) {
-        double s = coef(r, 0) * v[0];
+        T s = coef(r, 0) * v[0];
 #pragma unroll
         for (int k = 1; k < NE; ++k) s = mac<FAST>(s, coef(r, k), v[k]);
         out[r] = s;

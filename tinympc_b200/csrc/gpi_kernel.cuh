@@ -8,11 +8,9 @@
 //     mat-vec is RX (or RU) independent ascending-k dot products per lane (bit-identical to the pinned
 //     oracle in STRICT mode), and the freshly computed vector is all-gathered inside the lane group through
 //     a small shared-memory buffer (STS + 16-byte broadcast LDS);
-//   * the N-indexed state lives on chip for the whole solve: the primal pack (vnew rows, znew rows) as one
-//     16-byte vector per lane and knot point in shared memory; the dual pack (g rows, y rows) and d either next
-//     to it in shared memory, or (TM = true) in TENSOR MEMORY — the thread's own 32-bit TMEM columns, 5 per knot point in
-//     fp32 (two per fp64 value), tcgen05.ld/st.32x32b — which halves the shared-memory footprint and doubles the instances
-//     (= warps) resident per SM; only the final trajectories / residuals are written back;
+//   * the N-indexed state lives in shared memory for the whole solve: the primal pack (vnew rows, znew rows) and the
+//     dual pack (g rows, y rows) as one 16-byte vector per lane and knot point each, and d; only the final
+//     trajectories / residuals are written back;
 //   * fp64: only the rows of the running sweep are in registers (re-read from the resident blob at every sweep start), so
 //     that narrower lane groups fit (gpi_per_sweep_rows);
 //   * the kernel is persistent: one CTA per SM; every lane group ("slot") pulls its next instance from a
@@ -38,24 +36,17 @@ struct GpiCfg {
     static constexpr int NPV = PVP / W;     // vectors per pack
     static constexpr int NXP = (L * RX + W - 1) / W * W;  // gather buffer width (state vectors)
     static constexpr int NUP = (L * RU + W - 1) / W * W;  // gather buffer width (input vectors)
-    static constexpr int GBUF1 = IPW * (NXP > NUP ? NXP : NUP);  // one gather buffer
-    static constexpr int GBUF = 3 * GBUF1;  // tensor-memory variant: three of them, each hot call site owns one (see gather_x)
+    static constexpr int GBUF1 = IPW * (NXP > NUP ? NXP : NUP);  // the gather buffer
     // registers needed for the per-lane matrix rows (in elements of T)
     static constexpr int MAT_REGS = RX * (2 * NX + 2 * NU + 3) + RU * (2 * NX + NU + 2);
     // shared-memory elements per warp for horizon N: primal pack + dual pack per (k, lane), d, gather scratch
     __host__ __device__ static constexpr size_t warp_elems(int N) {
-        return (size_t)N * 32 * PVP * 2 + (size_t)(N - 1) * RU * 32 + GBUF1;  // shared memory is the constraint here: one gather buffer
+        return (size_t)N * 32 * PVP * 2 + (size_t)(N - 1) * RU * 32 + GBUF1;
     }
     // per-sweep register needs (elements): backward AmBKt / B^T rows, Kinf^T, Quu_inv, APf, BPf, Qd, Rd; forward A / Kinf rows, B, f
     static constexpr int BWD_REGS = (RX + RU) * NX + RX * NU + RU * NU + 2 * RX + 2 * RU;
     static constexpr int FWD_REGS = (RX + RU) * NX + RX * NU + RX;
     static constexpr int SWEEP_REGS = BWD_REGS > FWD_REGS ? BWD_REGS : FWD_REGS;
-    // TMEM variant: the dual pack and d live in tensor memory, CPK 32-bit columns per knot point (two per fp64 value) in
-    // the lane of the owning thread; shared memory keeps the primal pack and the gather scratch
-    static constexpr int CW = ES / 4;  // 32-bit columns per value
-    static constexpr int CPK = (PVP + RU) * CW;
-    __host__ __device__ static constexpr size_t warp_elems_tm(int N) { return (size_t)N * 32 * PVP + GBUF; }
-    __host__ __device__ static constexpr int tm_cols(int N) { return N * CPK; }
 };
 
 // fp64: only the rows of the RUNNING sweep are in registers (re-read from the staged blob in shared memory - or from the
@@ -112,56 +103,6 @@ __device__ __forceinline__ void stsv(unsigned a, const double (&v)[2]) {
     asm volatile("st.shared.v2.f64 [%0], {%1,%2};" ::"r"(a), "d"(v[0]), "d"(v[1]) : "memory");
 }
 
-// Tensor memory (TMEM, 128 lanes x 512 32-bit columns per SM) used as a per-thread scratchpad: warp w of a CTA owns
-// TMEM lanes [32*(w%4), +32), thread t of the warp lane 32*(w%4)+t.  `32x32b` moves n consecutive columns of the
-// thread's own lane to / from n registers.  Loads are asynchronous: tm_wait_ld() + tm_tie() before the first use.
-__device__ __forceinline__ void tm_ld(unsigned ta, float (&v)[1]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=f"(v[0]) : "r"(ta));
-}
-__device__ __forceinline__ void tm_ld(unsigned ta, float (&v)[2]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=f"(v[0]), "=f"(v[1]) : "r"(ta));
-}
-__device__ __forceinline__ void tm_ld(unsigned ta, float (&v)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(ta));
-}
-__device__ __forceinline__ void tm_st(unsigned ta, const float (&v)[1]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(ta), "f"(v[0]) : "memory");
-}
-__device__ __forceinline__ void tm_st(unsigned ta, const float (&v)[2]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1,%2};" ::"r"(ta), "f"(v[0]), "f"(v[1]) : "memory");
-}
-__device__ __forceinline__ void tm_st(unsigned ta, const float (&v)[4]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(ta), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
-}
-__device__ __forceinline__ void tm_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tm_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// makes every later use of v depend on an asm statement that is ordered after tm_wait_ld()
-__device__ __forceinline__ void tm_tie(float &v) { asm volatile("" : "+f"(v)); }
-// fp64 values occupy two consecutive 32-bit columns (low word first)
-__device__ __forceinline__ void tm_tie(double &v) { asm volatile("" : "+d"(v)); }
-__device__ __forceinline__ void tm_ld(unsigned ta, double (&v)[1]) {
-    unsigned lo, hi;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0,%1}, [%2];" : "=r"(lo), "=r"(hi) : "r"(ta));
-    asm volatile("mov.b64 %0, {%1,%2};" : "=d"(v[0]) : "r"(lo), "r"(hi));
-}
-__device__ __forceinline__ void tm_ld(unsigned ta, double (&v)[2]) {
-    unsigned w0, w1, w2, w3;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w0), "=r"(w1), "=r"(w2), "=r"(w3) : "r"(ta));
-    asm volatile("mov.b64 %0, {%1,%2};" : "=d"(v[0]) : "r"(w0), "r"(w1));
-    asm volatile("mov.b64 %0, {%1,%2};" : "=d"(v[1]) : "r"(w2), "r"(w3));
-}
-__device__ __forceinline__ void tm_st(unsigned ta, const double (&v)[1]) {
-    unsigned lo, hi;
-    asm volatile("mov.b64 {%0,%1}, %2;" : "=r"(lo), "=r"(hi) : "d"(v[0]));
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1,%2};" ::"r"(ta), "r"(lo), "r"(hi) : "memory");
-}
-__device__ __forceinline__ void tm_st(unsigned ta, const double (&v)[2]) {
-    unsigned w0, w1, w2, w3;
-    asm volatile("mov.b64 {%0,%1}, %2;" : "=r"(w0), "=r"(w1) : "d"(v[0]));
-    asm volatile("mov.b64 {%0,%1}, %2;" : "=r"(w2), "=r"(w3) : "d"(v[1]));
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(ta), "r"(w0), "r"(w1), "r"(w2), "r"(w3) : "memory");
-}
-
 template <bool B>
 struct BoolTag {
     static constexpr bool value = B;
@@ -192,13 +133,12 @@ __device__ __forceinline__ double absmax(double m, double d) {
 
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
-template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool TM, bool MM = false>
+template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool MM = false>
 __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     gpi_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
     using Cfg = GpiCfg<NX, NU, L, (int)sizeof(T)>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, PVP = Cfg::PVP, NPV = Cfg::NPV;
-    constexpr int NXP = Cfg::NXP, NUP = Cfg::NUP, CPK = Cfg::CPK;
-    constexpr int CW = Cfg::CW;        // 32-bit tensor-memory columns per value
+    constexpr int NXP = Cfg::NXP, NUP = Cfg::NUP;
     constexpr bool PS = gpi_per_sweep_rows<T>();  // matrix rows re-read at every sweep start (fp64)
     constexpr bool EXACT = (RX * L == NX) && (RU * L == NU);  // no padding rows: predicates vanish
     constexpr unsigned ES = (unsigned)sizeof(T);
@@ -335,34 +275,18 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // where this lane's rows come from at a sweep start (PS): the staged blob, or its slot's own blob (heterogeneous batch)
     const T *rowsrc = stage;
     if constexpr (!PS) load_rows(stage);
-    // TMEM variant: warp 0 allocates all 512 columns (one CTA per SM); warps w and w+4 share a lane quarter and
-    // take the column ranges [0, N*CPK) and [N*CPK, 2*N*CPK)
-    unsigned tbase = 0;
-    __shared__ unsigned tmem_addr_slot;
-    if constexpr (TM) {
-        if (warp == 0) {
-            asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"((unsigned)__cvta_generic_to_shared(&tmem_addr_slot)) : "memory");
-            asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    }
     __syncthreads();  // staging area is reused as state below
-    if constexpr (TM) {
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        tbase = tmem_addr_slot + ((unsigned)((warp & 3) * 32) << 16) + (unsigned)((warp >> 2) * N * CPK);
-    }
 
     // ---- shared-memory state of this warp ----
     //   PA[k][lane][PVP] : primal pack  (vnew rows of this lane, then znew rows)      16-byte vectors,
     //   PB[k][lane][PVP] : dual pack    (g rows, then y rows)                          conflict free
     //   D [k][b][lane]   : d
     //   GB[...]          : gather scratch (one vector of one instance per row)
-    //   TMEM variant: PB and D live in tensor memory instead, columns [k*CPK, +PVP) and [k*CPK+PVP, +RU) of the thread's lane
-    const int warp_elems = TM ? (int)Cfg::warp_elems_tm(N) : (int)Cfg::warp_elems(N);
+    const int warp_elems = (int)Cfg::warp_elems(N);
     // fp64 (PS): the staged blob stays in shared memory for the whole kernel, the state regions start behind it
     constexpr size_t BLOB_KEEP = PS ? (size_t)BLOB_BYTES : 0;
     T *wbase = reinterpret_cast<T *>(smem_raw + BLOB_KEEP) + (size_t)warp * warp_elems;
-    T *gPA = wbase, *gPB = gPA + N * 32 * PVP, *gD = gPB + N * 32 * PVP, *gGB = TM ? gPA + N * 32 * PVP : gD + (N - 1) * RU * 32;
+    T *gPA = wbase, *gPB = gPA + N * 32 * PVP, *gD = gPB + N * 32 * PVP, *gGB = gD + (N - 1) * RU * 32;
     const unsigned aPA = (unsigned)__cvta_generic_to_shared(gPA) + (unsigned)(lane * PVP) * ES;
     const unsigned aPB = (unsigned)__cvta_generic_to_shared(gPB) + (unsigned)(lane * PVP) * ES;
     const unsigned aD = (unsigned)__cvta_generic_to_shared(gD) + (unsigned)lane * ES;
@@ -387,104 +311,44 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             stsv(base + (unsigned)k * KSTR + (unsigned)(c * W) * ES, t);
         }
     };
-    // dual pack / d accessors.  TMEM loads are asynchronous: `pb_ready` / `d_ready` must run before the first use.
-    auto load_pb = [&](int k, T (&v)[PVP]) {
-        if constexpr (TM) {
-#pragma unroll
-            for (int c = 0; c < NPV; ++c) {
-                T t[W];
-                tm_ld(tbase + (unsigned)(k * CPK + c * W * CW), t);
-#pragma unroll
-                for (int e = 0; e < W; ++e) v[c * W + e] = t[e];
-            }
-        } else {
-            load_pack(aPB, k, v);
-        }
-    };
-    auto pb_ready = [&](T (&v)[PVP]) {
-        if constexpr (TM) {
-            tm_wait_ld();
-#pragma unroll
-            for (int e = 0; e < PVP; ++e) tm_tie(v[e]);
-        }
-    };
-    auto store_pb = [&](int k, const T (&v)[PVP]) {  // TMEM: warp-wide, unconditional
-        if constexpr (TM) {
-#pragma unroll
-            for (int c = 0; c < NPV; ++c) {
-                T t[W];
-#pragma unroll
-                for (int e = 0; e < W; ++e) t[e] = v[c * W + e];
-                tm_st(tbase + (unsigned)(k * CPK + c * W * CW), t);
-            }
-        } else {
-            store_pack(aPB, k, v);
-        }
-    };
+    // dual pack / d accessors
+    auto load_pb = [&](int k, T (&v)[PVP]) { load_pack(aPB, k, v); };
+    auto store_pb = [&](int k, const T (&v)[PVP]) { store_pack(aPB, k, v); };
     auto load_d = [&](int k, T (&d)[RU]) {
-        if constexpr (TM) {
 #pragma unroll
-            for (int b = 0; b < RU; ++b) {
-                T t[1];
-                tm_ld(tbase + (unsigned)(k * CPK + (PVP + b) * CW), t);
-                d[b] = t[0];
-            }
-        } else {
-#pragma unroll
-            for (int b = 0; b < RU; ++b) d[b] = lds(aD + (unsigned)k * DSTR + (unsigned)(b * 32) * ES, T());
-        }
-    };
-    auto d_ready = [&](T (&d)[RU]) {
-        if constexpr (TM) {
-            tm_wait_ld();
-#pragma unroll
-            for (int b = 0; b < RU; ++b) tm_tie(d[b]);
-        }
+        for (int b = 0; b < RU; ++b) d[b] = lds(aD + (unsigned)k * DSTR + (unsigned)(b * 32) * ES, T());
     };
     auto store_d = [&](int k, const T (&d)[RU], const bool live) {
-        if constexpr (TM) {
 #pragma unroll
-            for (int b = 0; b < RU; ++b) {
-                T t[1] = {d[b]};
-                tm_st(tbase + (unsigned)(k * CPK + (PVP + b) * CW), t);
-            }
-        } else {
-#pragma unroll
-            for (int b = 0; b < RU; ++b)
-                if (live && uv[b]) sts(aD + (unsigned)k * DSTR + (unsigned)(b * 32) * ES, d[b]);
-        }
+        for (int b = 0; b < RU; ++b)
+            if (live && uv[b]) sts(aD + (unsigned)k * DSTR + (unsigned)(b * 32) * ES, d[b]);
     };
     // all-gather inside the lane group through shared memory: every lane stores its R values, then reads the
     // whole vector with 16-byte broadcast loads (absolute row order -> ascending-k dot products as in the oracle).
-    // There are three gather buffers; every call site of the sweeps owns one (BUF) such that two consecutive uses of a
-    // buffer always have another gather's barrier between them: the barrier that would protect the buffer's previous
-    // readers before it is overwritten (LEAD) is then unnecessary, one __syncwarp per gather instead of two.
-    // (the all-shared-memory variant has no room for three buffers in its fourth warp: one buffer, both barriers)
-    constexpr bool G3 = TM;
-    constexpr unsigned GB0 = 0u, GB1 = G3 ? (unsigned)Cfg::GBUF1 * ES : 0u, GB2 = G3 ? 2u * (unsigned)Cfg::GBUF1 * ES : 0u;
-    auto gather_x = [&](const unsigned bo, const bool LEAD, const T (&own)[RX], T (&full)[NX]) {  // always inlined with literals
-        if (LEAD || !G3) __syncwarp();
+    // One buffer: the leading barrier protects the previous gather's readers before it is overwritten.
+    auto gather_x = [&](const T (&own)[RX], T (&full)[NX]) {
+        __syncwarp();
 #pragma unroll
-        for (int a = 0; a < RX; ++a) sts(aGB + bo + (unsigned)(slot * NXP + l * RX + a) * ES, own[a]);
+        for (int a = 0; a < RX; ++a) sts(aGB + (unsigned)(slot * NXP + l * RX + a) * ES, own[a]);
         __syncwarp();
 #pragma unroll
         for (int c = 0; c < NXP / W; ++c) {
             T t[W];
-            ldsv(aGB + bo + (unsigned)(slot * NXP + c * W) * ES, t);
+            ldsv(aGB + (unsigned)(slot * NXP + c * W) * ES, t);
 #pragma unroll
             for (int e = 0; e < W; ++e)
                 if (c * W + e < NX) full[c * W + e] = t[e];
         }
     };
-    auto gather_u = [&](const unsigned bo, const bool LEAD, const T (&own)[RU], T (&full)[NU]) {
-        if (LEAD || !G3) __syncwarp();
+    auto gather_u = [&](const T (&own)[RU], T (&full)[NU]) {
+        __syncwarp();
 #pragma unroll
-        for (int b = 0; b < RU; ++b) sts(aGB + bo + (unsigned)(slot * NUP + l * RU + b) * ES, own[b]);
+        for (int b = 0; b < RU; ++b) sts(aGB + (unsigned)(slot * NUP + l * RU + b) * ES, own[b]);
         __syncwarp();
 #pragma unroll
         for (int c = 0; c < NUP / W; ++c) {
             T t[W];
-            ldsv(aGB + bo + (unsigned)(slot * NUP + c * W) * ES, t);
+            ldsv(aGB + (unsigned)(slot * NUP + c * W) * ES, t);
 #pragma unroll
             for (int e = 0; e < W; ++e)
                 if (c * W + e < NU) full[c * W + e] = t[e];
@@ -575,7 +439,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         T xo[RX], Xf[NX];
 #pragma unroll
         for (int a = 0; a < RX; ++a) xo[a] = x0o[a];
-        gather_x(GB1, false, xo, Xf);
+        gather_x(xo, Xf);
         // one column: slack + dual update of this lane's rows, residual maxima; HASU = the column has inputs
         auto column = [&](int k, const bool HASU, const T (&u)[RU], const T (&vprev)[PVP], const T (&pb)[PVP]) {  // always inlined with a literal HASU
             T pa[PVP], na[PVP], nb[PVP];
@@ -675,10 +539,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     }
                 }
             }
-            if constexpr (TM) store_pb(k, nb);  // (a slot that is not busy holds no live state)
             if (busy) {
                 store_pack(aPA, k, na);
-                if constexpr (!TM) store_pb(k, nb);
+                store_pb(k, nb);
                 if constexpr (SLOW) {
                     // work->v / work->z of this iteration = the primal pack as it was before this column's update
                     // (kept in pack layout in global scratch: one 16-byte store; transposed out only if the solve converges)
@@ -720,11 +583,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             load_pb(k, pbk);
             load_d(k, dk);
             dots<FAST>(mS1f, Xf, t1);  // [A x_k ; Kinf x_k]
-            d_ready(dk);
-            pb_ready(pbk);
 #pragma unroll
             for (int b = 0; b < RU; ++b) u[b] = (-t1[RX + b]) - dk[b];  // u_k = -(Kinf x_k) - d_k
-            gather_u(GB0, false, u, Uf);
+            gather_u(u, Uf);
             column(k, true, u, vprev, pbk);
             dots<FAST>(mB, Uf, bu);
             {   // x_{k+1} = (A x_k + B u_k) + f
@@ -734,7 +595,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 vadd<T, RX>(ax, bu, tx);
                 vadd<T, RX>(tx, vf, xo);
             }
-            gather_x(GB1, false, xo, Xf);
+            gather_x(xo, Xf);
         }
         {
             T udummy[RU], vprev[PVP], pbk[PVP];
@@ -742,9 +603,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             for (int b = 0; b < RU; ++b) udummy[b] = T(0);
             load_vprev(N - 1, vprev);
             load_pb(N - 1, pbk);
-            pb_ready(pbk);
             column(N - 1, false, udummy, vprev, pbk);
-            if constexpr (TM) tm_wait_st();  // the dual packs are read back by the next backward pass / the write-back
         }
     };
 
@@ -761,47 +620,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             for (int e = lane; e < N * VPK; e += 32) {
                 const int k = e / VPK, w = e - k * VPK;
                 a4[k * ROW4 + s * VPK + w] = z4;
-                if constexpr (!TM) b4[k * ROW4 + s * VPK + w] = z4;
+                b4[k * ROW4 + s * VPK + w] = z4;
             }
         }
         __syncwarp();
-        if constexpr (TM) {
-            // the dual packs live in the lanes' own TMEM columns and TMEM stores are warp-wide: read-modify-write every
-            // knot point, replacing the values of slot s's lanes by zeros (cold) or the caller's g / y rows (warm start);
-            // the global loads of UNR knot points are issued together, ahead of the dependent TMEM traffic
-            const int64_t ox = ib * (int64_t)N * NX, ou = ib * (int64_t)(N - 1) * NU;
-            const bool mine = slot == s;
-            constexpr int UNR = 5;
-            for (int k0 = 0; k0 < N; k0 += UNR) {
-                T nv[UNR][PVP];
-#pragma unroll
-                for (int t = 0; t < UNR; ++t) {
-                    const int k = k0 + t;
-#pragma unroll
-                    for (int e = 0; e < PVP; ++e) nv[t][e] = T(0);
-#pragma unroll
-                    for (int a = 0; a < RX; ++a)
-                        nv[t][a] = (!cold && mine && k < N && xv[a] && P.s_g) ? P.s_g[ox + (int64_t)k * NX + l * RX + a] : T(0);
-#pragma unroll
-                    for (int b = 0; b < RU; ++b)
-                        nv[t][RX + b] = (!cold && mine && k < N - 1 && uv[b] && P.s_y) ? P.s_y[ou + (int64_t)k * NU + l * RU + b] : T(0);
-                }
-                __syncwarp();
-#pragma unroll
-                for (int t = 0; t < UNR; ++t) {
-                    const int k = k0 + t;
-                    if (k < N) {  // warp-uniform
-                        T old[PVP];
-                        load_pb(k, old);
-                        pb_ready(old);
-#pragma unroll
-                        for (int e = 0; e < PVP; ++e) old[e] = mine ? nv[t][e] : old[e];
-                        store_pb(k, old);
-                    }
-                }
-            }
-            tm_wait_st();
-        }
         if (!cold) {
             // warm start: the instance's vnew/g/znew/y blocks are contiguous in global memory; loads are batched four
             // deep before the dependent shared-memory stores (one warp cannot hide a load-use pair per iteration)
@@ -814,7 +636,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     const int e = e0 + 32 * t;
                     const bool ok = e < N * NX;
                     va[t] = (ok && P.s_vnew) ? P.s_vnew[ox + e] : T(0);
-                    vb[t] = (!TM && ok && P.s_g) ? P.s_g[ox + e] : T(0);
+                    vb[t] = (ok && P.s_g) ? P.s_g[ox + e] : T(0);
                 }
 #pragma unroll
                 for (int t = 0; t < UNR; ++t) {
@@ -823,7 +645,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                         const int k = e / NX, i = e - k * NX;
                         const int w = idx_x(s, k, i);
                         gPA[w] = va[t];
-                        if constexpr (!TM) gPB[w] = vb[t];
+                        gPB[w] = vb[t];
                     }
                 }
             }
@@ -834,7 +656,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     const int e = e0 + 32 * t;
                     const bool ok = e < (N - 1) * NU;
                     va[t] = (ok && P.s_znew) ? P.s_znew[ou + e] : T(0);
-                    vb[t] = (!TM && ok && P.s_y) ? P.s_y[ou + e] : T(0);
+                    vb[t] = (ok && P.s_y) ? P.s_y[ou + e] : T(0);
                 }
 #pragma unroll
                 for (int t = 0; t < UNR; ++t) {
@@ -843,7 +665,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                         const int k = e / NU, j = e - k * NU;
                         const int w = idx_u(s, k, j);
                         gPA[w] = va[t];
-                        if constexpr (!TM) gPB[w] = vb[t];
+                        gPB[w] = vb[t];
                     }
                 }
             }
@@ -970,8 +792,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             const T v = gPA[w];
             if (P.sol_x) P.sol_x[ox + e] = v;
             if (P.s_vnew) P.s_vnew[ox + e] = v;
-            if constexpr (!TM)
-                if (P.s_g) P.s_g[ox + e] = gPB[w];
+            if (P.s_g) P.s_g[ox + e] = gPB[w];
             // work->v: previous vnew if the solve converged (staged in the scratch during the last forward pass; unchanged
             // if that was the first iteration of a warm start), else = vnew (admm.cpp:445); untouched when no iteration
             // ran on a warm start
@@ -985,32 +806,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             const T z = gPA[w];
             if (P.sol_u) P.sol_u[ou + e] = z;
             if (P.s_znew) P.s_znew[ou + e] = z;
-            if constexpr (!TM)
-                if (P.s_y) P.s_y[ou + e] = gPB[w];
+            if (P.s_y) P.s_y[ou + e] = gPB[w];
             if (P.s_z && !s_solved && s_it > 0) P.s_z[ou + e] = z;
             else if (P.s_z && s_solved && !(s_it == 1 && !cold)) P.s_z[ou + e] = P.gpi_vscratch[((ib * N + k) * L + j / RU) * PVP + RX + (j % RU)];
             else if (P.s_z && cold && s_it == 0) P.s_z[ou + e] = T(0);
-        }
-        if constexpr (TM) {
-            if (P.s_g || P.s_y) {  // work->g / work->y from the lanes' own TMEM columns
-                __syncwarp();
-                for (int k = 0; k < N; ++k) {
-                    T v[PVP];
-                    load_pb(k, v);
-                    pb_ready(v);
-                    if (slot == s) {
-#pragma unroll
-                        for (int a = 0; a < RX; ++a)
-                            if (xv[a] && P.s_g) P.s_g[ox + (int64_t)k * NX + l * RX + a] = v[a];
-                        if (k < N - 1) {
-#pragma unroll
-                            for (int b = 0; b < RU; ++b)
-                                if (uv[b] && P.s_y) P.s_y[ou + (int64_t)k * NU + l * RU + b] = v[RX + b];
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
         }
         // work->u.col(0): one rollout step from d_0 (every lane computes, the lanes of slot s store)
         if constexpr (PS) {
@@ -1021,11 +820,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             T xo0[RX], Xf0[NX], t10[RX + RU];
 #pragma unroll
             for (int a = 0; a < RX; ++a) xo0[a] = x0o[a];
-            gather_x(GB1, true, xo0, Xf0);
+            gather_x(xo0, Xf0);
             T d0[RU];
             load_d(0, d0);
             dots<FAST>(mS1f, Xf0, t10);
-            d_ready(d0);
 #pragma unroll
             for (int b = 0; b < RU; ++b) {
                 T u0v = (-t10[RX + b]) - d0[b];
@@ -1042,7 +840,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             T xo[RX], Xf[NX];
 #pragma unroll
             for (int a = 0; a < RX; ++a) xo[a] = x0o[a];
-            gather_x(GB1, false, xo, Xf);
+            gather_x(xo, Xf);
             for (int k = 0; k < N; ++k) {
                 T na[PVP];
 #pragma unroll
@@ -1053,19 +851,18 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     T u[RU], Uf[NU], t1[RX + RU], bu[RX], dk[RU];
                     load_d(k, dk);
                     dots<FAST>(mS1f, Xf, t1);
-                    d_ready(dk);
 #pragma unroll
                     for (int b = 0; b < RU; ++b) {
                         u[b] = (-t1[RX + b]) - dk[b];
                         na[RX + b] = u[b];
                     }
-                    gather_u(GB0, false, u, Uf);
+                    gather_u(u, Uf);
                     dots<FAST>(mB, Uf, bu);
 #pragma unroll
                     for (int a = 0; a < RX; ++a) xo[a] = (t1[a] + bu[a]) + vf[a];
                 }
                 if (slot == s) store_pack(aPA, k, na);
-                if (k < N - 1) gather_x(GB1, true, xo, Xf);
+                if (k < N - 1) gather_x(xo, Xf);
             }
             __syncwarp();
             if (P.s_x)
@@ -1096,8 +893,8 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             const int64_t ib_old = __shfl_sync(0xffffffffu, inst, s * L);
             const int was_busy = __shfl_sync(0xffffffffu, (int)busy, s * L);
             // the queue ticket is requested before the write-back of the finished instance so that the atomic's
-            // latency hides behind it.  (Never hold a ticket in advance: measured on B200, a ticket prefetched by every
-            // warp kept up to 592 instances hostage until a slot freed up and cost a whole extra wave per launch.)
+            // latency hides behind it.  (Never hold a ticket in advance: a ticket prefetched by every warp keeps instances
+            // hostage until a slot frees up, which can cost a whole extra wave per launch.)
             unsigned long long nxt = 0;
             if (lane == 0) nxt = atomicAdd(queue, 1ULL);
             if (was_busy) store_slot(s, ib_old);
@@ -1124,21 +921,19 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             T pa[PVP], pb[PVP];
             load_pack(aPA, N - 1, pa);
             load_pb(N - 1, pb);
-            pb_ready(pb);
 #pragma unroll
             for (int a = 0; a < RX; ++a) po[a] = nmac<FAST>(pterm[a], rho_(), pa[a] - pb[a]);
         }
-        gather_x(GB1, false, po, Pf);
+        gather_x(po, Pf);
         T q[RX], r[RU], Rf[NU];
         const T *xp = xrefp + (int64_t)(N - 2) * NX;
         const T *up = urefp + (has_uref ? (int64_t)(N - 2) * NU : 0);
         {
             T xr[RX], ur[RU], pa[PVP], pb[PVP];
             cost_load(N - 2, xp, up, xr, ur, pa, pb);
-            pb_ready(pb);
             cost_eval(xr, ur, pa, pb, q, r);
         }
-        gather_u(GB2, false, r, Rf);
+        gather_u(r, Rf);
         // one backward step; MORE = another column follows (its cost inputs are fetched now and consumed at the end of
         // the step).  The last step (k = 0) is peeled so that the loop body carries no k > 0 predicates.
         auto bwd_step = [&](int k, const bool MORE) {  // always inlined with a literal MORE
@@ -1153,7 +948,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             dots<FAST>(mS1b, Pf, acc1);  // [AmBKt p_{k+1} ; B^T p_{k+1}]
 #pragma unroll
             for (int b = 0; b < RU; ++b) s_[b] = (acc1[RX + b] + r[b]) + vBPf[b];
-            gather_u(GB0, false, s_, Sf);
+            gather_u(s_, Sf);
             // p_k = ((q_k + AmBKt p_{k+1}) - Kinf^T r_k) + APf
             dots<FAST>(mKt, Rf, kr);
             {
@@ -1164,18 +959,16 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 vsub<T, RX>(t1_, kr, t2_);
                 vadd<T, RX>(t2_, vAPf, po);
             }
-            if (MORE) gather_x(GB1, false, po, Pf);  // p_0 itself is never used (the forward pass starts from x_0)
+            if (MORE) gather_x(po, Pf);  // p_0 itself is never used (the forward pass starts from x_0)
             dots<FAST>(mQuu, Sf, dq);
             store_d(k, dq, busy);
             if (MORE) {
-                pb_ready(pb_n);
                 cost_eval(xr_n, ur_n, pa_n, pb_n, q, r);
-                gather_u(GB2, false, r, Rf);
+                gather_u(r, Rf);
             }
         };
         for (int k = N - 2; k >= 1; --k) bwd_step(k, true);
         bwd_step(0, false);
-        if constexpr (TM) tm_wait_st();  // d is read back by the forward pass
         __syncwarp();
 
         T rpx = T(0), rdx = T(0), rpu = T(0), rdu = T(0);
@@ -1200,11 +993,6 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         }
         } while (!__any_sync(0xffffffffu, busy && (solved || it >= P.max_iter)));
     }
-    if constexpr (TM) {
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_addr_slot) : "memory");
-    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1213,32 +1001,19 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
 struct GpiPlan {
     int L = 0, warps = 0;
     size_t smem = 0;
-    bool tm = false;  // dual packs + d in tensor memory
 };
 
-// TINYMPC_GPI_TMEM=0 keeps everything in shared memory (A/B switch for measurements)
-inline bool gpi_allow_tm() {
-    const char *e = std::getenv("TINYMPC_GPI_TMEM");
-    return !(e && e[0] == '0');
-}
-
-template <typename T, int NX, int NU, int L, bool TM>
+template <typename T, int NX, int NU, int L>
 inline void gpi_consider(int N, int max_smem, GpiPlan &best) {
     if constexpr (gpi_feasible<T, NX, NU, L>()) {
         using Cfg = GpiCfg<NX, NU, L, (int)sizeof(T)>;
-        const size_t per_warp = (TM ? Cfg::warp_elems_tm(N) : Cfg::warp_elems(N)) * sizeof(T);
+        const size_t per_warp = Cfg::warp_elems(N) * sizeof(T);
         // fp32: the TMA staging area aliases the start of the state region (the allocation is at least as large as the blob);
         // fp64: the blob stays resident in front of the state regions (matrix rows are re-read at every sweep start)
         const size_t blob = ((size_t)(3 * NX * NX + 2 * NX * NU + NU * NU + 4 * NX + 2 * NU) * sizeof(T) + 15) / 16 * 16 + 64;
         const size_t keep = gpi_per_sweep_rows<T>() ? ((size_t)(3 * NX * NX + 2 * NX * NU + NU * NU + 4 * NX + 2 * NU) * sizeof(T) + 15) / 16 * 16 : 0;
         if ((size_t)max_smem < keep + per_warp) return;
-        int w = (int)std::min<size_t>(GPI_MAX_WARPS, ((size_t)max_smem - keep) / per_warp);
-        if (TM) {
-            // every TMEM lane quarter is shared by the warps w, w+4, ...: 512 columns / (N*CPK columns per warp)
-            const int cols = Cfg::tm_cols(N);
-            if (cols > 512) return;
-            w = std::min(w, 4 * (512 / cols));
-        }
+        const int w = (int)std::min<size_t>(GPI_MAX_WARPS, ((size_t)max_smem - keep) / per_warp);
         if (w < 1 || blob > (size_t)max_smem) return;
         // score: instances resident per SM, then fewer lanes per instance (less shuffle traffic)
         const int inst = w * Cfg::IPW, binst = best.warps * (best.L ? 32 / best.L : 0);
@@ -1247,7 +1022,6 @@ inline void gpi_consider(int N, int max_smem, GpiPlan &best) {
             best.L = L;
             best.warps = w;
             best.smem = std::max(keep + per_warp * (size_t)w, blob);
-            best.tm = TM;
         }
     }
 }
@@ -1266,16 +1040,10 @@ inline GpiPlan gpi_plan(int N, int max_smem) {
     // TINYMPC_GPI_LANES=4|8|16 restricts the choice to one group width (A/B switch for measurements)
     const char *e = std::getenv("TINYMPC_GPI_LANES");
     const int only = e ? std::atoi(e) : 0;
-    if (!only || only == 4) gpi_consider<T, NX, NU, 4, false>(N, max_smem, p);
-    if (!only || only == 8) gpi_consider<T, NX, NU, 8, false>(N, max_smem, p);
+    if (!only || only == 4) gpi_consider<T, NX, NU, 4>(N, max_smem, p);
+    if (!only || only == 8) gpi_consider<T, NX, NU, 8>(N, max_smem, p);
     if constexpr (L16)
-        if (!only || only == 16) gpi_consider<T, NX, NU, 16, false>(N, max_smem, p);
-    if (gpi_allow_tm()) {  // taken only when it holds more instances per SM
-        if (!only || only == 4) gpi_consider<T, NX, NU, 4, true>(N, max_smem, p);
-        if (!only || only == 8) gpi_consider<T, NX, NU, 8, true>(N, max_smem, p);
-        if constexpr (L16)
-            if (!only || only == 16) gpi_consider<T, NX, NU, 16, true>(N, max_smem, p);
-    }
+        if (!only || only == 16) gpi_consider<T, NX, NU, 16>(N, max_smem, p);
     return p;
 }
 
@@ -1284,16 +1052,16 @@ inline int gpi_fit_T(int N, int max_smem) {
     return (int)gpi_plan<T, NX, NU>(N, max_smem).smem;
 }
 
-template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool TM, bool MM = false>
+template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool MM = false>
 int launch_gpi_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P, const T *gmat) {
     if constexpr (gpi_feasible<T, NX, NU, L>()) {
-        auto kern = gpi_solve_kernel<T, NX, NU, L, FAST, HET, TM, MM>;
+        auto kern = gpi_solve_kernel<T, NX, NU, L, FAST, HET, MM>;
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem) != cudaSuccess)
             return TINYMPC_ERR_CUDA;
         const int64_t ngroups = (d->io.B + (32 / L) - 1) / (32 / L);
         // ngroups = warps the batch fills.  A batch smaller than one wave is spread over all SMs with fewer warps per CTA
         // (the kernel's carve-up is per warp, any block size up to plan.warps works): the latency of a solve is set by how
-        // many warps share a scheduler (C2: 2.08 ms per 100 iterations with 8 warps per SM, 1.34 ms with one).
+        // many warps share a scheduler.
         int warps = plan.warps;
         if ((ngroups + warps - 1) / warps < d->sm_count) warps = (int)std::max<int64_t>(1, (ngroups + d->sm_count - 1) / d->sm_count);
         const int64_t want = (ngroups + warps - 1) / warps;
@@ -1304,7 +1072,6 @@ int launch_gpi_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P
         d->out_smem = (int)plan.smem;
         d->out_lanes_per_instance = L;
         d->out_instances_per_cta = plan.warps * (32 / L);
-        d->out_tmem_cols = TM ? 512 : 0;
         return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
     } else {
         return TINYMPC_ERR_UNSUPPORTED;

@@ -1245,7 +1245,6 @@ int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     d->out_smem = (int)plan.smem;
     d->out_lanes_per_instance = L;
     d->out_instances_per_cta = plan.warps * (32 / L) * NI;
-    d->out_tmem_cols = 0;
     return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
 }
 

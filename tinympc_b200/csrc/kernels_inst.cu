@@ -47,7 +47,6 @@ int launch_tpi(LaunchDesc *d) {
     d->out_smem = 0;
     d->out_lanes_per_instance = 1;
     d->out_instances_per_cta = threads;
-    d->out_tmem_cols = 0;
     return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
 }
 
@@ -105,15 +104,15 @@ int launch_gpi(LaunchDesc *d) {
     fill_params<T, NX, NU>(P, *d);
     const T *gmat = (const T *)d->gmat;
     const bool het = d->io.models != nullptr;  // heterogeneous batch: per-instance model blobs
-    // STRICT, shared model, tensor-memory plan (the headline path): min / max clamp when no bound is a signed zero
-#define TM_GPI_CASE(LL, HH, TT)                                                                                          \
-    if (plan.L == LL && het == HH && plan.tm == TT) {                                                                    \
-        if constexpr (!FAST && !HH && TT && sizeof(T) == 4) {                                                            \
-            if (d->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, FAST, HH, TT, true>(d, plan, P, gmat);           \
+    // STRICT fp32, shared model (the headline path): min / max clamp when no bound is a signed zero
+#define TM_GPI_CASE(LL, HH)                                                                                              \
+    if (plan.L == LL && het == HH) {                                                                                     \
+        if constexpr (!FAST && !HH && sizeof(T) == 4) {                                                                  \
+            if (d->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, FAST, HH, true>(d, plan, P, gmat);               \
         }                                                                                                                \
-        return launch_gpi_L<T, NX, NU, LL, FAST, HH, TT>(d, plan, P, gmat);                                              \
+        return launch_gpi_L<T, NX, NU, LL, FAST, HH>(d, plan, P, gmat);                                                  \
     }
-#define TM_GPI_L(LL) TM_GPI_CASE(LL, false, false) TM_GPI_CASE(LL, true, false) TM_GPI_CASE(LL, false, true) TM_GPI_CASE(LL, true, true)
+#define TM_GPI_L(LL) TM_GPI_CASE(LL, false) TM_GPI_CASE(LL, true)
     TM_GPI_L(4)
     TM_GPI_L(8)
 #ifdef TM_GPI_L16

@@ -46,7 +46,7 @@ struct LaunchDesc {
     int max_smem_optin;
 
     // filled by the launcher
-    int out_threads, out_ctas, out_smem, out_lanes_per_instance, out_instances_per_cta, out_tmem_cols;
+    int out_threads, out_ctas, out_smem, out_lanes_per_instance, out_instances_per_cta;
     size_t out_ws_need;  // GPS: workspace bytes this launch needs (set when the launcher returns TM_ERR_WORKSPACE)
 };
 

@@ -1,7 +1,7 @@
 """Host-side problem description for the batched solve path.
 
 `MPCProblem` is the read-only part of the reference's TinyWorkspace + TinyCache
-(/root/reference/src/tinympc/types.hpp:43-59, 88-208) as numpy arrays; `Settings` mirrors TinySettings
+(TinyMPC src/tinympc/types.hpp:43-59, 88-208) as numpy arrays; `Settings` mirrors TinySettings
 (types.hpp:63-82, defaults tiny_api_constants.hpp:5-16).  All matrices are stored COLUMN-MAJOR
 (Fortran order), exactly as the reference's dynamic Eigen matrices, so that `.ctypes.data` can be handed
 straight to the C ABI (include/tinympc_b200.h).

@@ -1,3 +1,3 @@
-// forwarding header: the reference layout <tinympc/types.hpp> -> the B200 shim
+// forwarding header: the reference layout <tinympc/types.hpp> -> the H100 shim
 #pragma once
 #include "../../tinympc_shim.hpp"

@@ -1,11 +1,11 @@
 // tinympc_shim.hpp — source-compatible C++ front end of the reference's solver interface on top of the
-// B200 C ABI (include/tinympc_b200.h).
+// H100 C ABI (include/tinympc_b200.h).
 //
 // A program written against the reference (#include <tinympc/tiny_api.hpp>, TinySolver struct tree, tiny_setup /
 // tiny_set_* / tiny_solve) compiles unchanged against this header and links tinympc_shim.cpp +
 // libtinympc_b200.so; tiny_solve() then runs on the GPU (a batch of one through tinympc_b200_solve_host —
 // Eigen's dynamic matrices are contiguous column-major, so the struct tree's buffers are handed to the C ABI
-// without copies).  Names, argument order and return codes follow /root/reference/src/tinympc/tiny_api.hpp:10-62
+// without copies).  Names, argument order and return codes follow TinyMPC src/tinympc/tiny_api.hpp:10-62
 // and types.hpp:32-218, including the known quirks (SURVEY §8b / A.3): the cone setter's positional semantics,
 // the "double rho" in the cache, tiny_set_bound_constraints returning 0 on a dimension mismatch, and the
 // "Solver converged in N iterations" line on stdout (admm.cpp:439).

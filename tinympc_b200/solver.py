@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's solver interface for the batched B200 path.
+"""Host-side mirror of the reference's solver interface for the batched H100 path.
 
 The reference's user-facing calls (src/tinympc/tiny_api.hpp:10-62) map as follows:
 
@@ -94,7 +94,7 @@ def unpack_model(blob, nx, nu):
 
 
 class BatchedTinySolver:
-    """A TinySolver (types.hpp:213-218) for B independent instances on one B200."""
+    """A TinySolver (types.hpp:213-218) for B independent instances on one H100."""
 
     def __init__(self, problem: MPCProblem, settings: abi.Settings | None = None, device: int = 0,
                  mode: int = abi.MODE_STRICT, kernel: int = abi.KERNEL_AUTO):

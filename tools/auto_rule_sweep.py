@@ -24,7 +24,8 @@ FAM = {"gpi": abi.KERNEL_GPI, "gps": abi.KERNEL_GPS, "tpi": abi.KERNEL_TPI, "aut
 NAMES = {1: "tpi", 2: "gpi", 4: "gps"}
 shapes = [(np.float32, 4, 8, 100), (np.float32, 8, 8, 100), (np.float32, 12, 4, 100), (np.float32, 12, 8, 100), (np.float32, 16, 4, 100),
           (np.float32, 16, 8, 100), (np.float32, 12, 8, 50), (np.float32, 16, 8, 50), (np.float32, 12, 4, 50),
-          (np.float64, 12, 4, 50), (np.float64, 6, 3, 100), (np.float64, 4, 2, 50), (np.float64, 16, 8, 50),
+          (np.float64, 12, 4, 50), (np.float64, 6, 3, 100), (np.float64, 4, 2, 100), (np.float64, 4, 4, 100), (np.float64, 4, 2, 50),
+          (np.float64, 16, 8, 50),
           # small batches (one thread per instance cannot fill the GPU)
           (np.float64, 12, 4, 50, 4096), (np.float32, 12, 8, 100, 4096), (np.float32, 16, 4, 100, 8192), (np.float64, 8, 4, 50, 16384)]
 if a.only == "f64_12_4":
@@ -51,7 +52,7 @@ for shp in shapes:
                 ms.append(s.stats()["kernel_ms"])
             st = s.stats()
             best = min(ms[1:])
-            plan = f"L={st['lanes_per_instance']} {st['instances_per_cta']}/CTA x{st['ctas']}" + (" tmem" if st["tmem_cols_per_cta"] else "")
+            plan = f"L={st['lanes_per_instance']} {st['instances_per_cta']}/CTA x{st['ctas']}"
             print(f"| {np.dtype(dt).name} | {nx} | {nu} | {N} | {B} | {fam} | {NAMES[st['kernel_family']]} | {plan} | {best:.3f} | "
                   f"{int(out['iter'].sum().item()) / best * 1e3:.3e} |", flush=True)
             s.close()

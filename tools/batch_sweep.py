@@ -44,7 +44,7 @@ for cfg, sizes in (("C2 quadrotor hovering fp32 N=50, 100 it", [1, 64, 1024, 409
         st = s.stats()
         best = min(ms[1:])
         iters = int(out["iter"].sum().item())
-        plan = f"L={st['lanes_per_instance']} x{st['ctas']} CTAs" + (" tmem" if st["tmem_cols_per_cta"] else "")
+        plan = f"L={st['lanes_per_instance']} x{st['ctas']} CTAs"
         print(f"| {cfg} | {B} | {NAMES[st['kernel_family']]} | {plan} | {best:.3f} | {B / best * 1e3:.3e} | {iters / best * 1e3:.3e} | "
               f"{best * 1e3 / iters:.4f} |", flush=True)
         s.close()

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Markdown tables from bench.py JSON lines (what profiles/README.md quotes).
-usage: python tools/bench_table.py profiles/r02_bench_n1.json [profiles/r02_bench_reference_arm.json] [more GPU-arm lines ...]"""
+"""Markdown tables from bench.py JSON lines.
+usage: python tools/bench_table.py bench_n1.json [bench_reference_arm.json] [more GPU-arm lines ...]"""
 import json
 import sys
 
@@ -14,7 +14,7 @@ ref = [d for d in gpu if d.get("impl") == "reference"]
 gpu = [d for d in gpu if d.get("impl") != "reference"]
 for d in gpu:
     n = d["n_gpus"]
-    print(f"### {n} x B200  (steps {d['steps']}, warm-up {d['warmup']}, SM clock {d['clocks']['sm_mhz']} MHz, throttle reasons {d['clocks']['reasons']})\n")
+    print(f"### {n} GPU(s)  (steps {d['steps']}, warm-up {d['warmup']}, SM clock {d['clocks']['sm_mhz']} MHz, throttle reasons {d['clocks']['reasons']})\n")
     print("| config | kernel plan | ms / batch | instances/s | ADMM it/s/GPU | solved | mean it | algorithmic GB/s (frac of HBM peak) | e2e ms (inst/s) | reference CPU inst/s (threads, 1-thread) | GPU/CPU |")
     print("|---|---|---|---|---|---|---|---|---|---|---|")
     cb = d.get("cpu_baseline") or {}
@@ -23,7 +23,7 @@ for d in gpu:
         rows.append((k, v["plan"], v["ms_per_step"], v["value"], v["admm_iters_per_s_per_gpu"], v["solved_fraction"], v["mean_iters"], v["roofline"], v.get("e2e"),
                      v.get("cpu_reference") or {}))
     for name, plan, ms, val, its, sol, mi, roof, e2e, c in rows:
-        pl = f"{plan['kernel']} L={plan['lanes_per_instance']} {plan['instances_per_cta']}/SM" + (" tmem" if plan.get("tmem_cols_per_cta") else "")
+        pl = f"{plan['kernel']} L={plan['lanes_per_instance']} {plan['instances_per_cta']}/SM"
         e = f"{e2e['ms_per_step']:.2f} ({e2e['value']:.3e})" if e2e else "—"
         cpu = f"{c['value']:.0f} ({c['cores']}, {c['one_thread']:.0f})" if c.get("value") else "—"
         ratio = f"{val / c['value'] / n:.0f}x" if c.get("value") else "—"

@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """Extract the numeric problem/trajectory tables of the reference examples into .npz fixtures.
 
-Run in the build container only (needs /root/reference):
+Needs a TinyMPC checkout, named by TINYMPC_REFERENCE:
     python tools/extract_problem_data.py
-Reads   /root/reference/examples/problem_data/*.hpp and examples/trajectory_data/*.hpp  (numbers only)
+Reads   $TINYMPC_REFERENCE/examples/problem_data/*.hpp and examples/trajectory_data/*.hpp  (numbers only)
 Writes  tinympc_b200/data/{quadrotor_20hz,quadrotor_50hz,rocket_20hz}.npz  and quadrotor_20hz_y_axis_line.npz
 
 The .npz files hold INPUT DATA (A, B, f, Q, R, rho and a reference trajectory), i.e. the workload
@@ -17,7 +17,7 @@ import sys
 
 import numpy as np
 
-REF = os.environ.get("TINYMPC_REFERENCE", "/root/reference")
+REF = os.environ["TINYMPC_REFERENCE"]
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tinympc_b200", "data")
 
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Key figures of `ncu --set full` reports as a markdown table (what profiles/*_ncu_summary.md quotes).
+"""Key figures of `ncu --set full` reports as a markdown table.
 usage: python tools/ncu_summary.py label=path.ncu-rep [label=path ...]"""
 import csv
 import io

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """BASELINE config 5: synthetic random-LTI sweep nx x nu x N, fp32, fixed work (max_iter=50, tolerances 0) -> roofline
 table (ADMM iterations/s, algorithmic HBM bytes vs peak, fp32-pipe fraction), plus configs 3 and 4 at full size.
-Writes a markdown table to stdout; one B200.  B per GPU = 2^20 / 8 = 131072 (the 8-GPU share of the config)."""
+Writes a markdown table to stdout; one GPU.  B per GPU = 2^20 / 8 = 131072 (the 8-GPU share of the config)."""
 import argparse
 import json
 import os
@@ -21,7 +21,7 @@ ap.add_argument("--reps", type=int, default=3)
 ap.add_argument("--quick", action="store_true")
 a = ap.parse_args()
 peaks = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "MEASURED_PEAKS.json")
-HBM = float(json.load(open(peaks))["hbm_gbs"]) if os.path.exists(peaks) else 6650.0
+HBM = float(json.load(open(peaks))["hbm_gbs"]) if os.path.exists(peaks) else 3350.0  # H100 SXM data sheet
 
 
 def run(spec, dt, inst, kernel, mode, reps):
@@ -63,7 +63,7 @@ def row(name, spec, dt, inst, B, kernel, kname, mode, mname, per_inst_ref):
     gbs = B * bytes_inst(spec.nx, spec.nu, spec.N, es, per_inst_ref) / (ms * 1e-3) / 1e9
     tf = iters * flops_iter(spec.nx, spec.nu, spec.N) / (ms * 1e-3) / 1e12
     lanes, ipc = st["lanes_per_instance"], st["instances_per_cta"]
-    fam = {1: "tpi", 2: f"gpi L={lanes} {ipc}/SM" + (" tmem" if st["tmem_cols_per_cta"] else ""), 4: f"gps L={lanes} {ipc}/SM"}[st["kernel_family"]]
+    fam = {1: "tpi", 2: f"gpi L={lanes} {ipc}/SM", 4: f"gps L={lanes} {ipc}/SM"}[st["kernel_family"]]
     print(f"| {name} | {spec.nx} | {spec.nu} | {spec.N} | {B} | {np.dtype(dt).name} | {fam} | {mname} | {ms:.3f} | {B / ms * 1e3:.3e} | "
           f"{iters / ms * 1e3:.3e} | {solved / B:.2f} | {gbs:.1f} | {gbs / HBM:.5f} | {tf:.2f} |", flush=True)
 
