@@ -44,6 +44,85 @@ def bits_equal(a, b):
     return a.shape == b.shape and a.dtype == b.dtype and np.array_equal(a.view(np.uint8), b.view(np.uint8))
 
 
+# NaN bit patterns no arithmetic result carries (quiet NaNs with a fixed payload); int32 arrays get the 32-bit word, which is
+# no plausible iteration count or flag either
+POISON_BITS = {4: 0x7FA5A5A5, 8: 0x7FF4A5A5A5A5A5A5}
+
+
+def poison(a):
+    """Fill a numpy array or torch tensor in place with the POISON_BITS pattern of its element size, so that an element a
+    solve never writes cannot match an oracle value by accident (a zero-initialised buffer matches every zero)."""
+    if a is None:
+        return a
+    if isinstance(a, np.ndarray):
+        a.view(np.uint32 if a.itemsize == 4 else np.uint64).fill(POISON_BITS[a.itemsize])
+    else:
+        import torch
+
+        a.view(torch.int32 if a.element_size() == 4 else torch.int64).fill_(POISON_BITS[a.element_size()])
+    return a
+
+
+def assert_bits_per_instance(got, ref, keys, what):
+    """bits_equal on every key; on a mismatch, name how many instances differ and the first few of them (which tells a
+    first-wave fault from a refill / chunk-offset fault)."""
+    for key in keys:
+        a, b = np.ascontiguousarray(got[key]), np.ascontiguousarray(ref[key])
+        if bits_equal(a, b):
+            continue
+        assert a.shape == b.shape and a.dtype == b.dtype, (what, key, a.shape, a.dtype, b.shape, b.dtype)
+        n = a.shape[0]
+        bad = np.flatnonzero((a.view(np.uint8).reshape(n, -1) != b.view(np.uint8).reshape(n, -1)).any(axis=1))
+        raise AssertionError(f"{what}: {key} differs in {len(bad)} of {n} instances, first {bad[:8].tolist()}")
+
+
+def assert_mixed_termination(res):
+    """The instances of the batch retire at different iterations, and both converged and max_iter-capped ones occur."""
+    it, sv = np.asarray(res["iter"]), np.asarray(res["solved"])
+    assert len(np.unique(it)) >= 5, np.unique(it)
+    assert sv.any() and not sv.all(), int(sv.sum())
+
+
+def device_closed_loop_vs_oracle(solver, inst, steps, port):
+    """The reference's closed loop (set x0 -> solve warm-started with the duals reset -> x0 = A x0 + B u0) kept on the GPU
+    (DeviceMPCLoop + tinympc_b200_advance), compared at every step with the oracle stepping the same loop on the host.
+    port(prob, settings, x0, Xref, Uref, state, cold, want) -> oracle result dict.  Returns the oracle result of each step."""
+    from tinympc_b200.closed_loop import DeviceMPCLoop
+
+    prob, st = solver.problem, solver.settings
+    traj = inst["Xref"]
+    loop = DeviceMPCLoop(solver, inst["x0"], reset_duals=True)
+    x0 = inst["x0"].copy()
+    state = None
+    A, Bm, f = prob.A, prob.B, prob.f
+    outs = []
+    for k in range(steps):
+        Xref = np.ascontiguousarray(np.roll(traj, -k, axis=1))  # a different window every step
+        out = loop.step(Xref)
+        if state is not None:
+            state["g"] = np.zeros_like(state["g"])
+            state["y"] = np.zeros_like(state["y"])
+        o = port(prob, st, x0, Xref, None, state, state is None, tuple(BOX_STATE))
+        got = {key: out[key].cpu().numpy() for key in OUT_KEYS + list(loop.fields) + ["u0"]}
+        assert_bits_per_instance(got, o, OUT_KEYS + list(loop.fields), f"closed loop step {k}")
+        assert_bits_per_instance(got, dict(u0=np.ascontiguousarray(o["u"][:, 0, :])), ["u0"], f"closed loop step {k}")
+        outs.append(o)
+        state = {n: o[n] for n in BOX_STATE}
+        u0 = o["u"][:, 0, :]
+        nxt = np.zeros_like(x0)
+        for i in range(prob.nx):  # same ascending-k, no-FMA arithmetic as tinympc_b200_advance
+            ax = A[i, 0] * x0[:, 0]
+            for m in range(1, prob.nx):
+                ax = ax + A[i, m] * x0[:, m]
+            bu = Bm[i, 0] * u0[:, 0]
+            for j in range(1, prob.nu):
+                bu = bu + Bm[i, j] * u0[:, j]
+            nxt[:, i] = (ax + bu) + f[i]
+        x0 = nxt
+        assert bits_equal(loop.x0.cpu().numpy(), x0), ("advance", k)
+    return outs
+
+
 def problem_from_spec(spec: wl.ModelSpec, dtype, setup) -> MPCProblem:
     """setup(nx,nu,N,rho,A,B,f,Qdiag,Rdiag,dtype=..., **constraints) -> MPCProblem (oracle.ref_setup / port_setup)."""
     return setup(spec.nx, spec.nu, spec.N, spec.rho, spec.A, spec.B, spec.f, spec.Qdiag, spec.Rdiag, dtype=dtype,

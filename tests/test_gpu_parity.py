@@ -274,42 +274,11 @@ def test_errors_are_loud():
 def test_device_resident_closed_loop_matches_oracle(kernel):
     """SURVEY §8f-1: the reference's closed loop (set x0 -> solve warm-started -> x0 = A x0 + B u0) for 300 plants kept
     entirely on the GPU (DeviceMPCLoop + tinympc_b200_advance) equals the oracle stepping the same loop on the host."""
-    from tinympc_b200.closed_loop import DeviceMPCLoop
-
     spec = wl.quadrotor(N=10)
     dt = np.float32
     prob = setup_problem(spec, dt)
-    st = spec.settings
-    B, steps = 300, 6
-    inst = wl.tracking_instances(B, N=10, seed=12, dtype=dt)
-    traj = inst["Xref"]
-    loop = DeviceMPCLoop(_mk_solver(prob, st, kernel), inst["x0"], reset_duals=True)
-    x0 = inst["x0"].copy()
-    state = None
-    A, Bm, f = prob.A, prob.B, prob.f
-    for k in range(steps):
-        Xref = np.ascontiguousarray(np.roll(traj, -k, axis=1))  # a different window every step
-        out = loop.step(Xref)
-        if state is not None:
-            state["g"] = np.zeros_like(state["g"])
-            state["y"] = np.zeros_like(state["y"])
-        o = _port(prob, st, x0, Xref, None, state, state is None, tuple(H.BOX_STATE))
-        for key in H.OUT_KEYS + list(loop.fields):
-            assert H.bits_equal(out[key].cpu().numpy(), o[key]), (k, key)
-        assert H.bits_equal(out["u0"].cpu().numpy(), np.ascontiguousarray(o["u"][:, 0, :])), (k, "u0")
-        state = {n: o[n] for n in H.BOX_STATE}
-        u0 = o["u"][:, 0, :]
-        nxt = np.zeros_like(x0)
-        for i in range(prob.nx):  # same ascending-k, no-FMA arithmetic as tinympc_b200_advance
-            ax = A[i, 0] * x0[:, 0]
-            for m in range(1, prob.nx):
-                ax = ax + A[i, m] * x0[:, m]
-            bu = Bm[i, 0] * u0[:, 0]
-            for j in range(1, prob.nu):
-                bu = bu + Bm[i, j] * u0[:, j]
-            nxt[:, i] = (ax + bu) + f[i]
-        x0 = nxt
-        assert H.bits_equal(loop.x0.cpu().numpy(), x0), ("advance", k)
+    inst = wl.tracking_instances(300, N=10, seed=12, dtype=dt)
+    H.device_closed_loop_vs_oracle(_mk_solver(prob, spec.settings, kernel), inst, 6, _port)
 
 
 @pytest.mark.parametrize("kernel", ALLK)
