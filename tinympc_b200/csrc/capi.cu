@@ -15,6 +15,7 @@
 
 #include "host_precompute.h"
 #include "launch.h"
+#include "model_blob.h"
 
 #define TM_DECL(nx, nu) extern "C" const tmpc::DimEntry *tm_dim_entry_##nx##_##nu();
 TM_DIMS(TM_DECL)
@@ -31,7 +32,8 @@ __global__ void advance_kernel(int nx, int nu, int64_t ustride, int64_t B, const
     if (valid) {
         const int64_t b = t / nx;
         const int i = (int)(t - b * nx);
-        const T *A = blob, *Bm = blob + nx * nx, *f = Bm + nx * nu;
+        const tmpc::ModelBlob mb = tmpc::model_blob(nx, nu);
+        const T *A = blob + mb.A, *Bm = blob + mb.B, *f = blob + mb.f;
         const T *xb = x0 + b * nx, *ub = u + b * ustride;
         T ax = A[i] * xb[0];
         for (int m = 1; m < nx; ++m) ax = ax + A[i + nx * m] * xb[m];
@@ -189,16 +191,13 @@ int check_ready(const tinympc_b200_solver *s) {
 }
 
 // Which kernel family serves a solve.  GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane mapping covers); TPI = one thread per instance.
-// `smem_out`: shared-memory bytes of the on-chip plan (0 = not available).  Returns -1 when an explicit request cannot
-// be honoured.
-int resolve_family(const tinympc_b200_solver *s, const Features &ft, int *smem_out, int64_t B = 0) {
-    int smem = 0;
-    bool gpi_ok = false;
-    if (!ft.ext && s->dim->gpi_fit) {
-        smem = s->dim->gpi_fit(s->dtype, s->N, s->max_smem_optin);
-        gpi_ok = smem > 0;
-    }
-    if (smem_out) *smem_out = smem;
+// `gpi_out`: the on-chip kernel's launch plan (L == 0: not available).  Returns -1 when an explicit request cannot be
+// honoured.
+int resolve_family(const tinympc_b200_solver *s, const Features &ft, tmpc::GpiPlan *gpi_out, int64_t B = 0) {
+    tmpc::GpiPlan gpi;
+    if (!ft.ext && s->dim->gpi_plan) gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin);
+    const bool gpi_ok = gpi.smem > 0;
+    if (gpi_out) *gpi_out = gpi;
     const bool gps_ok = s->dim->gps_lanes && s->dim->gps_lanes(s->dtype) > 0;
     if (s->family == TINYMPC_KERNEL_GPI) return gpi_ok ? TINYMPC_KERNEL_GPI : (gps_ok ? TINYMPC_KERNEL_GPS : -1);
     if (s->family == TINYMPC_KERNEL_GPS) return gps_ok ? TINYMPC_KERNEL_GPS : -1;
@@ -218,8 +217,7 @@ int resolve_family(const tinympc_b200_solver *s, const Features &ft, int *smem_o
     // (12,4,100): 85 vs 94 ms) and loses at 8 ((4,8,100): 128 vs 78 ms); fp64 (rows re-read per sweep) on chip wins with three
     // warps per SM ((4,2,50): 13 vs 19 ms; (16,8,50): 80 vs 197 ms) unless they hold only 6 instances ((12,4,50): 73 vs 60 ms),
     // and loses badly with one warp ((6,3,100): 143 vs 60 ms thread per instance).
-    const int plan = s->dim->gpi_instances_per_cta ? s->dim->gpi_instances_per_cta(s->dtype, s->N, s->max_smem_optin) : 0;
-    const int ipc = plan & 0xffff, gpi_warps = plan >> 16;
+    const int ipc = gpi.instances_per_cta, gpi_warps = gpi.warps;
     const bool tpi_heavy = s->nx >= 16 && s->nu >= 8;
     const bool few = s->dtype == TINYMPC_F64 ? (gpi_warps < 2 || ipc < 8) : ipc < 16;
     if (ipc > 0 && few && !tpi_heavy && big_batch) return streamed;
@@ -335,10 +333,10 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     if (io->B <= 0) return TINYMPC_OK;
     const Features ft = features(s);
-    int smem = 0;
-    int family = resolve_family(s, ft, &smem, io->B);
+    tmpc::GpiPlan gpi;
+    int family = resolve_family(s, ft, &gpi, io->B);
     if (io->models) {  // per-instance models: on-chip kernel only
-        if (ft.ext || smem <= 0 || s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
+        if (ft.ext || gpi.smem <= 0 || s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
             return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models need the on-chip GPI kernel (box constraints, horizon fitting in shared memory)");
         family = TINYMPC_KERNEL_GPI;
     }
@@ -359,13 +357,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
         d.work_queue = s->queue.p;
         d.gpi_vscratch = nullptr;
         if (family == TINYMPC_KERNEL_GPI && (io->state.v || io->state.z)) {  // previous-iteration slacks are staged in pack layout, one 16-byte store per knot point
-            const int plan = s->dim->gpi_instances_per_cta(s->dtype, s->N, s->max_smem_optin);
-            const int warps = plan >> 16, ipc = plan & 0xffff;
-            const int L = (warps > 0 && ipc > 0) ? 32 * warps / ipc : 4;
-            const int W = s->dtype == TINYMPC_F64 ? 2 : 4;
-            const int pv = (s->nx + L - 1) / L + (s->nu + L - 1) / L;
-            const size_t pvp = (size_t)(pv + W - 1) / W * W;
-            if (s->vscratch.ensure((size_t)io->B * s->N * L * pvp * esize(s->dtype) + 256)) return fail(TINYMPC_ERR_CUDA, "GPI v-scratch allocation failed");
+            if (s->vscratch.ensure((size_t)io->B * gpi.vscratch_per_instance + 256)) return fail(TINYMPC_ERR_CUDA, "GPI v-scratch allocation failed");
             d.gpi_vscratch = s->vscratch.p;
         }
         d.Bpad = (io->B + 31) / 32 * 32;
@@ -422,16 +414,16 @@ namespace {
 template <typename T>
 int precompute_batch_T(int nx, int nu, int64_t B, const T *A, const T *Bm, const T *f, const T *Qd, const T *Rd, const T *rho,
                        T *out, int nthreads, int64_t *bad_index = nullptr) {
-    const int64_t M = tinympc_b200_model_blob_elems(nx, nu);
+    const tmpc::ModelBlobT<int64_t> mb = tmpc::model_blob<int64_t>(nx, nu);
     nthreads = (int)std::max<int64_t>(1, std::min<int64_t>(nthreads, B));
     std::vector<int64_t> bad(nthreads, 0);
     auto work = [&](int t) {
         std::vector<T> Qw(nx), Rw(nu);
         for (int64_t b = t; b < B; b += nthreads) {
             const T *Ab = A + b * nx * nx, *Bb = Bm + b * nx * nu, *fb = f + b * nx;
-            T *o = out + b * M;
-            T *oA = o, *oB = oA + nx * nx, *oF = oB + nx * nu, *oQ = oF + nx, *oR = oQ + nx, *oK = oR + nu, *oP = oK + nu * nx,
-              *oQuu = oP + nx * nx, *oAm = oQuu + nu * nu, *oAPf = oAm + nx * nx, *oBPf = oAPf + nx;
+            T *o = out + b * mb.model;
+            T *oA = o + mb.A, *oB = o + mb.B, *oF = o + mb.f, *oQ = o + mb.Qd, *oR = o + mb.Rd, *oK = o + mb.Kinf, *oP = o + mb.Pinf,
+              *oQuu = o + mb.Quu, *oAm = o + mb.AmBKt, *oAPf = o + mb.APf, *oBPf = o + mb.BPf;
             const T r = rho[b];
             for (int i = 0; i < nx; ++i) Qw[i] = Qd[b * nx + i] + r;  // tiny_api.cpp:117
             for (int j = 0; j < nu; ++j) Rw[j] = Rd[b * nu + j] + r;  // tiny_api.cpp:118
@@ -441,7 +433,7 @@ int precompute_batch_T(int nx, int nu, int64_t B, const T *A, const T *Bm, const
             std::copy(Qw.begin(), Qw.end(), oQ);
             std::copy(Rw.begin(), Rw.end(), oR);
             const int rc = tmpc::precompute_cache<T>(nx, nu, (double)r, Ab, Bb, fb, Qw.data(), Rw.data(), oK, oP, oQuu, oAm, oAPf, oBPf);
-            oBPf[nu] = r;
+            o[mb.rho] = r;
             if (rc < 0 && bad[t] == 0) bad[t] = b + 1;
         }
     };
@@ -509,7 +501,7 @@ int tinympc_b200_precompute_cache(int32_t dtype, int32_t nx, int32_t nu, double 
 }
 
 int64_t tinympc_b200_model_blob_elems(int32_t nx, int32_t nu) {
-    return (int64_t)3 * nx * nx + 2 * nx * nu + nu * nu + 3 * nx + 2 * nu + 1;
+    return tmpc::model_blob<int64_t>(nx, nu).model;
 }
 
 int tinympc_b200_precompute_cache_batch(int32_t dtype, int32_t nx, int32_t nu, int64_t B, const void *A, const void *Bm,
@@ -588,11 +580,12 @@ int tinympc_b200_create(const tinympc_problem_t *p, int32_t device, tinympc_b200
     s->APf = copy_bytes(p->APf, es * nx); s->BPf = copy_bytes(p->BPf, es * nu);
     tinympc_b200_default_settings(&s->settings);
     bool ok = true;
-    {   // packed cache blob for the GPI kernel's TMA staging: A,B,f,Qd,Rd,Kinf,Pinf,Quu,AmBKt,APf,BPf
-        std::vector<char> blob;
-        for (const std::vector<char> *v : {&s->A, &s->Bm, &s->f, &s->Qd, &s->Rd, &s->Kinf, &s->Pinf, &s->Quu, &s->AmBKt, &s->APf, &s->BPf})
-            blob.insert(blob.end(), v->begin(), v->end());
-        blob.resize((blob.size() + 63) / 64 * 64, 0);
+    {   // the cache blob (model_blob.h) the lane-group kernels stage into shared memory
+        const tmpc::ModelBlob mb = tmpc::model_blob(p->nx, p->nu);
+        std::vector<char> blob(((size_t)mb.cache * es + 63) / 64 * 64, 0);
+        auto put = [&](int off, const std::vector<char> &v) { std::memcpy(blob.data() + (size_t)off * es, v.data(), v.size()); };
+        put(mb.A, s->A); put(mb.B, s->Bm); put(mb.f, s->f); put(mb.Qd, s->Qd); put(mb.Rd, s->Rd); put(mb.Kinf, s->Kinf);
+        put(mb.Pinf, s->Pinf); put(mb.Quu, s->Quu); put(mb.AmBKt, s->AmBKt); put(mb.APf, s->APf); put(mb.BPf, s->BPf);
         ok &= !upload(s->d_blob, blob.data(), blob.size());
     }
     auto varies = [&](const void *m, size_t rows, size_t cols) {  // does a (rows x cols) column-major matrix vary along columns?
@@ -821,12 +814,6 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
     if (io->residuals) fields.push_back({nullptr, io->residuals, 4 * es, false, true, (void **)&dev.residuals});
 
     for (Field &f : fields) f.pinned = is_pinned(f.is_out ? f.dst : f.src) && (!f.is_in || !f.src || is_pinned(f.src));
-    size_t per_inst_dev = 0, per_inst_in = 0, per_inst_out = 0;
-    for (const Field &f : fields) {
-        per_inst_dev += f.per_inst;
-        if (f.is_in) per_inst_in += f.per_inst;
-        if (f.is_out) per_inst_out += f.per_inst;
-    }
     // chunking: big enough to fill the GPU several times over, small enough to pipeline
     int64_t chunk = B;
     if (B > 16384) chunk = std::max<int64_t>(8192, (B + 7) / 8);
@@ -834,10 +821,10 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
     {   // the persistent GPI kernel holds sm_count * instances_per_cta instances at a time: make a chunk a whole
         // number of such waves so that no chunk ends on a mostly empty wave
         const Features ft = features(s);
-        int smem = 0;
-        const int fam = resolve_family(s, ft, &smem, chunk);
-        if (fam == TINYMPC_KERNEL_GPI && s->dim->gpi_instances_per_cta && B > 16384) {
-            const int64_t wave = (int64_t)s->sm_count * (s->dim->gpi_instances_per_cta(s->dtype, s->N, s->max_smem_optin) & 0xffff);
+        tmpc::GpiPlan gpi;
+        const int fam = resolve_family(s, ft, &gpi, chunk);
+        if (fam == TINYMPC_KERNEL_GPI && B > 16384) {
+            const int64_t wave = (int64_t)s->sm_count * gpi.instances_per_cta;
             if (wave > 0 && wave < B) chunk = std::max<int64_t>(1, (chunk + wave / 2) / wave) * wave;
         }
     }
@@ -936,7 +923,6 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
     s->stats.kernel_launches = launches;
     s->timed = false;
     s->stats.kernel_ms = 0.f;
-    (void)per_inst_dev; (void)per_inst_in; (void)per_inst_out;
     return TINYMPC_OK;
 }
 

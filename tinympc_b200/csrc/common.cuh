@@ -1,4 +1,4 @@
-// common.cuh — arithmetic policy + kernel parameter block shared by the TPI and GPI kernels.
+// common.cuh — arithmetic policy, vector helpers and the kernel parameter block shared by the TPI, GPI and GPS kernels.
 //
 // Arithmetic contract (DESIGN.md §4; SURVEY.md Appendix A/B.2):
 //   every translation unit is compiled with -fmad=false, so plain `a*b + c` is NEVER contracted;
@@ -123,6 +123,34 @@ __device__ __forceinline__ void project_soc3_sel(T &s0, T &s1, T &s2, T mu_T) {
     s1 = below ? T(0) : (inside ? s1 : r1);
     s2 = below ? T(0) : (inside ? s2 : r2);
 }
+
+// sequential hyperplane projections on one column (admm.cpp:148-157 / :186-195, SURVEY A.5).
+// A is (ld x NE) column-major in global memory; rows row0 .. row0+n-1; b[k] at bvec[k].
+template <bool FAST, typename T, int NE>
+__device__ __forceinline__ void project_rows(T (&z)[NE], const T *A, int ld, int row0, int n, const T *bvec) {
+    for (int r = 0; r < n; ++r) {
+        T a[NE];
+#pragma unroll
+        for (int j = 0; j < NE; ++j) a[j] = __ldg(A + row0 + r + (int64_t)j * ld);
+        const T bb = __ldg(bvec + r);
+        T cv = a[0] * z[0];
+#pragma unroll
+        for (int j = 1; j < NE; ++j) cv = mac<FAST>(cv, a[j], z[j]);
+        if (cv > bb) {
+            T nn = a[0] * a[0];
+#pragma unroll
+            for (int j = 1; j < NE; ++j) nn = mac<FAST>(nn, a[j], a[j]);
+            const T dist = (cv - bb) / nn;  // a.dot(z) is recomputed by the reference; same value
+#pragma unroll
+            for (int j = 0; j < NE; ++j) z[j] = nmac<FAST>(z[j], dist, a[j]);
+        }
+    }
+}
+
+// the 16-byte vector type of T and its element count
+template <typename T> struct Vec16;
+template <> struct Vec16<float> { using type = float4; static constexpr int E = 4; };
+template <> struct Vec16<double> { using type = double2; static constexpr int E = 2; };
 
 constexpr int MAX_CONES = 4;  // cones per knot point and per side held in the parameter block
 

@@ -18,24 +18,22 @@
 // Reference semantics: tiny_solve -> solve (admm.cpp:331-455); per-iteration order as in SURVEY A.2.
 // Scope: box constraints (admm.cpp:85-98).  Cones / hyperplanes run on the streamed lane-group kernel (gps_kernel.cuh).
 #pragma once
-#include <cuda/barrier>
+#include <algorithm>
+#include <cstdlib>
 
 #include "common.cuh"
-#include "launch.h"
+#include "lanegroup.cuh"
+#include "model_blob.h"
 
 namespace tmpc {
 
 template <int NX, int NU, int L, int ES>
-struct GpiCfg {
-    static constexpr int RX = (NX + L - 1) / L;
-    static constexpr int RU = (NU + L - 1) / L;
-    static constexpr int IPW = 32 / L;      // instances per warp
-    static constexpr int W = 16 / ES;       // elements per 16-byte shared-memory vector
+struct GpiCfg : LaneGeom<NX, NU, L, ES> {
+    using G = LaneGeom<NX, NU, L, ES>;
+    static constexpr int RX = G::RX, RU = G::RU, IPW = G::IPW, W = G::W, NXP = G::NXP, NUP = G::NUP;
     static constexpr int PV = RX + RU;      // values a lane owns per knot point (state rows, then input rows)
     static constexpr int PVP = (PV + W - 1) / W * W;
     static constexpr int NPV = PVP / W;     // vectors per pack
-    static constexpr int NXP = (L * RX + W - 1) / W * W;  // gather buffer width (state vectors)
-    static constexpr int NUP = (L * RU + W - 1) / W * W;  // gather buffer width (input vectors)
     static constexpr int GBUF1 = IPW * (NXP > NUP ? NXP : NUP);  // the gather buffer
     // registers needed for the per-lane matrix rows (in elements of T)
     static constexpr int MAT_REGS = RX * (2 * NX + 2 * NU + 3) + RU * (2 * NX + NU + 2);
@@ -64,72 +62,7 @@ __host__ __device__ constexpr bool gpi_feasible() {
     return Cfg::MAT_REGS * (int)(sizeof(T) / 4) <= 150;
 }
 
-template <typename T, int L>
-__device__ __forceinline__ T group_max(T v) {
-#pragma unroll
-    for (int m = L / 2; m >= 1; m >>= 1) {
-        T o = __shfl_xor_sync(0xffffffffu, v, m, L);
-        v = (o > v) ? o : v;
-    }
-    return v;
-}
-
 constexpr int GPI_MAX_WARPS = 8;
-
-// Shared-memory accessors on 32-bit shared-window addresses (no generic->shared conversion, no 64-bit
-// address arithmetic in the hot loops).  16-byte vector forms move a whole per-lane pack per instruction.
-__device__ __forceinline__ float lds(unsigned a, float) {
-    float v;
-    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
-    return v;
-}
-__device__ __forceinline__ double lds(unsigned a, double) {
-    double v;
-    asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(a));
-    return v;
-}
-__device__ __forceinline__ void sts(unsigned a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
-__device__ __forceinline__ void sts(unsigned a, double v) { asm volatile("st.shared.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
-__device__ __forceinline__ void ldsv(unsigned a, float (&v)[4]) {
-    asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "r"(a));
-}
-__device__ __forceinline__ void ldsv(unsigned a, double (&v)[2]) {
-    asm volatile("ld.shared.v2.f64 {%0,%1}, [%2];" : "=d"(v[0]), "=d"(v[1]) : "r"(a));
-}
-__device__ __forceinline__ void stsv(unsigned a, const float (&v)[4]) {
-    asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(a), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
-}
-__device__ __forceinline__ void stsv(unsigned a, const double (&v)[2]) {
-    asm volatile("st.shared.v2.f64 [%0], {%1,%2};" ::"r"(a), "d"(v[0]), "d"(v[1]) : "memory");
-}
-
-template <bool B>
-struct BoolTag {
-    static constexpr bool value = B;
-};
-template <int J>
-struct IntTag {
-    static constexpr int value = J;
-};
-
-// Box clamp.  STRICT keeps Eigen's compare-select form (differs from fmax/fmin only in the sign of a zero
-// result when a bound is a signed zero); FAST uses the single-instruction min/max.
-template <bool FAST, typename T>
-__device__ __forceinline__ T clamp_box(T v, T lo, T hi) {
-    if constexpr (FAST) {
-        return fmin(fmax(v, lo), hi);
-    } else {
-        return clamp_ref(v, lo, hi);
-    }
-}
-// max(m, |d|): identical to the oracle's (|d| > m) ? |d| : m  because m is never NaN and |d| >= +0
-__device__ __forceinline__ float absmax(float m, float d) { return fmaxf(m, fabsf(d)); }
-// fp64: the oracle's compare-select itself.  fmax(double) has no single instruction: DSETP.MAX + SEL + FSEL + a NaN-quieting
-// LOP3 + register moves, 7 instructions per use and 9 % of the streamed fp64 kernel's instruction count (ncu source view).
-__device__ __forceinline__ double absmax(double m, double d) {
-    const double a = fabs(d);
-    return (a > m) ? a : m;
-}
 
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
@@ -155,38 +88,13 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         else return P.rho;
     };
 
-    // ---- stage the cache blob (A, B, f, Qd, Rd, Kinf, Pinf, Quu, AmBKt, APf, BPf) into shared memory with
-    // one TMA bulk copy per CTA, then pull this lane's rows into registers.  The staging area aliases the
-    // first warp's state region and is dead before the solve starts.
-    constexpr int OFF_A = 0, OFF_B = OFF_A + NX * NX, OFF_F = OFF_B + NX * NU, OFF_QD = OFF_F + NX, OFF_RD = OFF_QD + NX,
-                  OFF_K = OFF_RD + NU, OFF_PINF = OFF_K + NU * NX, OFF_QUU = OFF_PINF + NX * NX,
-                  OFF_AMBKT = OFF_QUU + NU * NU, OFF_APF = OFF_AMBKT + NX * NX, OFF_BPF = OFF_APF + NX,
-                  BLOB = OFF_BPF + NU;
-    constexpr unsigned BLOB_BYTES = (unsigned)(((BLOB * sizeof(T) + 15) / 16) * 16);
+    // ---- stage the cache blob into shared memory with one TMA bulk copy per CTA, then pull this lane's rows into
+    // registers.  The staging area aliases the first warp's state region and is dead before the solve starts.
+    constexpr ModelBlob MB = model_blob(NX, NU);
+    constexpr unsigned BLOB_BYTES = (unsigned)cache_stage_bytes(NX, NU, sizeof(T));
     T *stage = reinterpret_cast<T *>(smem_raw);
     __shared__ __align__(8) unsigned long long mbar;
-    if (threadIdx.x == 0) {
-        const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mb));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(BLOB_BYTES) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                         (unsigned)__cvta_generic_to_shared(stage)),
-                     "l"(gmat), "r"(BLOB_BYTES), "r"(mb)
-                     : "memory");
-    }
-    __syncthreads();
-    {
-        const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
-        unsigned done = 0;
-        while (!done) {
-            asm volatile(
-                "{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n selp.u32 %0, 1, 0, p;\n}\n"
-                : "=r"(done)
-                : "r"(mb)
-                : "memory");
-        }
-    }
+    stage_blob(stage, gmat, BLOB_BYTES, &mbar);
 
     // per-lane matrix rows (registers)
     // stage-1 rows (dot with the gathered nx-vector): backward = [AmBKt rows ; B^T rows], forward = [A rows ; Kinf rows]
@@ -202,74 +110,71 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // Backward-sweep rows (AmBKt, B^T, Kinf^T, Quu_inv, APf, BPf and the cost weights Qd, Rd) and forward-sweep rows (A, Kinf,
     // B, f) load separately: fp64 re-reads the rows of a sweep when it starts (PS), everything else loads both once.
     auto load_bwd_rows = [&](const T *src) {
+        auto rd = [src](int e) { return src[e]; };
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1b[a][m] = xv[a] ? src[OFF_AMBKT + ii + NX * m] : T(0);
-#pragma unroll
-            for (int j = 0; j < NU; ++j) mKt[a][j] = xv[a] ? src[OFF_K + j + NU * ii] : T(0);  // Kinf^T(i,j) = Kinf(j,i)
-            vQd[a] = xv[a] ? src[OFF_QD + ii] : T(0);
-            vAPf[a] = xv[a] ? src[OFF_APF + ii] : T(0);
+            blob_row<NX, NX>(rd, MB.AmBKt, ii, xv[a], mS1b[a]);
+            blob_col<NU, NU>(rd, MB.Kinf, ii, xv[a], mKt[a]);
+            vQd[a] = xv[a] ? rd(MB.Qd + ii) : T(0);
+            vAPf[a] = xv[a] ? rd(MB.APf + ii) : T(0);
         }
 #pragma unroll
         for (int b = 0; b < RU; ++b) {
             const int jj = uv[b] ? l * RU + b : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1b[RX + b][m] = uv[b] ? src[OFF_B + m + NX * jj] : T(0);  // B^T(j,m) = B(m,j)
-#pragma unroll
-            for (int m = 0; m < NU; ++m) mQuu[b][m] = uv[b] ? src[OFF_QUU + jj + NU * m] : T(0);
-            vRd[b] = uv[b] ? src[OFF_RD + jj] : T(0);
-            vBPf[b] = uv[b] ? src[OFF_BPF + jj] : T(0);
+            blob_col<NX, NX>(rd, MB.B, jj, uv[b], mS1b[RX + b]);
+            blob_row<NU, NU>(rd, MB.Quu, jj, uv[b], mQuu[b]);
+            vRd[b] = uv[b] ? rd(MB.Rd + jj) : T(0);
+            vBPf[b] = uv[b] ? rd(MB.BPf + jj) : T(0);
         }
     };
     auto load_fwd_rows = [&](const T *src) {
+        auto rd = [src](int e) { return src[e]; };
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1f[a][m] = xv[a] ? src[OFF_A + ii + NX * m] : T(0);
-#pragma unroll
-            for (int j = 0; j < NU; ++j) mB[a][j] = xv[a] ? src[OFF_B + ii + NX * j] : T(0);
-            vf[a] = xv[a] ? src[OFF_F + ii] : T(0);
+            blob_row<NX, NX>(rd, MB.A, ii, xv[a], mS1f[a]);
+            blob_row<NX, NU>(rd, MB.B, ii, xv[a], mB[a]);
+            vf[a] = xv[a] ? rd(MB.f + ii) : T(0);
         }
 #pragma unroll
         for (int b = 0; b < RU; ++b) {
             const int jj = uv[b] ? l * RU + b : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1f[RX + b][m] = uv[b] ? src[OFF_K + jj + NU * m] : T(0);
+            blob_row<NU, NX>(rd, MB.Kinf, jj, uv[b], mS1f[RX + b]);
         }
     };
-    auto load_rows = [&](const T *src) {  // both sets at once (everything but fp64), in the order of the blob
+    // both sets at once (everything but fp64), row by row with the backward and forward matrices interleaved: the load
+    // order the kernel was tuned with (load_bwd_rows + load_fwd_rows compiles to a different schedule)
+    auto load_rows = [&](const T *src) {
+        auto rd = [src](int e) { return src[e]; };
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
 #pragma unroll
             for (int m = 0; m < NX; ++m) {
-                mS1b[a][m] = xv[a] ? src[OFF_AMBKT + ii + NX * m] : T(0);
-                mS1f[a][m] = xv[a] ? src[OFF_A + ii + NX * m] : T(0);
+                mS1b[a][m] = xv[a] ? rd(MB.AmBKt + ii + NX * m) : T(0);
+                mS1f[a][m] = xv[a] ? rd(MB.A + ii + NX * m) : T(0);
             }
 #pragma unroll
             for (int j = 0; j < NU; ++j) {
-                mKt[a][j] = xv[a] ? src[OFF_K + j + NU * ii] : T(0);  // Kinf^T(i,j) = Kinf(j,i)
-                mB[a][j] = xv[a] ? src[OFF_B + ii + NX * j] : T(0);
+                mKt[a][j] = xv[a] ? rd(MB.Kinf + j + NU * ii) : T(0);  // Kinf^T(i,j) = Kinf(j,i)
+                mB[a][j] = xv[a] ? rd(MB.B + ii + NX * j) : T(0);
             }
-            vQd[a] = xv[a] ? src[OFF_QD + ii] : T(0);
-            vAPf[a] = xv[a] ? src[OFF_APF + ii] : T(0);
-            vf[a] = xv[a] ? src[OFF_F + ii] : T(0);
+            vQd[a] = xv[a] ? rd(MB.Qd + ii) : T(0);
+            vAPf[a] = xv[a] ? rd(MB.APf + ii) : T(0);
+            vf[a] = xv[a] ? rd(MB.f + ii) : T(0);
         }
 #pragma unroll
         for (int b = 0; b < RU; ++b) {
             const int jj = uv[b] ? l * RU + b : 0;
 #pragma unroll
             for (int m = 0; m < NX; ++m) {
-                mS1b[RX + b][m] = uv[b] ? src[OFF_B + m + NX * jj] : T(0);  // B^T(j,m) = B(m,j)
-                mS1f[RX + b][m] = uv[b] ? src[OFF_K + jj + NU * m] : T(0);
+                mS1b[RX + b][m] = uv[b] ? rd(MB.B + m + NX * jj) : T(0);  // B^T(j,m) = B(m,j)
+                mS1f[RX + b][m] = uv[b] ? rd(MB.Kinf + jj + NU * m) : T(0);
             }
-#pragma unroll
-            for (int m = 0; m < NU; ++m) mQuu[b][m] = uv[b] ? src[OFF_QUU + jj + NU * m] : T(0);
-            vRd[b] = uv[b] ? src[OFF_RD + jj] : T(0);
-            vBPf[b] = uv[b] ? src[OFF_BPF + jj] : T(0);
+            blob_row<NU, NU>(rd, MB.Quu, jj, uv[b], mQuu[b]);
+            vRd[b] = uv[b] ? rd(MB.Rd + jj) : T(0);
+            vBPf[b] = uv[b] ? rd(MB.BPf + jj) : T(0);
         }
     };
     // where this lane's rows come from at a sweep start (PS): the staged blob, or its slot's own blob (heterogeneous batch)
@@ -358,20 +263,11 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     const bool cold = P.cold != 0;
     const bool tvb = P.bounds_tv != 0;
     const bool enx = P.en_state_bound != 0, enu = P.en_input_bound != 0;
+    auto xok = [&](int a) { return xv[a]; };
+    auto uok = [&](int b) { return uv[b]; };
     T loX[RX], hiX[RX], loU[RU], hiU[RU];  // bounds of this lane's rows (reloaded per k only if time-varying)
-    // a disabled bound (en_*_bound = 0) or a padding row is (-inf, +inf): the clamp is then the identity on every
-    // non-NaN value, so it can stay unconditional in the hot loop
+    box_bounds<true>(P, l, 0, true, enx, enu, xok, uok, loX, hiX, loU, hiU);
     const T kInf = (T)INFINITY;
-#pragma unroll
-    for (int a = 0; a < RX; ++a) {
-        loX[a] = (enx && xv[a]) ? __ldg(P.x_min + l * RX + a) : -kInf;
-        hiX[a] = (enx && xv[a]) ? __ldg(P.x_max + l * RX + a) : kInf;
-    }
-#pragma unroll
-    for (int b = 0; b < RU; ++b) {
-        loU[b] = (enu && uv[b]) ? __ldg(P.u_min + l * RU + b) : -kInf;
-        hiU[b] = (enu && uv[b]) ? __ldg(P.u_max + l * RU + b) : kInf;
-    }
     const bool keep_v = (P.s_v != nullptr) || (P.s_z != nullptr);
     // where element (k, row i) of instance-slot s lives inside a pack region
     auto idx_x = [&](int s, int k, int i) { return (k * 32 + s * L + i / RX) * PVP + (i % RX); };
@@ -449,20 +345,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 na[e] = pa[e];
                 nb[e] = pb[e];
             }
-            if (tvb) {
-#pragma unroll
-                for (int a = 0; a < RX; ++a) {
-                    loX[a] = (enx && xv[a]) ? __ldg(P.x_min + (int64_t)k * NX + l * RX + a) : loX[a];
-                    hiX[a] = (enx && xv[a]) ? __ldg(P.x_max + (int64_t)k * NX + l * RX + a) : hiX[a];
-                }
-                if (HASU) {
-#pragma unroll
-                    for (int b = 0; b < RU; ++b) {
-                        loU[b] = (enu && uv[b]) ? __ldg(P.u_min + (int64_t)k * NU + l * RU + b) : loU[b];
-                        hiU[b] = (enu && uv[b]) ? __ldg(P.u_max + (int64_t)k * NU + l * RU + b) : hiU[b];
-                    }
-                }
-            }
+            if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
             if constexpr (FAST) {
     #pragma unroll
                 for (int a = 0; a < RX; ++a) {  // vnew = clamp(x + g), g += x - vnew
@@ -747,13 +630,13 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             // heterogeneous batch: this instance has its own model / cache blob (same layout as the shared one, rho appended)
             const T *pinf = P.Pinf_g;
             if constexpr (HET) {
-                const T *mb = P.models + ib * (int64_t)(BLOB + 1);
+                const T *mb = P.models + ib * (int64_t)MB.model;
                 if constexpr (PS) rowsrc = mb;
                 else load_rows(mb);
-                rho_m = mb[BLOB];
-                pinf = mb + OFF_PINF;
+                rho_m = mb[MB.rho];
+                pinf = mb + MB.Pinf;
             }
-            // x0 (own rows) and the iteration-invariant part of the terminal cost: -(Pinf^T xref_{N-1})
+            // x0 (own rows) and the iteration-invariant part of the terminal cost
             T xr[NX];
             const T *xl = xrefp - l * RX + (int64_t)(N - 1) * NX;
 #pragma unroll
@@ -762,10 +645,8 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             for (int a = 0; a < RX; ++a) {
                 const int i = l * RX + a, ii = xv[a] ? i : 0;
                 x0o[a] = xv[a] ? __ldg(P.x0 + ib * NX + ii) : T(0);
-                T sacc = xr[0] * __ldg(pinf + 0 + NX * ii);
-#pragma unroll
-                for (int m = 1; m < NX; ++m) sacc = mac<FAST>(sacc, xr[m], __ldg(pinf + m + NX * ii));
-                pterm[a] = xv[a] ? -sacc : T(0);
+                const T pt = terminal_cost<FAST, NX>([&](int m) { return xr[m]; }, pinf, ii);
+                pterm[a] = xv[a] ? pt : T(0);
             }
         }
         __syncwarp();
@@ -998,11 +879,6 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
 // ---------------------------------------------------------------------------------------------------------
 // host side: configuration choice + launch
 // ---------------------------------------------------------------------------------------------------------
-struct GpiPlan {
-    int L = 0, warps = 0;
-    size_t smem = 0;
-};
-
 template <typename T, int NX, int NU, int L>
 inline void gpi_consider(int N, int max_smem, GpiPlan &best) {
     if constexpr (gpi_feasible<T, NX, NU, L>()) {
@@ -1010,8 +886,9 @@ inline void gpi_consider(int N, int max_smem, GpiPlan &best) {
         const size_t per_warp = Cfg::warp_elems(N) * sizeof(T);
         // fp32: the TMA staging area aliases the start of the state region (the allocation is at least as large as the blob);
         // fp64: the blob stays resident in front of the state regions (matrix rows are re-read at every sweep start)
-        const size_t blob = ((size_t)(3 * NX * NX + 2 * NX * NU + NU * NU + 4 * NX + 2 * NU) * sizeof(T) + 15) / 16 * 16 + 64;
-        const size_t keep = gpi_per_sweep_rows<T>() ? ((size_t)(3 * NX * NX + 2 * NX * NU + NU * NU + 4 * NX + 2 * NU) * sizeof(T) + 15) / 16 * 16 : 0;
+        const size_t reserve = cache_reserve_bytes(NX, NU, sizeof(T));
+        const size_t blob = reserve + 64;
+        const size_t keep = gpi_per_sweep_rows<T>() ? reserve : 0;
         if ((size_t)max_smem < keep + per_warp) return;
         const int w = (int)std::min<size_t>(GPI_MAX_WARPS, ((size_t)max_smem - keep) / per_warp);
         if (w < 1 || blob > (size_t)max_smem) return;
@@ -1022,6 +899,8 @@ inline void gpi_consider(int N, int max_smem, GpiPlan &best) {
             best.L = L;
             best.warps = w;
             best.smem = std::max(keep + per_warp * (size_t)w, blob);
+            best.instances_per_cta = w * Cfg::IPW;
+            best.vscratch_per_instance = (size_t)N * L * Cfg::PVP * sizeof(T);
         }
     }
 }
@@ -1047,17 +926,11 @@ inline GpiPlan gpi_plan(int N, int max_smem) {
     return p;
 }
 
-template <typename T, int NX, int NU>
-inline int gpi_fit_T(int N, int max_smem) {
-    return (int)gpi_plan<T, NX, NU>(N, max_smem).smem;
-}
-
 template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool MM = false>
 int launch_gpi_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P, const T *gmat) {
     if constexpr (gpi_feasible<T, NX, NU, L>()) {
         auto kern = gpi_solve_kernel<T, NX, NU, L, FAST, HET, MM>;
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem) != cudaSuccess)
-            return TINYMPC_ERR_CUDA;
+        if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
         const int64_t ngroups = (d->io.B + (32 / L) - 1) / (32 / L);
         // ngroups = warps the batch fills.  A batch smaller than one wave is spread over all SMs with fewer warps per CTA
         // (the kernel's carve-up is per warp, any block size up to plan.warps works): the latency of a solve is set by how
@@ -1067,12 +940,7 @@ int launch_gpi_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P
         const int64_t want = (ngroups + warps - 1) / warps;
         const int ctas = (int)std::max<int64_t>(1, std::min<int64_t>(d->sm_count, want));
         kern<<<ctas, warps * 32, plan.smem, d->stream>>>(P, gmat, (unsigned long long *)d->work_queue);
-        d->out_threads = warps * 32;
-        d->out_ctas = ctas;
-        d->out_smem = (int)plan.smem;
-        d->out_lanes_per_instance = L;
-        d->out_instances_per_cta = plan.warps * (32 / L);
-        return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
+        return launch_done(d, warps * 32, ctas, plan.smem, L, plan.instances_per_cta);
     } else {
         return TINYMPC_ERR_UNSUPPORTED;
     }

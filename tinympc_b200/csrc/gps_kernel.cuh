@@ -31,8 +31,12 @@
 // The kernel is persistent (one CTA per SM); slots are refilled from a global atomic queue as instances terminate
 // (per-instance termination, admm.cpp:310-328).  Reference semantics: tiny_solve -> solve (admm.cpp:331-455).
 #pragma once
-#include "tpi_kernel.cuh"
-#include "gpi_kernel.cuh"
+#include <algorithm>
+#include <cstdlib>
+
+#include "common.cuh"
+#include "lanegroup.cuh"
+#include "model_blob.h"
 
 namespace tmpc {
 
@@ -40,14 +44,10 @@ __host__ __device__ constexpr int gps_gcd(int a, int b) { return b == 0 ? a : gp
 __host__ __device__ constexpr int gps_popc(int m) { return (m & 1) + ((m >> 1) & 1) + ((m >> 2) & 1); }
 
 template <int NX, int NU, int L, int ES, int NI, int FAM>
-struct GpsCfg {
-    static constexpr int RX = (NX + L - 1) / L;
-    static constexpr int RU = (NU + L - 1) / L;
-    static constexpr int IPW = 32 / L;    // lane groups per warp
+struct GpsCfg : LaneGeom<NX, NU, L, ES> {
+    using G = LaneGeom<NX, NU, L, ES>;
+    static constexpr int RX = G::RX, RU = G::RU, IPW = G::IPW, W = G::W, NXP = G::NXP, NUP = G::NUP;
     static constexpr int SPW = IPW * NI;  // instances (slots) per warp; slot index = j * IPW + group
-    static constexpr int W = 16 / ES;
-    static constexpr int NXP = (L * RX + W - 1) / W * W;
-    static constexpr int NUP = (L * RU + W - 1) / W * W;
     static constexpr int GBX = SPW * NXP, GBU = SPW * NUP;  // gather scratch (elements): state vectors, input vectors
     // chunk sizes (bytes) of a lane's piece: global side (limited by the row pitch of an instance) and shared side
     static constexpr int CX = gps_gcd(16, gps_gcd(NX * ES, RX * ES));
@@ -161,27 +161,8 @@ __device__ __forceinline__ void prefetch_l2(const void *p, unsigned pr) {
     asm volatile("{\n .reg .pred q;\n setp.ne.u32 q, %1, 0;\n @q prefetch.global.L2 [%0];\n}" ::"l"(p), "r"(pr));
 }
 
-// ---- chunked piece moves between registers and shared / global memory ----
-__device__ __forceinline__ void lds_chunk(unsigned a, float (&v)[1]) { v[0] = lds(a, 0.f); }
-__device__ __forceinline__ void lds_chunk(unsigned a, float (&v)[2]) {
-    asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(v[0]), "=f"(v[1]) : "r"(a));
-}
-__device__ __forceinline__ void lds_chunk(unsigned a, float (&v)[4]) { ldsv(a, v); }
-__device__ __forceinline__ void lds_chunk(unsigned a, double (&v)[1]) { v[0] = lds(a, 0.0); }
-__device__ __forceinline__ void lds_chunk(unsigned a, double (&v)[2]) { ldsv(a, v); }
-__device__ __forceinline__ void sts_chunk(unsigned a, const float (&v)[1]) { sts(a, v[0]); }
-__device__ __forceinline__ void sts_chunk(unsigned a, const float (&v)[2]) {
-    asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(a), "f"(v[0]), "f"(v[1]) : "memory");
-}
-__device__ __forceinline__ void sts_chunk(unsigned a, const float (&v)[4]) { stsv(a, v); }
-__device__ __forceinline__ void sts_chunk(unsigned a, const double (&v)[1]) { sts(a, v[0]); }
-__device__ __forceinline__ void sts_chunk(unsigned a, const double (&v)[2]) { stsv(a, v); }
-__device__ __forceinline__ void stg_chunk(float *p, const float (&v)[1]) { *p = v[0]; }
-__device__ __forceinline__ void stg_chunk(float *p, const float (&v)[2]) { *reinterpret_cast<float2 *>(p) = make_float2(v[0], v[1]); }
-__device__ __forceinline__ void stg_chunk(float *p, const float (&v)[4]) { *reinterpret_cast<float4 *>(p) = make_float4(v[0], v[1], v[2], v[3]); }
-__device__ __forceinline__ void stg_chunk(double *p, const double (&v)[1]) { *p = v[0]; }
-__device__ __forceinline__ void stg_chunk(double *p, const double (&v)[2]) { *reinterpret_cast<double2 *>(p) = make_double2(v[0], v[1]); }
-// predicated stores: one PTX predicate instead of a branch around the store (lanes that own only padding rows skip theirs)
+// ---- chunked piece stores to global memory, predicated: one PTX predicate instead of a branch around the store (lanes
+// that own only padding rows skip theirs) ----
 __device__ __forceinline__ void stg_chunk(float *p, const float (&v)[1], unsigned pr) {
     asm volatile("{\n .reg .pred q;\n setp.ne.u32 q, %2, 0;\n @q st.global.f32 [%0], %1;\n}" ::"l"(p), "f"(v[0]), "r"(pr) : "memory");
 }
@@ -201,39 +182,6 @@ __device__ __forceinline__ void stg_chunk(double *p, const double (&v)[2], unsig
 }
 
 template <typename T, int R, int CB>
-__device__ __forceinline__ void lds_piece(unsigned a, T (&v)[R]) {
-    constexpr int E = CB / (int)sizeof(T);
-#pragma unroll
-    for (int c = 0; c < R / E; ++c) {
-        T t[E];
-        lds_chunk(a + (unsigned)(c * CB), t);
-#pragma unroll
-        for (int e = 0; e < E; ++e) v[c * E + e] = t[e];
-    }
-}
-template <typename T, int R, int CB>
-__device__ __forceinline__ void sts_piece(unsigned a, const T (&v)[R]) {
-    constexpr int E = CB / (int)sizeof(T);
-#pragma unroll
-    for (int c = 0; c < R / E; ++c) {
-        T t[E];
-#pragma unroll
-        for (int e = 0; e < E; ++e) t[e] = v[c * E + e];
-        sts_chunk(a + (unsigned)(c * CB), t);
-    }
-}
-template <typename T, int R, int CB>
-__device__ __forceinline__ void stg_piece(T *p, const T (&v)[R]) {
-    constexpr int E = CB / (int)sizeof(T);
-#pragma unroll
-    for (int c = 0; c < R / E; ++c) {
-        T t[E];
-#pragma unroll
-        for (int e = 0; e < E; ++e) t[e] = v[c * E + e];
-        stg_chunk(p + c * E, t);
-    }
-}
-template <typename T, int R, int CB>
 __device__ __forceinline__ void stg_piece(T *p, const T (&v)[R], unsigned pr) {
     constexpr int E = CB / (int)sizeof(T);
 #pragma unroll
@@ -244,24 +192,6 @@ __device__ __forceinline__ void stg_piece(T *p, const T (&v)[R], unsigned pr) {
         stg_chunk(p + c * E, t, pr);
     }
 }
-
-// own rows of a vector every lane of the group holds in full: out[a] = full[l*R + a] without dynamic register indexing
-template <typename T, int NE, int R, int L>
-__device__ __forceinline__ void extract_own(const T (&full)[NE], int l, T (&out)[R]) {
-#pragma unroll
-    for (int a = 0; a < R; ++a) {
-        T v = T(0);
-#pragma unroll
-        for (int g = 0; g < L; ++g)
-            if (g * R + a < NE) v = (l == g) ? full[g * R + a] : v;
-        out[a] = v;
-    }
-}
-
-template <int J>
-struct IdxTag {
-    static constexpr int value = J;
-};
 
 template <typename T, int NX, int NU, int L, int NI, int FAM, bool FAST>
 __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
@@ -285,35 +215,11 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     const T rho = P.rho;
 
     // ---- stage the cache blob into shared memory with one TMA bulk copy per CTA, pull this lane's rows into registers
-    constexpr int OFF_A = 0, OFF_B = OFF_A + NX * NX, OFF_F = OFF_B + NX * NU, OFF_QD = OFF_F + NX, OFF_RD = OFF_QD + NX,
-                  OFF_K = OFF_RD + NU, OFF_PINF = OFF_K + NU * NX, OFF_QUU = OFF_PINF + NX * NX,
-                  OFF_AMBKT = OFF_QUU + NU * NU, OFF_APF = OFF_AMBKT + NX * NX, OFF_BPF = OFF_APF + NX,
-                  BLOB = OFF_BPF + NU;
-    constexpr unsigned BLOB_BYTES = (unsigned)(((BLOB * sizeof(T) + 15) / 16) * 16);
+    constexpr ModelBlob MB = model_blob(NX, NU);
+    constexpr unsigned BLOB_BYTES = (unsigned)cache_stage_bytes(NX, NU, sizeof(T));
     T *stage = reinterpret_cast<T *>(smem_raw);
     __shared__ __align__(8) unsigned long long mbar;
-    if (threadIdx.x == 0) {
-        const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mb));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mb), "r"(BLOB_BYTES) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                         (unsigned)__cvta_generic_to_shared(stage)),
-                     "l"(gmat), "r"(BLOB_BYTES), "r"(mb)
-                     : "memory");
-    }
-    __syncthreads();
-    {
-        const unsigned mb = (unsigned)__cvta_generic_to_shared(&mbar);
-        unsigned done = 0;
-        while (!done) {
-            asm volatile(
-                "{\n .reg .pred p;\n mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n selp.u32 %0, 1, 0, p;\n}\n"
-                : "=r"(done)
-                : "r"(mb)
-                : "memory");
-        }
-    }
+    stage_blob(stage, gmat, BLOB_BYTES, &mbar);
     const bool xvl = l * RX < NX, uvl = l * RU < NU;  // does this lane own real rows (else padding rows: zeros)
     const unsigned pxv = xvl ? 1u : 0u, puv = uvl ? 1u : 0u;  // the same as PTX predicate sources (predicated copies / stores)
     // The staged blob stays in shared memory for the whole kernel.  A sweep only needs half of the matrices (forward:
@@ -326,39 +232,32 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xvl ? l * RX + a : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1f[a][m] = xvl ? bl(OFF_A + ii + NX * m) : T(0);
-#pragma unroll
-            for (int j = 0; j < NU; ++j) mB[a][j] = xvl ? bl(OFF_B + ii + NX * j) : T(0);
-            vQd[a] = xvl ? bl(OFF_QD + ii) : T(0);
-            vf[a] = xvl ? bl(OFF_F + ii) : T(0);
+            blob_row<NX, NX>(bl, MB.A, ii, xvl, mS1f[a]);
+            blob_row<NX, NU>(bl, MB.B, ii, xvl, mB[a]);
+            vQd[a] = xvl ? bl(MB.Qd + ii) : T(0);
+            vf[a] = xvl ? bl(MB.f + ii) : T(0);
         }
 #pragma unroll
         for (int b = 0; b < RU; ++b) {
             const int jj = uvl ? l * RU + b : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1f[RX + b][m] = uvl ? bl(OFF_K + jj + NU * m) : T(0);
-            vRd[b] = uvl ? bl(OFF_RD + jj) : T(0);
+            blob_row<NU, NX>(bl, MB.Kinf, jj, uvl, mS1f[RX + b]);
+            vRd[b] = uvl ? bl(MB.Rd + jj) : T(0);
         }
     };
     auto load_bwd_rows = [&](T (&mS1b)[RX + RU][NX], T (&mKt)[RX][NU], T (&mQuu)[RU][NU], T (&vAPf)[RX], T (&vBPf)[RU]) {
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xvl ? l * RX + a : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1b[a][m] = xvl ? bl(OFF_AMBKT + ii + NX * m) : T(0);
-#pragma unroll
-            for (int j = 0; j < NU; ++j) mKt[a][j] = xvl ? bl(OFF_K + j + NU * ii) : T(0);  // Kinf^T(i,j) = Kinf(j,i)
-            vAPf[a] = xvl ? bl(OFF_APF + ii) : T(0);
+            blob_row<NX, NX>(bl, MB.AmBKt, ii, xvl, mS1b[a]);
+            blob_col<NU, NU>(bl, MB.Kinf, ii, xvl, mKt[a]);
+            vAPf[a] = xvl ? bl(MB.APf + ii) : T(0);
         }
 #pragma unroll
         for (int b = 0; b < RU; ++b) {
             const int jj = uvl ? l * RU + b : 0;
-#pragma unroll
-            for (int m = 0; m < NX; ++m) mS1b[RX + b][m] = uvl ? bl(OFF_B + m + NX * jj) : T(0);  // B^T(j,m) = B(m,j)
-#pragma unroll
-            for (int m = 0; m < NU; ++m) mQuu[b][m] = uvl ? bl(OFF_QUU + jj + NU * m) : T(0);
-            vBPf[b] = uvl ? bl(OFF_BPF + jj) : T(0);
+            blob_col<NX, NX>(bl, MB.B, jj, uvl, mS1b[RX + b]);
+            blob_row<NU, NU>(bl, MB.Quu, jj, uvl, mQuu[b]);
+            vBPf[b] = uvl ? bl(MB.BPf + jj) : T(0);
         }
     };
 
@@ -378,8 +277,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
         asm volatile("st.shared.v4.f32 [%0], {%1,%1,%1,%1};" ::"r"(aZero + o), "f"(0.f) : "memory");
     if (lane == 0) {
 #pragma unroll
-        for (int b = 0; b < RING::NBAR; ++b) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(aBar + 8u * b));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int b = 0; b < RING::NBAR; ++b) mbar_init(aBar + 8u * b);
+        mbar_init_fence();
     }
     __syncthreads();
     unsigned phase = 0;  // bit b = parity the next wait on barrier b expects (warp-uniform)
@@ -407,7 +306,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     // the records are written with ordinary stores (all lanes) and read back by bulk copies (async proxy): every lane orders
     // its stores before later async-proxy operations, the warp converges, then lane 0 may issue copies
     auto sweep_fence = [&]() {
-        asm volatile("fence.proxy.async.global;" ::: "memory");
+        fence_proxy_async_global();
         __syncwarp();
     };
     // gather scratch of instance j of this lane's group (slot j*IPW + grp): own rows / whole vector
@@ -465,18 +364,11 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     const bool cold = P.cold != 0;
     const bool tvb = P.bounds_tv != 0;
     const bool enx = P.en_state_bound != 0, enu = P.en_input_bound != 0;
-    const T kInf = (T)INFINITY;
+    // a lane owns all of its rows or none (NX % RX == 0, NU % RU == 0)
+    auto xok = [&](int) { return xvl; };
+    auto uok = [&](int) { return uvl; };
     T loX[RX], hiX[RX], loU[RU], hiU[RU];
-#pragma unroll
-    for (int a = 0; a < RX; ++a) {
-        loX[a] = (enx && xvl) ? __ldg(P.x_min + l * RX + a) : -kInf;
-        hiX[a] = (enx && xvl) ? __ldg(P.x_max + l * RX + a) : kInf;
-    }
-#pragma unroll
-    for (int b = 0; b < RU; ++b) {
-        loU[b] = (enu && uvl) ? __ldg(P.u_min + l * RU + b) : -kInf;
-        hiU[b] = (enu && uvl) ? __ldg(P.u_max + l * RU + b) : kInf;
-    }
+    box_bounds<true>(P, l, 0, true, enx, enu, xok, uok, loX, hiX, loU, hiU);
     const bool keep_v = has_b && (P.s_v != nullptr || P.s_z != nullptr);
     // family slacks are kept (region B) when the caller wants them back
     const bool keep_f[3] = {has_b && (P.s_vcnew || P.s_zcnew), has_b && (P.s_vlnew || P.s_zlnew), has_b && (P.s_vlnew_tv || P.s_zlnew_tv)};
@@ -708,20 +600,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                     for (int b = 0; b < RU; ++b) u[j][b] = (-t1[j][RX + b]) - dk[j][b];  // u_k = -(Kinf x_k) - d_k
                 gather_u(u, Uf);
             }
-            if (tvb) {
-#pragma unroll
-                for (int a = 0; a < RX; ++a) {
-                    loX[a] = (enx && xvl) ? __ldg(P.x_min + (int64_t)k * NX + l * RX + a) : loX[a];
-                    hiX[a] = (enx && xvl) ? __ldg(P.x_max + (int64_t)k * NX + l * RX + a) : hiX[a];
-                }
-                if (HASU) {
-#pragma unroll
-                    for (int b = 0; b < RU; ++b) {
-                        loU[b] = (enu && uvl) ? __ldg(P.u_min + (int64_t)k * NU + l * RU + b) : loU[b];
-                        hiU[b] = (enu && uvl) ? __ldg(P.u_max + (int64_t)k * NU + l * RU + b) : hiU[b];
-                    }
-                }
-            }
+            if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
             // ---- box constraints: state column k and input column k ----
             T q[NI][RX], r[NI][RU];
 #pragma unroll
@@ -810,8 +689,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                 }
             }
             // ---- hyperplanes (families 1, 2) ----
-            if constexpr ((FAM & 2) != 0) planes_family(IdxTag<1>{}, k, HASU, bx, bu, cx, cu, xo, u, q, r);
-            if constexpr ((FAM & 4) != 0) planes_family(IdxTag<2>{}, k, HASU, bx, bu, cx, cu, xo, u, q, r);
+            if constexpr ((FAM & 2) != 0) planes_family(IntTag<1>{}, k, HASU, bx, bu, cx, cu, xo, u, q, r);
+            if constexpr ((FAM & 4) != 0) planes_family(IntTag<2>{}, k, HASU, bx, bu, cx, cu, xo, u, q, r);
 #pragma unroll
             for (int j = 0; j < NI; ++j) {
                 stg_piece<T, RX, CX>(cx + REC::q + j * JX, q[j], pxv);
@@ -922,12 +801,10 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             const T v_in = (!cold && P.s_v) ? P.s_v[ox + e] : T(0);
             T acc;
             if (k < N - 1) {
-                acc = -(__ldg(xrefb + e) * __ldg(gmat + OFF_QD + i));
+                acc = -(__ldg(xrefb + e) * __ldg(gmat + MB.Qd + i));
             } else {  // -(Pinf^T xref_{N-1})(i), m ascending
                 const T *xl = xrefb + (int64_t)(N - 1) * NX;
-                T sacc = __ldg(xl) * __ldg(gmat + OFF_PINF + NX * i);
-                for (int m = 1; m < NX; ++m) sacc = mac<FAST>(sacc, __ldg(xl + m), __ldg(gmat + OFF_PINF + m + NX * i));
-                acc = -sacc;
+                acc = terminal_cost<FAST, NX>([&](int m) { return __ldg(xl + m); }, gmat + MB.Pinf, i);
             }
             acc = nmac<FAST>(acc, rho, vnew_in - g_in);
             T *r_ = wsw + (int64_t)k * recA + sidx * NX + i;
@@ -954,7 +831,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             const T y_in = (!cold && P.s_y) ? P.s_y[ou + e] : T(0);
             const T z_in = (!cold && P.s_z) ? P.s_z[ou + e] : T(0);
             const T ur = has_uref ? __ldg(urefb + e) : T(0);
-            T acc = nmac<FAST>(-(ur * __ldg(gmat + OFF_RD + j)), rho, znew_in - y_in);
+            T acc = nmac<FAST>(-(ur * __ldg(gmat + MB.Rd + j)), rho, znew_in - y_in);
             T *r_ = wsw + (int64_t)k * recA + sidx * NU + j;
             T *rb_ = wsb + (int64_t)k * recB + sidx * NU + j;
             r_[REC::znew] = z_in;
@@ -984,9 +861,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             for (int a = 0; a < RX; ++a) {
                 const int ii = xvl ? l * RX + a : 0;
                 x0v[a] = xvl ? __ldg(P.x0 + ib * NX + ii) : T(0);
-                T sacc = __ldg(xl) * __ldg(gmat + OFF_PINF + NX * ii);
-                for (int m = 1; m < NX; ++m) sacc = mac<FAST>(sacc, __ldg(xl + m), __ldg(gmat + OFF_PINF + m + NX * ii));
-                ptv[a] = xvl ? -sacc : T(0);
+                const T pt = terminal_cost<FAST, NX>([&](int m) { return __ldg(xl + m); }, gmat + MB.Pinf, ii);
+                ptv[a] = xvl ? pt : T(0);
             }
             sts_piece<T, RX, SX>(aPark + (unsigned)((2 * J) * RX) * ES, x0v);
             sts_piece<T, RX, SX>(aPark + (unsigned)((2 * J + 1) * RX) * ES, ptv);
@@ -1142,8 +1018,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     // ---- persistent loop (same protocol as the on-chip kernel): retire / refill slots, then iterate until some
     // slot terminates; the iteration loop has warp-uniform control flow only ----
     for (;;) {
-        service(IdxTag<0>{});
-        if constexpr (NI > 1) service(IdxTag<1>{});
+        service(IntTag<0>{});
+        if constexpr (NI > 1) service(IntTag<1>{});
         bool anyb = false, over = false;
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
@@ -1208,7 +1084,7 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     // region B: previous box slacks (work->v / work->z) and family slacks, only when the caller wants them back
     p.ly.has_b = (s.v || s.z || s.vcnew || s.zcnew || s.vlnew || s.zlnew || s.vlnew_tv || s.zlnew_tv) ? 1 : 0;
     const int max_smem = d.max_smem_optin - 64;
-    const size_t blob = ((size_t)(3 * NX * NX + 2 * NX * NU + NU * NU + 4 * NX + 2 * NU) * sizeof(T) + 15) / 16 * 16;
+    const size_t blob = cache_reserve_bytes(NX, NU, sizeof(T));
     using RINGH = GpsRing<NX, NU, L, (int)sizeof(T), NI, FAM>;
     const size_t per_warp = RINGH::WARP_BYTES, fixed = blob + RINGH::ZERO_BYTES;
     if (fixed + per_warp > (size_t)max_smem) return p;
@@ -1238,14 +1114,9 @@ int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     P.gps = plan.ly;
     P.gps_ws = (T *)d->gps_ws;
     auto kern = gps_solve_kernel<T, NX, NU, L, NI, FAM, FAST>;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)plan.smem) != cudaSuccess) return TINYMPC_ERR_CUDA;
+    if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
     kern<<<plan.ctas, plan.warps * 32, plan.smem, d->stream>>>(P, (const T *)d->gmat, (unsigned long long *)d->work_queue);
-    d->out_threads = plan.warps * 32;
-    d->out_ctas = plan.ctas;
-    d->out_smem = (int)plan.smem;
-    d->out_lanes_per_instance = L;
-    d->out_instances_per_cta = plan.warps * (32 / L) * NI;
-    return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
+    return launch_done(d, plan.warps * 32, plan.ctas, plan.smem, L, plan.warps * (32 / L) * NI);
 }
 
 // family mask of the kernel that serves a feature set: 0 box only, 1 cones only, 6 hyperplanes only, 7 anything else

@@ -21,8 +21,7 @@
 
 // cross-part entry points of this dimension pair
 extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d);
-extern "C" int TM_SYM(tm_gpi_fit_)(int dtype, int N, int max_smem_optin);
-extern "C" int TM_SYM(tm_gpi_ipc_)(int dtype, int N, int max_smem_optin);
+extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin);
 extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d);
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype);
 
@@ -42,12 +41,7 @@ int launch_tpi(LaunchDesc *d) {
     const int64_t blocks = (d->io.B + threads - 1) / threads;
     if (blocks <= 0) return TINYMPC_OK;
     tpi_solve_kernel<T, TM_NX, TM_NU, FAST, EXT><<<(unsigned)blocks, threads, 0, d->stream>>>(P);
-    d->out_threads = threads;
-    d->out_ctas = (int)blocks;
-    d->out_smem = 0;
-    d->out_lanes_per_instance = 1;
-    d->out_instances_per_cta = threads;
-    return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
+    return launch_done(d, threads, (int)blocks, 0, 1, threads);
 }
 
 template <typename T>
@@ -81,8 +75,7 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
     static const tmpc::DimEntry e = {TM_NX,
                                      TM_NU,
                                      &tmpc::launch,
-                                     &TM_SYM(tm_gpi_fit_),
-                                     &TM_SYM(tm_gpi_ipc_),
+                                     &TM_SYM(tm_gpi_plan_),
                                      &tmpc::precompute_batch,
                                      &TM_SYM(tm_gps_lanes_)};
     return &e;
@@ -90,7 +83,6 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
 
 #elif TM_PART == 1
 // =========================================================================================================
-#include "tpi_kernel.cuh"  // Vec16
 #include "gpi_kernel.cuh"
 
 namespace tmpc {
@@ -141,21 +133,10 @@ extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d) {
     if (d->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
     return TINYMPC_ERR_ARG;
 }
-extern "C" int TM_SYM(tm_gpi_fit_)(int dtype, int N, int max_smem_optin) {
-    if (dtype == TINYMPC_F32) return tmpc::gpi_fit_T<float, TM_NX, TM_NU>(N, max_smem_optin - 64);
-    if (dtype == TINYMPC_F64) return tmpc::gpi_fit_T<double, TM_NX, TM_NU>(N, max_smem_optin - 64);
-    return 0;
-}
-extern "C" int TM_SYM(tm_gpi_ipc_)(int dtype, int N, int max_smem_optin) {
-    if (dtype == TINYMPC_F32) {
-        const tmpc::GpiPlan p = tmpc::gpi_plan<float, TM_NX, TM_NU>(N, max_smem_optin - 64);
-        return p.L ? ((p.warps << 16) | (p.warps * (32 / p.L))) : 0;
-    }
-    if (dtype == TINYMPC_F64) {
-        const tmpc::GpiPlan p = tmpc::gpi_plan<double, TM_NX, TM_NU>(N, max_smem_optin - 64);
-        return p.L ? ((p.warps << 16) | (p.warps * (32 / p.L))) : 0;
-    }
-    return 0;
+extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin) {
+    if (dtype == TINYMPC_F32) return tmpc::gpi_plan<float, TM_NX, TM_NU>(N, max_smem_optin - 64);
+    if (dtype == TINYMPC_F64) return tmpc::gpi_plan<double, TM_NX, TM_NU>(N, max_smem_optin - 64);
+    return tmpc::GpiPlan{};
 }
 
 #else
@@ -184,16 +165,12 @@ extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d) {
 // lanes per instance of the streamed lane-group kernel for this shape (0 = not available)
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype) {
     // lanes per instance in bits 0-7, instances per lane group (1 or 2) in bits 8-15
-    if (dtype == TINYMPC_F32) {
-        constexpr int Lf = tmpc::gps_pick_L<float, TM_NX, TM_NU>();
-        if constexpr (Lf == 0) return 0;
-        else return Lf | (tmpc::gps_pick_NI<float, TM_NX, TM_NU, Lf>() << 8);
-    }
-    if (dtype == TINYMPC_F64) {
-        constexpr int Ld = tmpc::gps_pick_L<double, TM_NX, TM_NU>();
-        if constexpr (Ld == 0) return 0;
-        else return Ld | (tmpc::gps_pick_NI<double, TM_NX, TM_NU, Ld>() << 8);
-    }
-    return 0;
+    auto lanes = [](auto t) {
+        using T = decltype(t);
+        constexpr int L = tmpc::gps_pick_L<T, TM_NX, TM_NU>();
+        if constexpr (L == 0) return 0;
+        else return L | (tmpc::gps_pick_NI<T, TM_NX, TM_NU, L>() << 8);
+    };
+    return dtype == TINYMPC_F32 ? lanes(0.f) : (dtype == TINYMPC_F64 ? lanes(0.0) : 0);
 }
 #endif

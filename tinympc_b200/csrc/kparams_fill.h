@@ -5,6 +5,7 @@
 
 #include "common.cuh"
 #include "launch.h"
+#include "model_blob.h"
 
 namespace tmpc {
 
@@ -55,7 +56,7 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
             P.uhi[j] = (d.en_input_bound && d.h_uhi) ? ((const T *)d.h_uhi)[j] : inf;
         }
     }
-    P.Pinf_g = d.gmat ? (const T *)d.gmat + (NX * NX + NX * NU + NX + NX + NU + NU * NX) : nullptr;
+    P.Pinf_g = d.gmat ? (const T *)d.gmat + model_blob(NX, NU).Pinf : nullptr;
     P.xref_pi = io.xref_per_instance;
     P.uref_pi = io.uref_per_instance;
     P.x0 = (const T *)io.x0; P.Xref = (const T *)io.Xref; P.Uref = (const T *)io.Uref;

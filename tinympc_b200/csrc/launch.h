@@ -2,6 +2,7 @@
 // kernel translation units (kernels_inst.cu compiled once per supported dimension pair).
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #include "../../include/tinympc_b200.h"
@@ -50,19 +51,39 @@ struct LaunchDesc {
     size_t out_ws_need;  // GPS: workspace bytes this launch needs (set when the launcher returns TM_ERR_WORKSPACE)
 };
 
+// launch epilogue of every kernel family: record the launch geometry in the descriptor, return the launch status
+inline int launch_done(LaunchDesc *d, int threads, int ctas, size_t smem, int lanes, int instances_per_cta) {
+    d->out_threads = threads;
+    d->out_ctas = ctas;
+    d->out_smem = (int)smem;
+    d->out_lanes_per_instance = lanes;
+    d->out_instances_per_cta = instances_per_cta;
+    return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
+}
+template <typename K>
+inline bool set_dynamic_smem(K kern, size_t smem) {
+    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess;
+}
+
 // internal: the launcher needs a larger gps_ws (size in out_ws_need); never leaves the library
 constexpr int TM_ERR_WORKSPACE = -100;
 
 // per-(nx,nu) entry: returns 0 on success, TINYMPC_ERR_UNSUPPORTED when (dtype,family,...) is not compiled
 typedef int (*launch_fn)(LaunchDesc *);
 
+// launch plan of the on-chip lane-group kernel (gpi_kernel.cuh: gpi_plan) for one (dtype, N); L == 0: not available
+struct GpiPlan {
+    int L = 0, warps = 0;              // lanes per instance, warps per CTA
+    size_t smem = 0;                   // dynamic shared memory per CTA (bytes)
+    int instances_per_cta = 0;         // instances resident per CTA (warps * 32 / L)
+    size_t vscratch_per_instance = 0;  // bytes of work->v / work->z scratch per instance (launch.h: gpi_vscratch)
+};
+
 struct DimEntry {
     int nx, nu;
     launch_fn launch;
-    // GPI capability query: shared-memory bytes per CTA for a given (dtype, N) or 0 if GPI not available
-    int (*gpi_fit)(int dtype, int N, int max_smem_optin);
-    // GPI plan for (dtype, N): (warps per CTA << 16) | instances resident per CTA; 0 if GPI is not available
-    int (*gpi_instances_per_cta)(int dtype, int N, int max_smem_optin);
+    // GPI capability query: the on-chip kernel's launch plan for (dtype, N)
+    GpiPlan (*gpi_plan)(int dtype, int N, int max_smem_optin);
     // batched cache precompute on the device (precompute_kernel.cuh): device pointers, one model blob per instance
     int (*precompute_batch)(int dtype, int64_t B, const void *A, const void *Bm, const void *f, const void *Qdiag, const void *Rdiag,
                             const void *rho, void *models_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);

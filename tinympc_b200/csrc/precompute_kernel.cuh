@@ -17,6 +17,7 @@
 // each product; the matrices live in shared memory (≈ 6 nx² + 6 nx·nu + 3 nu² elements per warp).
 #pragma once
 #include "common.cuh"
+#include "model_blob.h"
 
 namespace tmpc {
 
@@ -110,12 +111,12 @@ __global__ void __launch_bounds__(PC_WARPS * 32)
     T *A = w + Lo::A, *Bm = w + Lo::B, *P = w + Lo::P, *Pn = w + Lo::PN, *BtP = w + Lo::BTP, *BtPA = w + Lo::BTPA, *K = w + Lo::K,
       *Kp = w + Lo::KP, *S = w + Lo::S, *Si = w + Lo::SI, *AmBK = w + Lo::AMBK, *AtP = w + Lo::ATP, *f = w + Lo::F, *Pf = w + Lo::PF,
       *Q1 = w + Lo::Q1, *R1 = w + Lo::R1;
-    constexpr int64_t BLOB = 3 * Lo::XX + 2 * Lo::XU + Lo::UU + 3 * NX + 2 * NU + 1;
+    constexpr ModelBlob MB = model_blob(NX, NU);
 
     for (int64_t b = (int64_t)blockIdx.x * PC_WARPS + warp; b < Bn; b += (int64_t)gridDim.x * PC_WARPS) {
-        T *o = out + b * BLOB;
-        T *oA = o, *oB = oA + Lo::XX, *oF = oB + Lo::XU, *oQ = oF + NX, *oR = oQ + NX, *oK = oR + NU, *oP = oK + Lo::XU,
-          *oQuu = oP + Lo::XX, *oAm = oQuu + Lo::UU, *oAPf = oAm + Lo::XX, *oBPf = oAPf + NX;
+        T *o = out + b * (int64_t)MB.model;
+        T *oA = o + MB.A, *oB = o + MB.B, *oF = o + MB.f, *oQ = o + MB.Qd, *oR = o + MB.Rd, *oK = o + MB.Kinf, *oP = o + MB.Pinf,
+          *oQuu = o + MB.Quu, *oAm = o + MB.AmBKt, *oAPf = o + MB.APf, *oBPf = o + MB.BPf;
         const T rho = rhog[b];
         for (int e = lane; e < Lo::XX; e += 32) {
             const T a = Ag[b * Lo::XX + e];
@@ -214,7 +215,7 @@ __global__ void __launch_bounds__(PC_WARPS * 32)
             }
         }
         if (lane == 0) {
-            oBPf[NU] = rho;
+            o[MB.rho] = rho;
             if (sweeps_out) sweeps_out[b] = ok ? sweeps : -1;
         }
         __syncwarp();
