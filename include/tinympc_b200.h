@@ -113,7 +113,8 @@ typedef struct tinympc_problem {
     const void *tv_blin_u; /* num_tv_input_linear x (N-1)      */
 } tinympc_problem_t;
 
-/* TinySettings (types.hpp:63-82) without the adaptive-rho fields (out of scope, SURVEY §2 #5). */
+/* TinySettings (types.hpp:63-82) without the adaptive-rho fields: adaptive rho is a separate call
+ * (tinympc_b200_solve_adaptive, tinympc_adaptive_rho_t below). */
 typedef struct tinympc_settings {
     double abs_pri_tol;
     double abs_dua_tol;
@@ -266,6 +267,38 @@ int tinympc_b200_solve(tinympc_b200_solver_t *s, const tinympc_batch_t *io, void
 int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io);
 
 int tinympc_b200_get_stats(const tinympc_b200_solver_t *s, tinympc_b200_stats_t *stats);
+
+/*
+ * Adaptive rho (admm.cpp:397-423, rho_benchmark.cpp), per instance.  After the dual update of loop index i with
+ * i > 0 && i % 5 == 0, the residuals of format_matrices / compute_residuals (Eigen's summation order) give
+ *     new = rho * sqrt((pri / (pri_norm + 1e-10)) / ((dual / (dual_norm + 1e-10)) + 1e-10)),
+ * clipped to [rho_min, rho_max] when enable_clipping != 0, and update_matrices_with_derivatives runs twice:
+ *     Kinf += (new - rho) * dKinf_drho;  Pinf += (new - rho) * dPinf_drho;  rho = new.
+ * The same iteration's termination check and every later iteration use the new rho / Kinf / Pinf.  Quu_inv, AmBKt,
+ * APf, BPf, Q, R stay as they are (as in the reference); C1 / C2 are never read by a solve and are not modelled.
+ * The reference declares its RhoAdapter uninitialised (admm.cpp:340) and then reads it (rho_benchmark.cpp:56), which
+ * makes its adaptive solve undefined behaviour; this library implements the value-initialised adapter.
+ *
+ *   dKinf_drho (nu x nx), dPinf_drho (nx x nx): HOST pointers of the handle's dtype, column-major, read during the call.
+ *   models: [B][tinympc_b200_model_blob_elems(nx,nu)] (layout: tinympc_batch_t.models), IN/OUT: every instance starts from
+ *           its blob's model, cache and rho, and its adapted rho / Kinf / Pinf are written back, so passing the same
+ *           buffer to the next solve continues the adaptation (the reference's one-TinySolver-per-robot semantics).
+ * Served by the on-chip (GPI) kernel in STRICT mode with box constraints only; io->models must be NULL.
+ */
+typedef struct tinympc_adaptive_rho {
+    double rho_min, rho_max;  /* settings->adaptive_rho_min / max (rounded to the dtype) */
+    int32_t enable_clipping;  /* settings->adaptive_rho_enable_clipping */
+    int32_t reserved;         /* must be 0 */
+    const void *dKinf_drho;   /* nu x nx */
+    const void *dPinf_drho;   /* nx x nx */
+    void *models;             /* [B][blob] in/out */
+} tinympc_adaptive_rho_t;
+
+/* tinympc_b200_solve with adaptive rho: io and ar->models are DEVICE pointers; asynchronous on `cuda_stream` */
+int tinympc_b200_solve_adaptive(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar,
+                                void *cuda_stream);
+/* the same with HOST pointers (chunked like tinympc_b200_solve_host; ar->models is copied back); synchronous */
+int tinympc_b200_solve_adaptive_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar);
 
 /*
  * Closed-loop helper (the caller of the hot path, e.g. examples/quadrotor_tracking.cpp:105):

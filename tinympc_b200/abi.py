@@ -85,6 +85,16 @@ class Stats(C.Structure):
     ]
 
 
+class AdaptiveRho(C.Structure):
+    """tinympc_adaptive_rho_t: adaptive-rho settings, sensitivity tables (host pointers) and the in/out model blobs."""
+    _fields_ = [
+        ("rho_min", C.c_double), ("rho_max", C.c_double),
+        ("enable_clipping", C.c_int32), ("reserved", C.c_int32),
+        ("dKinf_drho", vp), ("dPinf_drho", vp),
+        ("models", vp),
+    ]
+
+
 # every entry point declared in include/tinympc_b200.h
 EXPORTS = [
     "tinympc_b200_default_settings",
@@ -99,6 +109,8 @@ EXPORTS = [
     "tinympc_b200_set_mode",
     "tinympc_b200_solve",
     "tinympc_b200_solve_host",
+    "tinympc_b200_solve_adaptive",
+    "tinympc_b200_solve_adaptive_host",
     "tinympc_b200_get_stats",
     "tinympc_b200_advance",
     "tinympc_b200_supported",

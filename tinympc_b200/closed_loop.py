@@ -14,7 +14,7 @@ import ctypes as C
 
 from . import abi
 from ._lib import check
-from .solver import BatchedTinySolver
+from .solver import AdaptiveRho, BatchedTinySolver, pack_models
 
 # box-constrained warm start: slacks + duals (+ the previous-iteration slacks v, z, which only feed the dual residual of
 # the next solve's first iteration; drop them with exact_first_residual=False for ~30 % more steps per second)
@@ -25,7 +25,10 @@ WARM_FIELDS_FAST = ("vnew", "znew", "g", "y")
 
 
 class DeviceMPCLoop:
-    def __init__(self, solver: BatchedTinySolver, x0, reset_duals: bool = False, extra_state=(), exact_first_residual: bool = True):
+    def __init__(self, solver: BatchedTinySolver, x0, reset_duals: bool = False, extra_state=(), exact_first_residual: bool = True,
+                 adaptive_rho: AdaptiveRho | None = None, models=None):
+        """adaptive_rho: every plant adapts its own rho / Kinf / Pinf, kept on the device across steps in self.models
+        ([B, blob], starting from `models` or the problem's own cache), as one TinySolver per robot would."""
         import torch
 
         self.solver = solver
@@ -40,6 +43,11 @@ class DeviceMPCLoop:
         self.out = None
         self._first = True
         self.want_solution = True  # also return solution->x / solution->u (= vnew / znew) every step
+        self.adaptive_rho = adaptive_rho
+        self.models = None
+        if adaptive_rho is not None:
+            m = pack_models(p, self.B) if models is None else models
+            self.models = torch.as_tensor(m, dtype=self._tdt, device=self.dev).reshape(self.B, -1).contiguous().clone()
 
     def step(self, Xref, Uref=None, stream=None):
         """One MPC step for every instance: solve (warm-started), then advance the plants.  Returns the output dict
@@ -52,7 +60,10 @@ class DeviceMPCLoop:
             self.state["y"].zero_()
         batch, out = s.make_device_batch(self.x0, Xref, Uref, state=self.state, cold_start=self._first, want_state=self.fields,
                                          want_u0=True, want_solution=self.want_solution)
-        s.solve_device(batch, stream)
+        if self.adaptive_rho is None:
+            s.solve_device(batch, stream)
+        else:
+            s.solve_device_adaptive(batch, self.models, self.adaptive_rho, stream)
         self.state = {n: out[n] for n in self.fields}
         self.out = out
         self._first = False

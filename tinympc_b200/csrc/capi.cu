@@ -13,6 +13,7 @@
 #include <thread>
 #include <vector>
 
+#include "adapt.h"
 #include "host_precompute.h"
 #include "launch.h"
 #include "model_blob.h"
@@ -141,6 +142,13 @@ struct tinympc_b200_solver {
     DevBuf vscratch;
     DevBuf gps_ws;
     DevBuf shared_ref;  // host path: references shared by the whole batch
+    DevBuf d_adapt;     // adaptive rho: GpiAdapt arguments + dKinf_drho + dPinf_drho (adapt.h)
+    // page-locked staging of d_adapt's contents, a ring so that the copy stays asynchronous: slot i is rewritten only once
+    // the copy three solves back (ev_adapt[i]) has read it
+    PinBuf adapt_pin[3];
+    cudaEvent_t ev_adapt[3] = {};
+    bool adapt_used[3] = {false, false, false};
+    int adapt_next = 0;
     cudaEvent_t ev_last = nullptr;  // recorded after the last enqueue
     cudaStream_t last_stream = nullptr;
     bool have_last = false;
@@ -327,14 +335,73 @@ int64_t tpi_chunk_instances(const tinympc_b200_solver *s, const Features &ft, in
     return B;  // sub-batching only lowers occupancy: TPI is latency-, not L2-, limited
 }
 
-// enqueue one batched solve on `stream` (device pointers); fills stats
-int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stream, bool timed) {
+// shared memory the adaptive kernel adds per CTA for its tables
+size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->nx, s->nu, esize(s->dtype)); }
+
+// checks of an adaptive-rho solve that need no device; `gpi` = the adaptive kernel's launch plan
+int check_adaptive(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar, tmpc::GpiPlan *gpi) {
+    if (io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
+    if (!ar->models || !ar->dKinf_drho || !ar->dPinf_drho || ar->reserved != 0)
+        return fail(TINYMPC_ERR_ARG, "adaptive rho: models, dKinf_drho and dPinf_drho are required and reserved must be 0");
+    if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho is available in STRICT mode only");
+    if (features(s).ext) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho covers box constraints only (no cones or hyperplanes)");
+    if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
+        return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs on the on-chip (GPI) kernel family only");
+    *gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin - (int)adapt_smem(s));
+    if (gpi->smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho: the horizon does not fit the on-chip kernel");
+    gpi->smem += adapt_smem(s);
+    return 0;
+}
+
+// the adaptive kernel's arguments (GpiAdapt<T>, then the tables) into s->d_adapt, ordered on `stream`: an asynchronous copy
+// from a page-locked staging slot (the host returns without waiting for earlier work on the stream)
+template <typename T>
+int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, cudaStream_t stream) {
+    const size_t nk = (size_t)s->nu * s->nx, np = (size_t)s->nx * s->nx;
+    const size_t bytes = tmpc::GPI_ADAPT_HDR + (nk + np) * sizeof(T);
+    if (s->d_adapt.bytes < bytes) {
+        if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still read the old buffer
+        if (s->d_adapt.ensure(bytes)) return fail(TINYMPC_ERR_CUDA, "adaptive-rho argument allocation failed");
+    }
+    const int slot = s->adapt_next;
+    s->adapt_next = (slot + 1) % 3;
+    if (!s->ev_adapt[slot]) CUDA_TRY(cudaEventCreateWithFlags(&s->ev_adapt[slot], cudaEventDisableTiming));
+    if (s->adapt_used[slot]) CUDA_TRY(cudaEventSynchronize(s->ev_adapt[slot]));  // its previous copy has been read
+    if (s->adapt_pin[slot].ensure(bytes)) return fail(TINYMPC_ERR_CUDA, "adaptive-rho staging allocation failed");
+    char *h = (char *)s->adapt_pin[slot].p;
+    std::memset(h, 0, bytes);
+    T *tab = (T *)(h + tmpc::GPI_ADAPT_HDR);
+    std::memcpy(tab, ar->dKinf_drho, nk * sizeof(T));
+    std::memcpy(tab + nk, ar->dPinf_drho, np * sizeof(T));
+    tmpc::GpiAdapt<T> a{};
+    a.models = (T *)ar->models;
+    a.dK = (const T *)((char *)s->d_adapt.p + tmpc::GPI_ADAPT_HDR);
+    a.dP = a.dK + nk;
+    a.rho_min = (T)ar->rho_min;
+    a.rho_max = (T)ar->rho_max;
+    a.clip = ar->enable_clipping != 0;
+    const long cols = (long)s->nx * s->N + (long)s->nu * (s->N - 1);
+    a.maskA = tmpc::gemv_block_mask((long)(s->nx + s->nu) * (s->N - 1), cols, sizeof(T));
+    a.maskP = tmpc::gemv_block_mask(cols, cols, sizeof(T));
+    static_assert(sizeof(a) <= tmpc::GPI_ADAPT_HDR, "GpiAdapt must fit its header");
+    std::memcpy(h, &a, sizeof(a));
+    CUDA_TRY(cudaMemcpyAsync(s->d_adapt.p, h, bytes, cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaEventRecord(s->ev_adapt[slot], stream));
+    s->adapt_used[slot] = true;
+    return 0;
+}
+
+// enqueue one batched solve on `stream` (device pointers); fills stats.  ar: adaptive rho (device model blobs), or null
+int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stream, bool timed,
+            const tinympc_adaptive_rho_t *ar = nullptr) {
     if (int rc = check_ready(s)) return rc;
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
+    tmpc::GpiPlan gpi;
+    if (ar)
+        if (int rc = check_adaptive(s, io, ar, &gpi)) return rc;
     if (io->B <= 0) return TINYMPC_OK;
     const Features ft = features(s);
-    tmpc::GpiPlan gpi;
-    int family = resolve_family(s, ft, &gpi, io->B);
+    int family = ar ? TINYMPC_KERNEL_GPI : resolve_family(s, ft, &gpi, io->B);
     if (io->models) {  // per-instance models: on-chip kernel only
         if (ft.ext || gpi.smem <= 0 || s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
             return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models need the on-chip GPI kernel (box constraints, horizon fitting in shared memory)");
@@ -348,6 +415,11 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     size_t ws_bytes = 0;
     tmpc::LaunchDesc d;
     base_desc(s, d, ft);
+    if (ar) {
+        if (int rc = s->dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, stream) : upload_adaptive<float>(s, ar, stream)) return rc;
+        d.adapt = 1;
+        d.adapt_args = s->d_adapt.p;
+    }
     if (timed) CUDA_TRY(cudaEventRecord(s->ev0, stream));
     d.family = family;
     d.stream = stream;
@@ -362,6 +434,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
         }
         d.Bpad = (io->B + 31) / 32 * 32;
         d.io = *io;
+        if (ar) d.io.models = ar->models;
         d.gps_ws = s->gps_ws.p;
         d.gps_ws_bytes = s->gps_ws.bytes;
         int rc = s->dim->launch(&d);
@@ -640,8 +713,12 @@ int tinympc_b200_destroy(tinympc_b200_solver_t *s) {
     cudaSetDevice(s->device);
     DevBuf *bufs[] = {&s->d_xmin, &s->d_xmax, &s->d_umin, &s->d_umax, &s->d_Alin_x, &s->d_blin_x, &s->d_Alin_u,
                       &s->d_blin_u, &s->d_tvA_x, &s->d_tvb_x, &s->d_tvA_u, &s->d_tvb_u, &s->ws, &s->queue, &s->d_blob, &s->vscratch,
-                      &s->gps_ws, &s->shared_ref};
+                      &s->gps_ws, &s->shared_ref, &s->d_adapt};
     for (DevBuf *b : bufs) b->release();
+    for (int i = 0; i < 3; ++i) {
+        s->adapt_pin[i].release();
+        if (s->ev_adapt[i]) cudaEventDestroy(s->ev_adapt[i]);
+    }
     for (int i = 0; i < tinympc_b200_solver::SLOTS; ++i) {
         s->dio[i].release();
         s->pin_in[i].release();
@@ -687,6 +764,13 @@ int tinympc_b200_solve(tinympc_b200_solver_t *s, const tinympc_batch_t *io, void
     if (!s || !io) return fail(TINYMPC_ERR_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(s->device));
     return enqueue(s, io, (cudaStream_t)cuda_stream, true);
+}
+
+int tinympc_b200_solve_adaptive(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar,
+                                void *cuda_stream) {
+    if (!s || !io || !ar) return fail(TINYMPC_ERR_ARG, "null argument");
+    CUDA_TRY(cudaSetDevice(s->device));
+    return enqueue(s, io, (cudaStream_t)cuda_stream, true, ar);
 }
 
 int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, void *cuda_stream) {
@@ -749,11 +833,15 @@ bool is_pinned(const void *p) {
 
 }  // namespace
 
-int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io) {
-    if (!s || !io) return fail(TINYMPC_ERR_ARG, "null argument");
+namespace {
+// tinympc_b200_solve_host; with `ar` (host model blobs, in/out) the adaptive-rho solve
+int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     CUDA_TRY(cudaSetDevice(s->device));
     if (int rc = check_ready(s)) return rc;
+    tmpc::GpiPlan adapt_plan;
+    if (ar)
+        if (int rc = check_adaptive(s, io, ar, &adapt_plan)) return rc;
     const int64_t B = io->B;
     if (B <= 0) return TINYMPC_OK;
     const size_t es = esize(s->dtype);
@@ -779,6 +867,9 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
     if (io->xref_per_instance) fields.push_back({io->Xref, nullptr, bx, true, false, (void **)&dev.Xref});
     if (io->Uref && io->uref_per_instance) fields.push_back({io->Uref, nullptr, bu, true, false, (void **)&dev.Uref});
     if (io->models) fields.push_back({io->models, nullptr, es * (size_t)tinympc_b200_model_blob_elems(s->nx, s->nu), true, false, (void **)&dev.models});
+    // adaptive rho: the model blobs are in/out; they travel in dev.models (io->models is NULL) and are handed to the kernel as
+    // the adaptive argument's blobs
+    if (ar) fields.push_back({ar->models, ar->models, es * (size_t)tinympc_b200_model_blob_elems(s->nx, s->nu), true, true, (void **)&dev.models});
     {
         size_t need = (io->xref_per_instance ? 0 : bx) + ((io->Uref && !io->uref_per_instance) ? bu : 0);
         if (need) {
@@ -822,7 +913,11 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
         // number of such waves so that no chunk ends on a mostly empty wave
         const Features ft = features(s);
         tmpc::GpiPlan gpi;
-        const int fam = resolve_family(s, ft, &gpi, chunk);
+        int fam = resolve_family(s, ft, &gpi, chunk);
+        if (ar) {  // the adaptive kernel's own plan (its tables take shared memory)
+            fam = TINYMPC_KERNEL_GPI;
+            gpi = adapt_plan;
+        }
         if (fam == TINYMPC_KERNEL_GPI && B > 16384) {
             const int64_t wave = (int64_t)s->sm_count * gpi.instances_per_cta;
             if (wave > 0 && wave < B) chunk = std::max<int64_t>(1, (chunk + wave / 2) / wave) * wave;
@@ -896,7 +991,14 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
         }
         CUDA_TRY(cudaEventRecord(s->ev_in[slot], s->st_h2d));
         CUDA_TRY(cudaStreamWaitEvent(s->st_k, s->ev_in[slot], 0));
-        if (int rc = enqueue(s, &d, s->st_k, false)) return rc;
+        if (ar) {
+            tinympc_adaptive_rho_t a = *ar;
+            a.models = (void *)d.models;
+            d.models = nullptr;
+            if (int rc = enqueue(s, &d, s->st_k, false, &a)) return rc;
+        } else if (int rc = enqueue(s, &d, s->st_k, false)) {
+            return rc;
+        }
         launches += s->stats.kernel_launches;
         CUDA_TRY(cudaEventRecord(s->ev_k[slot], s->st_k));
         CUDA_TRY(cudaStreamWaitEvent(s->st_d2h, s->ev_k[slot], 0));
@@ -924,6 +1026,17 @@ int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io)
     s->timed = false;
     s->stats.kernel_ms = 0.f;
     return TINYMPC_OK;
+}
+}  // namespace
+
+int tinympc_b200_solve_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io) {
+    if (!s || !io) return fail(TINYMPC_ERR_ARG, "null argument");
+    return solve_host_impl(s, io, nullptr);
+}
+
+int tinympc_b200_solve_adaptive_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
+    if (!s || !io || !ar) return fail(TINYMPC_ERR_ARG, "null argument");
+    return solve_host_impl(s, io, ar);
 }
 
 }  // extern "C"

@@ -21,6 +21,7 @@
 #include <algorithm>
 #include <cstdlib>
 
+#include "adapt.h"
 #include "common.cuh"
 #include "lanegroup.cuh"
 #include "model_blob.h"
@@ -64,11 +65,23 @@ __host__ __device__ constexpr bool gpi_feasible() {
 
 constexpr int GPI_MAX_WARPS = 8;
 
+// Adaptive rho (tinympc_b200_solve_adaptive): the kernel is instantiated with GPI_ADAPT added to its lane count; it then
+// runs heterogeneous STRICT batches and reads its GpiAdapt arguments (adapt.h: gpi_adapt_args).  (A separate template
+// parameter or kernel argument would rename the existing kernels, a shared __device__ body or a larger KParams changes their
+// machine code.)
+constexpr int GPI_ADAPT = 64;
+
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
-template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool MM = false>
+template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
 __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     gpi_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
+    constexpr bool ADAPT = LA >= GPI_ADAPT;  // adaptive rho
+    constexpr int L = LA % GPI_ADAPT;
+    static_assert(LA < 2 * GPI_ADAPT && L > 0, "lane count: 4, 8 or 16, plus GPI_ADAPT for the adaptive variant");
+    static_assert(!ADAPT || (HET && !FAST && !MM), "adaptive rho runs on heterogeneous STRICT batches");
+    GpiAdapt<T> AP{};
+    if constexpr (ADAPT) AP = *gpi_adapt_args<T>(P);
     using Cfg = GpiCfg<NX, NU, L, (int)sizeof(T)>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, PVP = Cfg::PVP, NPV = Cfg::NPV;
     constexpr int NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -110,7 +123,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // Backward-sweep rows (AmBKt, B^T, Kinf^T, Quu_inv, APf, BPf and the cost weights Qd, Rd) and forward-sweep rows (A, Kinf,
     // B, f) load separately: fp64 re-reads the rows of a sweep when it starts (PS), everything else loads both once.
     auto load_bwd_rows = [&](const T *src) {
-        auto rd = [src](int e) { return src[e]; };
+        auto rd = [src](int e) {
+            if constexpr (ADAPT) return __ldcg(src + e);
+            else return src[e];
+        };
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
@@ -129,7 +145,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         }
     };
     auto load_fwd_rows = [&](const T *src) {
-        auto rd = [src](int e) { return src[e]; };
+        auto rd = [src](int e) {
+            if constexpr (ADAPT) return __ldcg(src + e);
+            else return src[e];
+        };
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
@@ -146,7 +165,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // both sets at once (everything but fp64), row by row with the backward and forward matrices interleaved: the load
     // order the kernel was tuned with (load_bwd_rows + load_fwd_rows compiles to a different schedule)
     auto load_rows = [&](const T *src) {
-        auto rd = [src](int e) { return src[e]; };
+        auto rd = [src](int e) {
+            if constexpr (ADAPT) return __ldcg(src + e);
+            else return src[e];
+        };
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
@@ -178,8 +200,11 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         }
     };
     // where this lane's rows come from at a sweep start (PS): the staged blob, or its slot's own blob (heterogeneous batch)
+    // ADAPT reads rows with ld.global.cg (the blobs are rewritten during the launch), so its rows come from a global blob
+    // (the first instance's) even for a slot that never gets an instance, never from the staged shared-memory copy
     const T *rowsrc = stage;
-    if constexpr (!PS) load_rows(stage);
+    if constexpr (ADAPT) rowsrc = P.models;
+    if constexpr (!PS) load_rows(rowsrc);
     __syncthreads();  // staging area is reused as state below
 
     // ---- shared-memory state of this warp ----
@@ -196,6 +221,17 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     const unsigned aPB = (unsigned)__cvta_generic_to_shared(gPB) + (unsigned)(lane * PVP) * ES;
     const unsigned aD = (unsigned)__cvta_generic_to_shared(gD) + (unsigned)lane * ES;
     const unsigned aGB = (unsigned)__cvta_generic_to_shared(gGB);
+    // ADAPT: dKinf_drho / dPinf_drho staged behind the state regions of all warps (and behind the dead blob staging area)
+    const T *sdK = nullptr, *sdP = nullptr;
+    if constexpr (ADAPT) {
+        size_t off = BLOB_KEEP + (size_t)(blockDim.x >> 5) * warp_elems * ES;
+        off = ((off > BLOB_BYTES ? off : (size_t)BLOB_BYTES) + 15) / 16 * 16;
+        T *t = reinterpret_cast<T *>(smem_raw + off);
+        for (int e = threadIdx.x; e < NU * NX + NX * NX; e += blockDim.x) t[e] = AP.dK[e];  // dP follows dK
+        __syncthreads();
+        sdK = t;
+        sdP = t + NU * NX;
+    }
     constexpr unsigned KSTR = 32u * PVP * ES;  // bytes per knot point in PA / PB
     constexpr unsigned DSTR = (unsigned)RU * 32u * ES;
     auto load_pack = [&](unsigned base, int k, T (&v)[PVP]) {
@@ -278,6 +314,11 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     bool busy = false;    // the slot holds an unfinished instance
     bool want = true;     // the slot should try to fetch an instance
     int it = 0, solved = 0;
+    // ADAPT: an adaptation of this slot's Kinf / Pinf waiting to be applied (at the next iteration start or at retire: the
+    // retire-time replay of work->x / work->u must use the Kinf of the last forward pass); the two deltas of
+    // update_matrices_with_derivatives (rho_benchmark.cpp:240, admm.cpp:421)
+    bool pend = false;
+    T adelta = T(0), adelta2 = T(0);
     T res_px = T(0), res_dx = T(0), res_pu = T(0), res_du = T(0);
     T x0o[RX], pterm[RX];
 #pragma unroll
@@ -620,6 +661,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         if (slot == s) {
             inst = ib;
             busy = true;
+            pend = false;
             it = 0;
             solved = 0;
             res_px = res_dx = res_pu = res_du = T(0);
@@ -650,6 +692,209 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             }
         }
         __syncwarp();
+    };
+
+    // ---- ADAPT: adaptive rho (admm.cpp:397-423 with a value-initialised RhoAdapter) ----
+    // Kinf += delta*dK; Kinf += delta2*dK (and Pinf) in this slot's blob for a pending slot, elements split over its L lanes
+    auto adapt_blob = [&](const bool on) {
+        T *mb = AP.models + (inst < 0 ? 0 : inst) * (int64_t)MB.model;
+        for (int e0 = 0; e0 < NU * NX + NX * NX; e0 += L) {
+            const int e = e0 + l;
+            if (on && e < NU * NX + NX * NX) {
+                const int o = e < NU * NX ? MB.Kinf + e : MB.Pinf + (e - NU * NX);
+                const T dv = e < NU * NX ? sdK[e] : sdP[e - NU * NX];
+                const T v1 = __ldcg(mb + o) + adelta * dv;
+                mb[o] = v1 + adelta2 * dv;
+            }
+        }
+    };
+    // apply the pending adaptation before an iteration: blob, fp32 register copies of Kinf (mKt and the forward rows, same
+    // arithmetic as the blob), terminal-cost constant from the new Pinf
+    auto adapt_apply = [&]() {
+        adapt_blob(pend);
+        __syncwarp();
+        if (pend) {
+            if constexpr (!PS) {
+#pragma unroll
+                for (int a = 0; a < RX; ++a) {
+                    const int ii = xv[a] ? l * RX + a : 0;
+#pragma unroll
+                    for (int j = 0; j < NU; ++j) {
+                        const T dv = sdK[j + NU * ii];
+                        mKt[a][j] = xv[a] ? (mKt[a][j] + adelta * dv) + adelta2 * dv : T(0);
+                    }
+                }
+#pragma unroll
+                for (int b = 0; b < RU; ++b) {
+                    const int jj = uv[b] ? l * RU + b : 0;
+#pragma unroll
+                    for (int m = 0; m < NX; ++m) {
+                        const T dv = sdK[jj + NU * m];
+                        mS1f[RX + b][m] = uv[b] ? (mS1f[RX + b][m] + adelta * dv) + adelta2 * dv : T(0);
+                    }
+                }
+            }
+            const T *pinf = AP.models + inst * (int64_t)MB.model + MB.Pinf;
+            const T *xl = xrefp - l * RX + (int64_t)(N - 1) * NX;
+#pragma unroll
+            for (int a = 0; a < RX; ++a) {
+                const int ii = xv[a] ? l * RX + a : 0;
+                T sacc = __ldg(xl) * __ldcg(pinf + NX * ii);
+                for (int m = 1; m < NX; ++m) sacc = mac<false>(sacc, __ldg(xl + m), __ldcg(pinf + m + NX * ii));
+                pterm[a] = xv[a] ? -sacc : T(0);
+            }
+            pend = false;
+        }
+    };
+    // residuals of format_matrices / compute_residuals (rho_benchmark.cpp:47-188) for the slots with `ad`, then predict_rho:
+    // the rollout of this iteration is replayed from x0 and d (bit-identical to the forward pass), vnew / znew / g / y are the
+    // updated packs.  A x and P x follow Eigen's column-major GEMV (sums of column-block partials), A^T y its row-major one.
+    auto adapt_sweep = [&](const bool ad) {
+        if constexpr (PS) load_fwd_rows(rowsrc);
+        const T *mbp = AP.models + (inst < 0 ? 0 : inst) * (int64_t)MB.model;
+        const int S = NX + NU, mA = AP.maskA, mP = AP.maskP;
+        T ax_m = T(0), z_m = T(0), rp_m = T(0), px_m = T(0), aty_m = T(0), q_m = T(0), rd_m = T(0);
+        auto amax = [](T &m, T v) {
+            const T a = fabs(v);
+            m = (m < a) ? a : m;
+        };
+        T xo[RX], Xf[NX];
+#pragma unroll
+        for (int a = 0; a < RX; ++a) xo[a] = x0o[a];
+        gather_x(xo, Xf);
+        for (int k = 0; k < N; ++k) {
+            const bool more = k < N - 1;  // uniform
+            T pa[PVP], pb[PVP], pa1[PVP], Gf[NX], u[RU], Uf[NU], t1[RX + RU], bu[RX], xn[RX];
+            load_pack(aPA, k, pa);
+            load_pb(k, pb);
+#pragma unroll
+            for (int b = 0; b < RU; ++b) u[b] = T(0);
+#pragma unroll
+            for (int a = 0; a < RX; ++a) xn[a] = T(0);
+#pragma unroll
+            for (int m = 0; m < NX; ++m) Gf[m] = T(0);
+#pragma unroll
+            for (int e = 0; e < PVP; ++e) pa1[e] = T(0);
+            if (more) {
+                T dk[RU];
+                load_d(k, dk);
+                dots<false>(mS1f, Xf, t1);
+#pragma unroll
+                for (int b = 0; b < RU; ++b) u[b] = (-t1[RX + b]) - dk[b];
+                gather_u(u, Uf);
+                dots<false>(mB, Uf, bu);
+#pragma unroll
+                for (int a = 0; a < RX; ++a) xn[a] = (t1[a] + bu[a]) + vf[a];
+                T pb1[PVP], gown[RX];
+                load_pb(k + 1, pb1);
+                load_pack(aPA, k + 1, pa1);
+#pragma unroll
+                for (int a = 0; a < RX; ++a) gown[a] = pb1[a];
+                gather_x(gown, Gf);
+            }
+            const int c0 = k * S;
+#pragma unroll
+            for (int a = 0; a < RX; ++a) {
+                if (!xv[a]) continue;
+                const int i = l * RX + a;
+                const T q = __ldg(mbp + MB.Qd + i) * xo[a];
+                T px = q;
+                if (!more) {  // P x of the terminal block: Pinf row i against x_{N-1}
+                    T res = T(0), c = T(0);
+                    int blk = c0 & ~mP;
+#pragma unroll
+                    for (int j = 0; j < NX; ++j) {
+                        const int bj = (c0 + j) & ~mP;
+                        if (bj != blk) { res = res + c; c = T(0); blk = bj; }
+                        c = (__ldcg(mbp + MB.Pinf + i + NX * j) * Xf[j]) + c;
+                    }
+                    px = res + c;
+                }
+                T aty = T(0);
+                if (k >= 1) aty = (T(-1) * pb[a]) + aty;
+                if (more) {
+#pragma unroll
+                    for (int r = 0; r < NX; ++r) aty = (__ldg(mbp + MB.A + r + NX * i) * Gf[r]) + aty;
+                }
+                amax(px_m, px);
+                amax(q_m, q);
+                amax(aty_m, aty);
+                amax(rd_m, (px + q) + aty);
+                if (more) {  // dynamics row i of step k: A(i,:) x_k + B(i,:) u_k - x_{k+1}(i) against vnew_{k+1}(i)
+                    T res = T(0), c = T(0);
+                    int blk = c0 & ~mA;
+#pragma unroll
+                    for (int j = 0; j < NX; ++j) {
+                        const int bj = (c0 + j) & ~mA;
+                        if (bj != blk) { res = res + c; c = T(0); blk = bj; }
+                        c = (mS1f[a][j] * Xf[j]) + c;
+                    }
+#pragma unroll
+                    for (int j = 0; j < NU; ++j) {
+                        const int bj = (c0 + NX + j) & ~mA;
+                        if (bj != blk) { res = res + c; c = T(0); blk = bj; }
+                        c = (mB[a][j] * Uf[j]) + c;
+                    }
+                    {
+                        const int bj = (c0 + S + i) & ~mA;
+                        if (bj != blk) { res = res + c; c = T(0); blk = bj; }
+                        c = (T(-1) * xn[a]) + c;
+                    }
+                    const T axv = res + c, z = pa1[a];
+                    amax(ax_m, axv);
+                    amax(z_m, z);
+                    amax(rp_m, axv - z);
+                }
+            }
+            if (more) {
+#pragma unroll
+                for (int b = 0; b < RU; ++b) {
+                    if (!uv[b]) continue;
+                    const int j = l * RU + b;
+                    const T rj = __ldg(mbp + MB.Rd + j);
+                    const T px = rj * u[b], q = rj * u[b];
+                    T aty = (T(1) * pb[RX + b]) + T(0);
+#pragma unroll
+                    for (int r = 0; r < NX; ++r) aty = (__ldg(mbp + MB.B + r + NX * j) * Gf[r]) + aty;
+                    amax(px_m, px);
+                    amax(q_m, q);
+                    amax(aty_m, aty);
+                    amax(rd_m, (px + q) + aty);
+                    const T z = pa[RX + b];
+                    amax(ax_m, u[b]);
+                    amax(z_m, z);
+                    amax(rp_m, u[b] - z);
+                }
+#pragma unroll
+                for (int a = 0; a < RX; ++a) xo[a] = xn[a];
+                gather_x(xo, Xf);
+            }
+        }
+        rp_m = group_max<T, L>(rp_m);
+        rd_m = group_max<T, L>(rd_m);
+        ax_m = group_max<T, L>(ax_m);
+        z_m = group_max<T, L>(z_m);
+        px_m = group_max<T, L>(px_m);
+        aty_m = group_max<T, L>(aty_m);
+        q_m = group_max<T, L>(q_m);
+        if (ad) {  // predict_rho (rho_benchmark.cpp:190-213), then update_matrices_with_derivatives twice (deferred)
+            const T pn = (ax_m < z_m) ? z_m : ax_m;
+            const T dm = (px_m < aty_m) ? aty_m : px_m;
+            const T dn = (dm < q_m) ? q_m : dm;
+            const T eps = (T)1e-10;
+            const T np_ = rp_m / (pn + eps);
+            const T nd_ = rd_m / (dn + eps);
+            const T ratio = np_ / (nd_ + eps);
+            T nr = rho_m * sqrt(ratio);
+            if (AP.clip) {
+                nr = (nr < AP.rho_min) ? AP.rho_min : nr;
+                nr = (AP.rho_max < nr) ? AP.rho_max : nr;
+            }
+            adelta = nr - rho_m;
+            adelta2 = nr - nr;
+            rho_m = nr;
+            pend = true;
+        }
     };
 
     // ---- cooperative write-back of slot `s` (instance `ib`): solution, info, optional state and rollout ----
@@ -759,6 +1004,11 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     else if (cold) P.s_u[ou + e] = T(0);
                 }
         }
+        if constexpr (ADAPT) {  // the adapted cache persists in the instance's blob (after the replay above)
+            adapt_blob(slot == s && pend);
+            if (slot == s && l == 0) AP.models[ib * (int64_t)MB.model + MB.rho] = rho_m;
+            if (slot == s) pend = false;
+        }
         __syncwarp();
     };
 
@@ -795,6 +1045,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         // control flow only, so the compiler keeps the warp converged (no divergence bookkeeping around the
         // shared-memory gathers).
         do {
+        if constexpr (ADAPT) {
+            if (__any_sync(0xffffffffu, pend)) adapt_apply();
+        }
         // ---- terminal cost + backward pass (update_linear_cost fused, software-pipelined by one column) ----
         if constexpr (PS) load_bwd_rows(rowsrc);
         T po[RX], Pf[NX];
@@ -862,6 +1115,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         rdx = group_max<T, L>(rdx);
         rpu = group_max<T, L>(rpu);
         rdu = group_max<T, L>(rdu);
+        if constexpr (ADAPT) {  // after update_dual of loop index i = it: adapt when i > 0 && i % 5 == 0 (admm.cpp:407)
+            const bool ad = busy && it > 0 && it % 5 == 0;
+            if (__any_sync(0xffffffffu, ad)) adapt_sweep(ad);
+        }
         if (busy) {
             it += 1;
             if (it % P.check_termination == 0) {
@@ -935,6 +1192,25 @@ int launch_gpi_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P
         // ngroups = warps the batch fills.  A batch smaller than one wave is spread over all SMs with fewer warps per CTA
         // (the kernel's carve-up is per warp, any block size up to plan.warps works): the latency of a solve is set by how
         // many warps share a scheduler.
+        int warps = plan.warps;
+        if ((ngroups + warps - 1) / warps < d->sm_count) warps = (int)std::max<int64_t>(1, (ngroups + d->sm_count - 1) / d->sm_count);
+        const int64_t want = (ngroups + warps - 1) / warps;
+        const int ctas = (int)std::max<int64_t>(1, std::min<int64_t>(d->sm_count, want));
+        kern<<<ctas, warps * 32, plan.smem, d->stream>>>(P, gmat, (unsigned long long *)d->work_queue);
+        return launch_done(d, warps * 32, ctas, plan.smem, L, plan.instances_per_cta);
+    } else {
+        return TINYMPC_ERR_UNSUPPORTED;
+    }
+}
+
+// the adaptive kernel (plan.smem includes gpi_adapt_bytes); same launch geometry as launch_gpi_L
+template <typename T, int NX, int NU, int L>
+int launch_gpi_adapt_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P, const T *gmat) {
+    static_assert(L < GPI_ADAPT, "the lane count must leave GPI_ADAPT free");
+    if constexpr (gpi_feasible<T, NX, NU, L>()) {
+        auto kern = gpi_solve_kernel<T, NX, NU, L + GPI_ADAPT, false, true>;
+        if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
+        const int64_t ngroups = (d->io.B + (32 / L) - 1) / (32 / L);
         int warps = plan.warps;
         if ((ngroups + warps - 1) / warps < d->sm_count) warps = (int)std::max<int64_t>(1, (ngroups + d->sm_count - 1) / d->sm_count);
         const int64_t want = (ngroups + warps - 1) / warps;

@@ -119,9 +119,31 @@ int launch_gpi(LaunchDesc *d) {
     return TINYMPC_ERR_UNSUPPORTED;
 }
 
+// adaptive rho: heterogeneous STRICT batches; the tables take gpi_adapt_bytes of shared memory per CTA
+template <typename T, int NX, int NU>
+int launch_gpi_adapt(LaunchDesc *d) {
+    const int extra = (int)gpi_adapt_bytes(NX, NU, sizeof(T));
+    GpiPlan plan = gpi_plan<T, NX, NU>(d->N, d->max_smem_optin - 64 - extra);
+    if (plan.L == 0 || d->fast || !d->gmat || !d->work_queue || !d->io.models) return TINYMPC_ERR_UNSUPPORTED;
+    plan.smem += extra;
+    KParams<T, NX, NU> P;
+    fill_params<T, NX, NU>(P, *d);
+    if (!d->adapt_args) return TINYMPC_ERR_UNSUPPORTED;
+    set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
+    const T *gmat = (const T *)d->gmat;
+    if (plan.L == 4) return launch_gpi_adapt_L<T, NX, NU, 4>(d, plan, P, gmat);
+    if (plan.L == 8) return launch_gpi_adapt_L<T, NX, NU, 8>(d, plan, P, gmat);
+#ifndef TM_GPI_L16
+    if constexpr (sizeof(T) == 8)
+#endif
+        if (plan.L == 16) return launch_gpi_adapt_L<T, NX, NU, 16>(d, plan, P, gmat);
+    return TINYMPC_ERR_UNSUPPORTED;
+}
+
 template <typename T>
 int launch_T(LaunchDesc *d) {
     if (d->ext) return TINYMPC_ERR_UNSUPPORTED;  // the on-chip kernel covers box constraints; the rest streams (gps)
+    if (d->adapt) return launch_gpi_adapt<T, TM_NX, TM_NU>(d);
     return d->fast ? launch_gpi<T, TM_NX, TM_NU, true>(d) : launch_gpi<T, TM_NX, TM_NU, false>(d);
 }
 

@@ -42,6 +42,11 @@ struct LaunchDesc {
     void *gps_ws;        // GPS: streamed state records of the resident slots (allocated by the caller, see out_ws_need)
     size_t gps_ws_bytes;
 
+    // adaptive rho (tinympc_b200_solve_adaptive): io.models is then the in/out blob array; adapt_args = device copy of
+    // GpiAdapt<T> (adapt.h) followed by dKinf_drho and dPinf_drho
+    int adapt;
+    const void *adapt_args;
+
     cudaStream_t stream;
     int sm_count;
     int max_smem_optin;

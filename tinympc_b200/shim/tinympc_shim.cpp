@@ -1,5 +1,6 @@
 // tinympc_shim.cpp — implementation of the reference-compatible front end (tinympc_shim.hpp) over the C ABI.
-// Host-side bookkeeping only; every tiny_solve() is one tinympc_b200_solve_host() call (batch of one).
+// Host-side bookkeeping only; every tiny_solve() is one tinympc_b200_solve_host() call (batch of one), or with
+// settings->adaptive_rho one tinympc_b200_solve_adaptive_host() call.
 #include "tinympc_shim.hpp"
 
 #include <cstdint>
@@ -67,15 +68,21 @@ uint64_t fnv_m(uint64_t h, const M &m) {
     return m.size() ? fnv(h, m.data(), sizeof(typename M::Scalar) * m.size()) : h;
 }
 
-uint64_t fingerprint(const TinySolver *s) {
+// adaptive: rho, Kinf and Pinf travel in the solve's model blob (adaptive rho rewrites them after every solve), so they do not
+// key the handle
+uint64_t fingerprint(const TinySolver *s, bool adaptive) {
     const TinyWorkspace *w = s->work;
     const TinyCache *c = s->cache;
     uint64_t h = 1469598103934665603ULL;
-    int dims[3] = {w->nx, w->nu, w->N};
+    int dims[4] = {w->nx, w->nu, w->N, (int)adaptive};
     h = fnv(h, dims, sizeof(dims));
-    h = fnv(h, &c->rho, sizeof(c->rho));
+    if (!adaptive) h = fnv(h, &c->rho, sizeof(c->rho));
     h = fnv_m(h, w->Adyn); h = fnv_m(h, w->Bdyn); h = fnv_m(h, w->fdyn); h = fnv_m(h, w->Q); h = fnv_m(h, w->R);
-    h = fnv_m(h, c->Kinf); h = fnv_m(h, c->Pinf); h = fnv_m(h, c->Quu_inv); h = fnv_m(h, c->AmBKt); h = fnv_m(h, c->APf); h = fnv_m(h, c->BPf);
+    if (!adaptive) {
+        h = fnv_m(h, c->Kinf);
+        h = fnv_m(h, c->Pinf);
+    }
+    h = fnv_m(h, c->Quu_inv); h = fnv_m(h, c->AmBKt); h = fnv_m(h, c->APf); h = fnv_m(h, c->BPf);
     h = fnv_m(h, w->x_min); h = fnv_m(h, w->x_max); h = fnv_m(h, w->u_min); h = fnv_m(h, w->u_max);
     h = fnv_m(h, w->Acx); h = fnv_m(h, w->qcx); h = fnv_m(h, w->cx); h = fnv_m(h, w->Acu); h = fnv_m(h, w->qcu); h = fnv_m(h, w->cu);
     h = fnv_m(h, w->Alin_x); h = fnv_m(h, w->blin_x); h = fnv_m(h, w->Alin_u); h = fnv_m(h, w->blin_u);
@@ -89,7 +96,7 @@ const void *ptr(const M &m) {
 }
 
 int ensure_handle(TinySolver *s, Impl &im) {
-    const uint64_t fp = fingerprint(s);
+    const uint64_t fp = fingerprint(s, s->settings && s->settings->adaptive_rho);
     if (im.h && fp == im.fingerprint) return 0;
     if (im.h) tinympc_b200_destroy(im.h);
     im.h = nullptr;
@@ -376,6 +383,17 @@ int tiny_set_u_ref(TinySolver *s, tinyMatrix u_ref) {
 // admm.hpp:9 — the ADMM driver itself (admm.cpp:331-455); tiny_solve is the reference's trampoline onto it
 int solve(TinySolver *s) {
     TinyWorkspace *w = s->work;
+    if (s->settings->adaptive_rho) {  // the reference adds these tables to Kinf / Pinf (rho_benchmark.cpp:204-205)
+        const TinyCache *c = s->cache;
+        const long nx = w->nx, nu = w->nu;
+        if (c->dKinf_drho.rows() != nu || c->dKinf_drho.cols() != nx || c->dPinf_drho.rows() != nx || c->dPinf_drho.cols() != nx) {
+            std::cout << "tinympc_b200 shim: settings->adaptive_rho needs cache->dKinf_drho (" << nu << " x " << nx
+                      << ") and cache->dPinf_drho (" << nx << " x " << nx << "), got " << c->dKinf_drho.rows() << " x "
+                      << c->dKinf_drho.cols() << " and " << c->dPinf_drho.rows() << " x " << c->dPinf_drho.cols()
+                      << " (tiny_initialize_sensitivity_matrices fills 4 x 12 / 12 x 12 tables)" << std::endl;
+            return 1;
+        }
+    }
     Impl &im = impl_of(s);
     if (ensure_handle(s, im)) return 1;
     push_settings(s, im);
@@ -400,7 +418,42 @@ int solve(TinySolver *s) {
     int32_t iter = 0, solved = 0;
     tinytype res[4] = {0, 0, 0, 0};
     io.iter = &iter; io.solved = &solved; io.residuals = res;
-    int rc = tinympc_b200_solve_host(im.h, &io);
+    int rc;
+    if (s->settings->adaptive_rho) {
+        // admm.cpp:397-423 with a value-initialised RhoAdapter (the reference's is uninitialised, admm.cpp:340): one instance
+        // whose model blob carries this solver's cache in and the adapted rho / Kinf / Pinf out
+        TinyCache *c = s->cache;
+        std::vector<tinytype> blob((size_t)tinympc_b200_model_blob_elems((int)nx, (int)nu));
+        tinytype *o = blob.data();
+        auto put = [&o](const tinytype *p, long n) {
+            std::memcpy(o, p, sizeof(tinytype) * n);
+            o += n;
+        };
+        put(w->Adyn.data(), nx * nx); put(w->Bdyn.data(), nx * nu); put(w->fdyn.data(), nx); put(w->Q.data(), nx);
+        put(w->R.data(), nu);
+        tinytype *oK = o;
+        put(c->Kinf.data(), nu * nx);
+        tinytype *oP = o;
+        put(c->Pinf.data(), nx * nx);
+        put(c->Quu_inv.data(), nu * nu); put(c->AmBKt.data(), nx * nx); put(c->APf.data(), nx); put(c->BPf.data(), nu);
+        *o = c->rho;
+        tinympc_adaptive_rho_t ar;
+        std::memset(&ar, 0, sizeof(ar));
+        ar.rho_min = s->settings->adaptive_rho_min;
+        ar.rho_max = s->settings->adaptive_rho_max;
+        ar.enable_clipping = s->settings->adaptive_rho_enable_clipping;
+        ar.dKinf_drho = c->dKinf_drho.data();
+        ar.dPinf_drho = c->dPinf_drho.data();
+        ar.models = blob.data();
+        rc = tinympc_b200_solve_adaptive_host(im.h, &io, &ar);
+        if (!rc) {  // the adapted cache persists in the TinySolver, as in the reference
+            std::memcpy(c->Kinf.data(), oK, sizeof(tinytype) * nu * nx);
+            std::memcpy(c->Pinf.data(), oP, sizeof(tinytype) * nx * nx);
+            c->rho = *o;
+        }
+    } else {
+        rc = tinympc_b200_solve_host(im.h, &io);
+    }
     if (rc) {
         std::cout << "tinympc_b200 shim: " << tinympc_b200_last_error() << std::endl;
         return 1;
@@ -427,8 +480,8 @@ void update_dual(TinySolver *) { fused_stage("update_dual"); }
 bool termination_condition(TinySolver *) { fused_stage("termination_condition"); }
 
 // tiny_api.hpp:54 / tiny_api.cpp:479-540: fills the four sensitivity matrices of the cache with the reference's hard-coded
-// (quadrotor-sized: 4x12, 12x12, 4x4, 12x12) tables, whatever the solver's dimensions - as the reference does.  Adaptive rho
-// itself stays out of scope (settings->adaptive_rho must remain 0); this keeps programs that call the initialiser working.
+// (quadrotor-sized: 4x12, 12x12, 4x4, 12x12) tables, whatever the solver's dimensions - as the reference does.  solve() uses
+// dKinf_drho / dPinf_drho when settings->adaptive_rho is set, and refuses tables of another shape.
 void tiny_initialize_sensitivity_matrices(TinySolver *s) {
     if (!s || !s->cache) return;
     s->cache->dKinf_drho = Map<const Matrix<double, 4, 12>>(k_dKinf_drho);

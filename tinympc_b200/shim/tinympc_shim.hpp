@@ -51,7 +51,7 @@ typedef struct {
     int max_iter, check_termination;
     int en_state_bound, en_input_bound, en_state_soc, en_input_soc;
     int en_state_linear, en_input_linear, en_tv_state_linear, en_tv_input_linear;
-    int adaptive_rho;  // must stay 0
+    int adaptive_rho;  // 1: solve() adapts rho / Kinf / Pinf (tinympc_b200_solve_adaptive_host); needs cache->dKinf_drho / dPinf_drho
     tinytype adaptive_rho_min, adaptive_rho_max;
     int adaptive_rho_enable_clipping;
 } TinySettings;

@@ -93,6 +93,35 @@ def unpack_model(blob, nx, nu):
     return out
 
 
+def pack_models(problem: MPCProblem, B: int):
+    """The problem's own model, cache and rho as B identical model blobs [B, blob] (layout: tinympc_batch_t.models,
+    csrc/model_blob.h): the starting point of an adaptive-rho batch whose instances share one model."""
+    dt = problem.dtype
+    pieces = [problem.A, problem.B, problem.f, problem.Q, problem.R, problem.Kinf, problem.Pinf, problem.Quu_inv, problem.AmBKt,
+              problem.APf, problem.BPf]
+    blob = np.concatenate([np.asarray(a, dtype=dt).reshape(-1, order="F") for a in pieces] + [np.array([problem.rho], dtype=dt)])
+    return np.ascontiguousarray(np.tile(blob, (int(B), 1)))
+
+
+class AdaptiveRho:
+    """The reference's adaptive-rho settings (settings->adaptive_rho_min / _max / _enable_clipping) and sensitivity tables
+    (cache->dKinf_drho nu x nx, dPinf_drho nx x nx), for BatchedTinySolver.solve(..., adaptive_rho=...)."""
+
+    def __init__(self, dKinf_drho, dPinf_drho, rho_min=1.0, rho_max=100.0, enable_clipping=True):
+        self.dKinf_drho, self.dPinf_drho = dKinf_drho, dPinf_drho
+        self.rho_min, self.rho_max, self.enable_clipping = float(rho_min), float(rho_max), bool(enable_clipping)
+
+    def to_c(self, problem: MPCProblem, models_ptr) -> abi.AdaptiveRho:
+        dt = problem.dtype
+        dK = np.asfortranarray(np.asarray(self.dKinf_drho, dtype=dt).reshape(problem.nu, problem.nx))
+        dP = np.asfortranarray(np.asarray(self.dPinf_drho, dtype=dt).reshape(problem.nx, problem.nx))
+        a = abi.AdaptiveRho()
+        a.rho_min, a.rho_max, a.enable_clipping, a.reserved = self.rho_min, self.rho_max, int(self.enable_clipping), 0
+        a.dKinf_drho, a.dPinf_drho, a.models = dK.ctypes.data, dP.ctypes.data, models_ptr
+        a._owner = (dK, dP)
+        return a
+
+
 class BatchedTinySolver:
     """A TinySolver (types.hpp:213-218) for B independent instances on one H100."""
 
@@ -138,11 +167,22 @@ class BatchedTinySolver:
         return {n: getattr(st, n) for n, _ in abi.Stats._fields_}
 
     # ---- host buffers (numpy): the call a reference user would make; H2D/D2H inside ------------------
-    def solve(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), models=None) -> dict:
-        hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, models=models)
-        cb = hb.to_c()
-        check(self._lib.tinympc_b200_solve_host(self._h, C.byref(cb)))
-        return hb.result()
+    def solve(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), models=None,
+              adaptive_rho: AdaptiveRho | None = None) -> dict:
+        """With adaptive_rho: every instance adapts its own rho / Kinf / Pinf, starting from its blob in `models` (default:
+        the problem's own cache, pack_models); the result's "models" holds the adapted blobs, the start of the next solve."""
+        if adaptive_rho is None:
+            hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, models=models)
+            cb = hb.to_c()
+            check(self._lib.tinympc_b200_solve_host(self._h, C.byref(cb)))
+            return hb.result()
+        hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state)
+        m = pack_models(self.problem, hb.B) if models is None else np.array(models, dtype=self.problem.dtype).reshape(hb.B, -1)
+        cb, ar = hb.to_c(), adaptive_rho.to_c(self.problem, m.ctypes.data)
+        check(self._lib.tinympc_b200_solve_adaptive_host(self._h, C.byref(cb), C.byref(ar)))
+        out = hb.result()
+        out["models"] = m
+        return out
 
     def solve_prepared(self, hb: HostBatch, cb: abi.Batch | None = None):
         """Same as solve() on an already-built HostBatch (bench.py: keeps numpy allocation out of the timed region)."""
@@ -239,3 +279,17 @@ class BatchedTinySolver:
 
         s = stream if stream is not None else torch.cuda.current_stream(self.device)
         check(self._lib.tinympc_b200_solve(self._h, C.byref(batch), C.c_void_p(s.cuda_stream)))
+
+    def solve_device_adaptive(self, batch: abi.Batch, models, adaptive_rho: AdaptiveRho, stream=None):
+        """solve_device with adaptive rho: `models` = torch CUDA tensor [B, blob] (in/out, e.g. from pack_models), updated in
+        place with every instance's adapted rho / Kinf / Pinf."""
+        import torch
+
+        p = self.problem
+        M = int(self._lib.tinympc_b200_model_blob_elems(p.nx, p.nu))
+        if not (isinstance(models, torch.Tensor) and models.is_cuda and models.is_contiguous() and models.numel() == batch.B * M
+                and models.dtype == (torch.float32 if p.dtype == np.float32 else torch.float64)):
+            raise ValueError(f"models must be a contiguous CUDA tensor of {batch.B} x {M} elements of the problem dtype")
+        s = stream if stream is not None else torch.cuda.current_stream(self.device)
+        ar = adaptive_rho.to_c(p, models.data_ptr())
+        check(self._lib.tinympc_b200_solve_adaptive(self._h, C.byref(batch), C.byref(ar), C.c_void_p(s.cuda_stream)))
