@@ -175,8 +175,10 @@ typedef struct tinympc_batch {
     /* Heterogeneous batch (optional, SURVEY §8f-2): one model + cache per instance instead of the handle's shared one.
      * [B][tinympc_b200_model_blob_elems(nx,nu)] elements of the problem dtype, each blob =
      *   Adyn | Bdyn | fdyn | Q | R | Kinf | Pinf | Quu_inv | AmBKt | APf | BPf | rho      (column-major pieces, as in
-     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Bounds / settings stay shared.
-     * Served by the on-chip (GPI) kernel only: box constraints, horizons that fit in shared memory. */
+     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Bounds, cones, hyperplanes and settings
+     * stay shared.  Served by the lane-group kernels: the on-chip (GPI) kernel when the family is AUTO or GPI, the problem
+     * has box constraints only and the horizon fits in shared memory; otherwise (explicit GPS, cones or hyperplanes, a
+     * horizon off chip) the streamed (GPS) kernel, one instance per lane group.  TPI returns TINYMPC_ERR_UNSUPPORTED. */
     const void *models;
 } tinympc_batch_t;
 
@@ -309,6 +311,13 @@ int tinympc_b200_solve_adaptive_host(tinympc_b200_solver_t *s, const tinympc_bat
  * tinympc_b200_solve calls.
  */
 int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, void *cuda_stream);
+
+/*
+ * The same step for a heterogeneous batch: instance b is advanced with Adyn, Bdyn, fdyn of its own blob models[b]
+ * ([B][tinympc_b200_model_blob_elems(nx,nu)], layout: tinympc_batch_t.models, DEVICE pointer), same arithmetic.
+ */
+int tinympc_b200_advance_models(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *models,
+                                void *cuda_stream);
 
 /* 1 if a kernel is compiled for (dtype,nx,nu); used by callers to fail early */
 int tinympc_b200_supported(int32_t dtype, int32_t nx, int32_t nu);

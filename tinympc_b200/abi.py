@@ -113,6 +113,7 @@ EXPORTS = [
     "tinympc_b200_solve_adaptive_host",
     "tinympc_b200_get_stats",
     "tinympc_b200_advance",
+    "tinympc_b200_advance_models",
     "tinympc_b200_supported",
     "tinympc_b200_last_error",
     "tinympc_b200_version",

@@ -6,7 +6,8 @@ Mirrors the loop of the reference's examples (examples/quadrotor_tracking.cpp:77
     x0 = Adyn * x0 + Bdyn * work->u.col(0)
 
 with the whole TinyWorkspace state of every instance kept on the GPU between steps (warm start) and the plant
-update done by tinympc_b200_advance().  torch only owns the device buffers.
+update done by tinympc_b200_advance() (tinympc_b200_advance_models() for a fleet with per-instance models).  torch only
+owns the device buffers.
 """
 from __future__ import annotations
 
@@ -27,8 +28,10 @@ WARM_FIELDS_FAST = ("vnew", "znew", "g", "y")
 class DeviceMPCLoop:
     def __init__(self, solver: BatchedTinySolver, x0, reset_duals: bool = False, extra_state=(), exact_first_residual: bool = True,
                  adaptive_rho: AdaptiveRho | None = None, models=None):
-        """adaptive_rho: every plant adapts its own rho / Kinf / Pinf, kept on the device across steps in self.models
-        ([B, blob], starting from `models` or the problem's own cache), as one TinySolver per robot would."""
+        """models ([B, blob], tinympc_batch_t.models, e.g. from setup_models): a heterogeneous fleet, one model, cache and rho
+        per plant.  Every step solves with them and advances plant b with its own A, B, f (tinympc_b200_advance_models).
+        adaptive_rho: every plant adapts its own rho / Kinf / Pinf, kept on the device across steps in self.models
+        (starting from `models` or the problem's own cache), as one TinySolver per robot would."""
         import torch
 
         self.solver = solver
@@ -45,7 +48,7 @@ class DeviceMPCLoop:
         self.want_solution = True  # also return solution->x / solution->u (= vnew / znew) every step
         self.adaptive_rho = adaptive_rho
         self.models = None
-        if adaptive_rho is not None:
+        if adaptive_rho is not None or models is not None:
             m = pack_models(p, self.B) if models is None else models
             self.models = torch.as_tensor(m, dtype=self._tdt, device=self.dev).reshape(self.B, -1).contiguous().clone()
 
@@ -58,8 +61,9 @@ class DeviceMPCLoop:
         if self.state is not None and self.reset_duals:
             self.state["g"].zero_()
             self.state["y"].zero_()
+        het = self.models is not None and self.adaptive_rho is None
         batch, out = s.make_device_batch(self.x0, Xref, Uref, state=self.state, cold_start=self._first, want_state=self.fields,
-                                         want_u0=True, want_solution=self.want_solution)
+                                         want_u0=True, want_solution=self.want_solution, models=self.models if het else None)
         if self.adaptive_rho is None:
             s.solve_device(batch, stream)
         else:
@@ -68,6 +72,10 @@ class DeviceMPCLoop:
         self.out = out
         self._first = False
         st = stream if stream is not None else torch.cuda.current_stream(s.device)
-        check(s._lib.tinympc_b200_advance(s._h, self.B, C.c_void_p(self.x0.data_ptr()), C.c_void_p(out["u0"].data_ptr()),
-                                          s.problem.nu, C.c_void_p(st.cuda_stream)))
+        x0p, u0p = C.c_void_p(self.x0.data_ptr()), C.c_void_p(out["u0"].data_ptr())
+        if self.models is None:
+            check(s._lib.tinympc_b200_advance(s._h, self.B, x0p, u0p, s.problem.nu, C.c_void_p(st.cuda_stream)))
+        else:
+            check(s._lib.tinympc_b200_advance_models(s._h, self.B, x0p, u0p, s.problem.nu, C.c_void_p(self.models.data_ptr()),
+                                                     C.c_void_p(st.cuda_stream)))
         return out

@@ -24,9 +24,11 @@ TM_DIMS(TM_DECL)
 
 namespace {
 
-// x0[b] <- (A x0[b] + B u[b][:,0]) + f ; one thread per (instance, row); matrices column-major in the blob
+// x0[b] <- (A x0[b] + B u[b][:,0]) + f ; one thread per (instance, row); matrices column-major in the blob of instance b,
+// blob + b * bstride (bstride 0: one blob for every instance)
 template <typename T>
-__global__ void advance_kernel(int nx, int nu, int64_t ustride, int64_t B, const T *__restrict__ blob, T *x0, const T *__restrict__ u) {
+__global__ void advance_kernel(int nx, int nu, int64_t ustride, int64_t B, const T *__restrict__ blob, int64_t bstride, T *x0,
+                               const T *__restrict__ u) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = t < B * nx;
     T r = T(0);
@@ -34,7 +36,8 @@ __global__ void advance_kernel(int nx, int nu, int64_t ustride, int64_t B, const
         const int64_t b = t / nx;
         const int i = (int)(t - b * nx);
         const tmpc::ModelBlob mb = tmpc::model_blob(nx, nu);
-        const T *A = blob + mb.A, *Bm = blob + mb.B, *f = blob + mb.f;
+        const T *mdl = blob + b * bstride;
+        const T *A = mdl + mb.A, *Bm = mdl + mb.B, *f = mdl + mb.f;
         const T *xb = x0 + b * nx, *ub = u + b * ustride;
         T ax = A[i] * xb[0];
         for (int m = 1; m < nx; ++m) ax = ax + A[i + nx * m] * xb[m];
@@ -232,6 +235,23 @@ int resolve_family(const tinympc_b200_solver *s, const Features &ft, tmpc::GpiPl
     return TINYMPC_KERNEL_GPI;
 }
 
+// Which kernel family serves a batch with per-instance models (tinympc_batch_t.models).  The on-chip kernel, exactly as
+// without models, when the family is AUTO or GPI and the problem has box constraints only and an on-chip plan (`gpi`, from
+// resolve_family).  Otherwise the streamed kernel's per-instance-model variant: explicit GPS, cones or hyperplanes, or a
+// horizon that does not fit on chip.  One thread per instance has no such variant.  -1: not available, reason in *why.
+int models_family(const tinympc_b200_solver *s, const Features &ft, const tmpc::GpiPlan &gpi, const char **why) {
+    if (s->family == TINYMPC_KERNEL_TPI) {
+        *why = "per-instance models run on the lane-group kernel families (GPI, GPS), not on one thread per instance";
+        return -1;
+    }
+    if (s->family != TINYMPC_KERNEL_GPS && !ft.ext && gpi.smem > 0) return TINYMPC_KERNEL_GPI;
+    if (!s->dim->gps_lanes || s->dim->gps_lanes(s->dtype) <= 0) {
+        *why = "per-instance models: this problem needs the streamed lane-group kernel, which does not cover this shape";
+        return -1;
+    }
+    return TINYMPC_KERNEL_GPS;
+}
+
 // carve the TPI structure-of-arrays workspace
 int setup_workspace(tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features &ft, int64_t B, int family) {
     const int64_t Bpad = (B + 31) / 32 * 32;
@@ -402,10 +422,10 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     if (io->B <= 0) return TINYMPC_OK;
     const Features ft = features(s);
     int family = ar ? TINYMPC_KERNEL_GPI : resolve_family(s, ft, &gpi, io->B);
-    if (io->models) {  // per-instance models: on-chip kernel only
-        if (ft.ext || gpi.smem <= 0 || s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models need the on-chip GPI kernel (box constraints, horizon fitting in shared memory)");
-        family = TINYMPC_KERNEL_GPI;
+    if (io->models) {
+        const char *why = nullptr;
+        family = models_family(s, ft, gpi, &why);
+        if (family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, why);
     }
     if (family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
     // The launch scratch of a handle (work queue, workspaces, timing events) is single-buffered: a solve enqueued on a
@@ -773,8 +793,10 @@ int tinympc_b200_solve_adaptive(tinympc_b200_solver_t *s, const tinympc_batch_t 
     return enqueue(s, io, (cudaStream_t)cuda_stream, true, ar);
 }
 
-int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, void *cuda_stream) {
-    if (!s || !x0 || !u) return fail(TINYMPC_ERR_ARG, "null argument");
+namespace {
+// tinympc_b200_advance[_models]: x0[b] <- (A_b x0[b] + B_b u_b) + f_b with the model of blob + b * bstride
+int advance_impl(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *blob, int64_t bstride,
+                 void *cuda_stream) {
     if (B <= 0) return TINYMPC_OK;
     CUDA_TRY(cudaSetDevice(s->device));
     // threads per block = a multiple of nx so that all rows of an instance read x0 before any row writes it
@@ -783,11 +805,23 @@ int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const vo
     const unsigned blocks = (unsigned)((total + per - 1) / per);
     cudaStream_t st = (cudaStream_t)cuda_stream;
     if (s->dtype == TINYMPC_F32)
-        advance_kernel<float><<<blocks, per, 0, st>>>(s->nx, s->nu, u_stride, B, (const float *)s->d_blob.p, (float *)x0, (const float *)u);
+        advance_kernel<float><<<blocks, per, 0, st>>>(s->nx, s->nu, u_stride, B, (const float *)blob, bstride, (float *)x0, (const float *)u);
     else
-        advance_kernel<double><<<blocks, per, 0, st>>>(s->nx, s->nu, u_stride, B, (const double *)s->d_blob.p, (double *)x0, (const double *)u);
+        advance_kernel<double><<<blocks, per, 0, st>>>(s->nx, s->nu, u_stride, B, (const double *)blob, bstride, (double *)x0, (const double *)u);
     CUDA_TRY(cudaGetLastError());
     return TINYMPC_OK;
+}
+}  // namespace
+
+int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, void *cuda_stream) {
+    if (!s || !x0 || !u) return fail(TINYMPC_ERR_ARG, "null argument");
+    return advance_impl(s, B, x0, u, u_stride, s->d_blob.p, 0, cuda_stream);
+}
+
+int tinympc_b200_advance_models(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *models,
+                                void *cuda_stream) {
+    if (!s || !x0 || !u || !models) return fail(TINYMPC_ERR_ARG, "null argument");
+    return advance_impl(s, B, x0, u, u_stride, models, tinympc_b200_model_blob_elems(s->nx, s->nu), cuda_stream);
 }
 
 int tinympc_b200_get_stats(const tinympc_b200_solver_t *s, tinympc_b200_stats_t *out) {
@@ -910,16 +944,26 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     if (B > 16384) chunk = std::max<int64_t>(8192, (B + 7) / 8);
     chunk = (chunk + 31) / 32 * 32;
     {   // the persistent GPI kernel holds sm_count * instances_per_cta instances at a time: make a chunk a whole
-        // number of such waves so that no chunk ends on a mostly empty wave
+        // number of such waves so that no chunk ends on a mostly empty wave (per-instance models: the same for the
+        // streamed kernel's per-instance-model variant when that is what runs)
         const Features ft = features(s);
         tmpc::GpiPlan gpi;
         int fam = resolve_family(s, ft, &gpi, chunk);
+        int64_t per_cta = gpi.instances_per_cta;
+        const char *why = nullptr;
+        if (io->models && models_family(s, ft, gpi, &why) == TINYMPC_KERNEL_GPS) {
+            tmpc::LaunchDesc d;
+            base_desc(s, d, ft);
+            d.io = *io;
+            fam = TINYMPC_KERNEL_GPS;
+            per_cta = s->dim->gps_het_slots(&d);
+        }
         if (ar) {  // the adaptive kernel's own plan (its tables take shared memory)
             fam = TINYMPC_KERNEL_GPI;
-            gpi = adapt_plan;
+            per_cta = adapt_plan.instances_per_cta;
         }
-        if (fam == TINYMPC_KERNEL_GPI && B > 16384) {
-            const int64_t wave = (int64_t)s->sm_count * gpi.instances_per_cta;
+        if ((fam == TINYMPC_KERNEL_GPI || (fam == TINYMPC_KERNEL_GPS && io->models)) && B > 16384) {
+            const int64_t wave = (int64_t)s->sm_count * per_cta;
             if (wave > 0 && wave < B) chunk = std::max<int64_t>(1, (chunk + wave / 2) / wave) * wave;
         }
     }

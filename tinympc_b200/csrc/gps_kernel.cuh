@@ -193,9 +193,19 @@ __device__ __forceinline__ void stg_piece(T *p, const T (&v)[R], unsigned pr) {
     }
 }
 
-template <typename T, int NX, int NU, int L, int NI, int FAM, bool FAST>
+// Per-instance models (tinympc_batch_t.models): the kernel is instantiated with GPS_HET added to its family mask (FAMH).
+// Every instance then brings its own model / cache blob and rho.  A slot keeps a pointer to its instance's blob and the
+// sweeps read their matrix rows from it (ld.global.nc: the blobs are read-only for the launch) instead of from the CTA's
+// staged copy.  It runs one instance per lane group: the NI = 2 variant shares the matrix registers between the two
+// instances of a group, and two sets of rows do not fit.
+constexpr int GPS_HET = 8;
+
+template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     gps_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
+    constexpr bool HET = (FAMH & GPS_HET) != 0;  // per-instance models
+    constexpr int FAM = FAMH & ~GPS_HET;         // constraint families compiled in
+    static_assert(!HET || NI == 1, "per-instance models run one instance per lane group");
     using Cfg = GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAM>;
     using REC = GpsRec<NX, NU, Cfg::SPW, (int)sizeof(T), FAM>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -213,6 +223,14 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     const int l = lane % L, grp = lane / L;
     const bool has_b = P.gps.has_b != 0;
     const T rho = P.rho;
+    // HET: rho and model blob of this lane's slot, set when the slot is loaded.  A slot that never gets an instance keeps
+    // instance 0's blob, so that the row loads of idle and padding lanes stay inside a blob.
+    T rho_h = rho;
+    const T *mrow = P.models;
+    auto rho_ = [&]() -> T {
+        if constexpr (HET) return rho_h;
+        else return rho;
+    };
 
     // ---- stage the cache blob into shared memory with one TMA bulk copy per CTA, pull this lane's rows into registers
     constexpr ModelBlob MB = model_blob(NX, NU);
@@ -227,7 +245,11 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     // registers when it starts: about half the register footprint of keeping everything resident, which is what makes
     // room for the second instance per lane group.
     const unsigned aBlob = (unsigned)__cvta_generic_to_shared(stage);
-    auto bl = [&](int idx) { return lds(aBlob + (unsigned)idx * ES, T()); };
+    // element idx of the blob the sweeps read their rows from: the staged copy, or (HET) the slot's own blob in global memory
+    auto bl = [&](int idx) -> T {
+        if constexpr (HET) return __ldg(mrow + idx);
+        else return lds(aBlob + (unsigned)idx * ES, T());
+    };
     auto load_fwd_rows = [&](T (&mS1f)[RX + RU][NX], T (&mB)[RX][NU], T (&vQd)[RX], T (&vf)[RX], T (&vRd)[RU]) {
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
@@ -514,7 +536,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
                 for (int a = 0; a < RX; ++a) {
                     gfn[a] = (gf[j][a] + xo[j][a]) - sf[j][a];
-                    q[j][a] = nmac<FAST>(q[j][a], rho, sf[j][a] - gfn[a]);
+                    q[j][a] = nmac<FAST>(q[j][a], rho_(), sf[j][a] - gfn[a]);
                 }
                 stg_piece<T, RX, CX>(cx + REC::gf(F) + j * JX, gfn, pxv);
                 if (keep_f[F]) stg_piece<T, RX, CX>(wsb + (int64_t)k * recB + REC::vf(F) + (j * IPW + grp) * NX + l * RX, sf[j], pxv);
@@ -536,7 +558,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
                 for (int b = 0; b < RU; ++b) {
                     yfn[b] = (yf[j][b] + u[j][b]) - sf[j][b];
-                    r[j][b] = nmac<FAST>(r[j][b], rho, sf[j][b] - yfn[b]);
+                    r[j][b] = nmac<FAST>(r[j][b], rho_(), sf[j][b] - yfn[b]);
                 }
                 stg_piece<T, RU, CU>(cu + REC::yf(F) + j * JU, yfn, puv);
                 if (keep_f[F]) stg_piece<T, RU, CU>(wsb + (int64_t)k * recB + REC::zf(F) + (j * IPW + grp) * NU + l * RU, sf[j], puv);
@@ -620,7 +642,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                     rdx[j] = absmax(rdx[j], vo[a] - v);
                     // k < N-1: q_k = -(xref*Q) - rho (vnew - g);  k = N-1: p_{N-1} = -(Pinf^T xref) - rho (vnew - g)
                     const T base = HASU ? -(xrf[a] * vQd[a]) : pt[a];
-                    q[j][a] = nmac<FAST>(base, rho, v - gn[a]);
+                    q[j][a] = nmac<FAST>(base, rho_(), v - gn[a]);
                 }
                 stg_piece<T, RX, CX>(cx + REC::vnew + j * JX, vn, pxv);
                 stg_piece<T, RX, CX>(cx + REC::g + j * JX, gn, pxv);
@@ -641,7 +663,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                         rpu[j] = absmax(rpu[j], u[j][b] - z);
                         rdu[j] = absmax(rdu[j], zo[b] - z);
                         const T urb = has_uref ? urf[b] : T(0);
-                        r[j][b] = nmac<FAST>(-(urb * vRd[b]), rho, z - yn[b]);
+                        r[j][b] = nmac<FAST>(-(urb * vRd[b]), rho_(), z - yn[b]);
                     }
                     stg_piece<T, RU, CU>(cu + REC::znew + j * JU, zn, puv);
                     stg_piece<T, RU, CU>(cu + REC::y + j * JU, yn, puv);
@@ -670,7 +692,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
                             for (int a = 0; a < RX; ++a) {
                                 gfn[a] = (gf[j][a] + xo[j][a]) - sx[j][a];
-                                q[j][a] = nmac<FAST>(q[j][a], rho, sx[j][a] - gfn[a]);
+                                q[j][a] = nmac<FAST>(q[j][a], rho_(), sx[j][a] - gfn[a]);
                             }
                             stg_piece<T, RX, CX>(cx + REC::gf(0) + j * JX, gfn, pxv);
                             if (keep_f[0]) stg_piece<T, RX, CX>(wsb + (int64_t)k * recB + REC::vf(0) + (j * IPW + grp) * NX + l * RX, sx[j], pxv);
@@ -680,7 +702,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
                             for (int b = 0; b < RU; ++b) {
                                 yfn[b] = (yf[j][b] + u[j][b]) - su[j][b];
-                                r[j][b] = nmac<FAST>(r[j][b], rho, su[j][b] - yfn[b]);
+                                r[j][b] = nmac<FAST>(r[j][b], rho_(), su[j][b] - yfn[b]);
                             }
                             stg_piece<T, RU, CU>(cu + REC::yf(0) + j * JU, yfn, puv);
                             if (keep_f[0]) stg_piece<T, RU, CU>(wsb + (int64_t)k * recB + REC::zf(0) + (j * IPW + grp) * NU + l * RU, su[j], puv);
@@ -792,6 +814,13 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
         const int64_t ox = ib * (int64_t)N * NX, ou = ib * (int64_t)(N - 1) * NU;
         const T *xrefb = P.Xref + (P.xref_pi ? ox : 0);
         const T *urefb = has_uref ? P.Uref + (P.uref_pi ? ou : 0) : nullptr;
+        // model and rho of the instance being loaded: the handle's cache blob, or (HET) the instance's own blob
+        const T *mbl = gmat;
+        T rho_l = rho;
+        if constexpr (HET) {
+            mbl = P.models + ib * (int64_t)MB.model;
+            rho_l = __ldg(mbl + MB.rho);
+        }
         const T *const sgf[3] = {P.s_gc, P.s_gl, P.s_gl_tv};
         const T *const syf[3] = {P.s_yc, P.s_yl, P.s_yl_tv};
         for (int e = lane; e < N * NX; e += 32) {
@@ -801,12 +830,12 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             const T v_in = (!cold && P.s_v) ? P.s_v[ox + e] : T(0);
             T acc;
             if (k < N - 1) {
-                acc = -(__ldg(xrefb + e) * __ldg(gmat + MB.Qd + i));
+                acc = -(__ldg(xrefb + e) * __ldg(mbl + MB.Qd + i));
             } else {  // -(Pinf^T xref_{N-1})(i), m ascending
                 const T *xl = xrefb + (int64_t)(N - 1) * NX;
-                acc = terminal_cost<FAST, NX>([&](int m) { return __ldg(xl + m); }, gmat + MB.Pinf, i);
+                acc = terminal_cost<FAST, NX>([&](int m) { return __ldg(xl + m); }, mbl + MB.Pinf, i);
             }
-            acc = nmac<FAST>(acc, rho, vnew_in - g_in);
+            acc = nmac<FAST>(acc, rho_l, vnew_in - g_in);
             T *r_ = wsw + (int64_t)k * recA + sidx * NX + i;
             T *rb_ = wsb + (int64_t)k * recB + sidx * NX + i;
             r_[REC::vnew] = v_in;  // the slot of the box slack holds work->v until the first forward sweep rewrites it
@@ -817,7 +846,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                 for (int f = 0; f < 3; ++f) {
                     if (((FAM >> f) & 1) && fx[f]) {
                         const T gf_in = (!cold && sgf[f]) ? sgf[f][ox + e] : T(0);
-                        acc = nmac<FAST>(acc, rho, xin - gf_in);
+                        acc = nmac<FAST>(acc, rho_l, xin - gf_in);
                         r_[REC::gf(f)] = gf_in;
                         if (keep_f[f]) rb_[REC::vf(f)] = xin;
                     }
@@ -831,7 +860,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             const T y_in = (!cold && P.s_y) ? P.s_y[ou + e] : T(0);
             const T z_in = (!cold && P.s_z) ? P.s_z[ou + e] : T(0);
             const T ur = has_uref ? __ldg(urefb + e) : T(0);
-            T acc = nmac<FAST>(-(ur * __ldg(gmat + MB.Rd + j)), rho, znew_in - y_in);
+            T acc = nmac<FAST>(-(ur * __ldg(mbl + MB.Rd + j)), rho_l, znew_in - y_in);
             T *r_ = wsw + (int64_t)k * recA + sidx * NU + j;
             T *rb_ = wsb + (int64_t)k * recB + sidx * NU + j;
             r_[REC::znew] = z_in;
@@ -842,7 +871,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                 for (int f = 0; f < 3; ++f) {
                     if (((FAM >> f) & 1) && fu[f]) {
                         const T yf_in = (!cold && syf[f]) ? syf[f][ou + e] : T(0);
-                        acc = nmac<FAST>(acc, rho, uin - yf_in);
+                        acc = nmac<FAST>(acc, rho_l, uin - yf_in);
                         r_[REC::yf(f)] = yf_in;
                         if (keep_f[f]) rb_[REC::zf(f)] = uin;
                     }
@@ -855,13 +884,17 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             busy[J] = true;
             it[J] = 0;
             solved[J] = 0;
+            if constexpr (HET) {
+                rho_h = rho_l;
+                mrow = mbl;
+            }
             const T *xl = xrefb + (int64_t)(N - 1) * NX;
             T x0v[RX], ptv[RX];
 #pragma unroll
             for (int a = 0; a < RX; ++a) {
                 const int ii = xvl ? l * RX + a : 0;
                 x0v[a] = xvl ? __ldg(P.x0 + ib * NX + ii) : T(0);
-                const T pt = terminal_cost<FAST, NX>([&](int m) { return __ldg(xl + m); }, gmat + MB.Pinf, ii);
+                const T pt = terminal_cost<FAST, NX>([&](int m) { return __ldg(xl + m); }, mbl + MB.Pinf, ii);
                 ptv[a] = xvl ? pt : T(0);
             }
             sts_piece<T, RX, SX>(aPark + (unsigned)((2 * J) * RX) * ES, x0v);
@@ -1046,7 +1079,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                 if (busy[j]) {
                     it[j] += 1;
                     if (it[j] % P.check_termination == 0) {
-                        const T r_px = a, r_dx = b * rho, r_pu = c, r_du = d * rho;
+                        const T r_px = a, r_dx = b * rho_(), r_pu = c, r_du = d * rho_();
                         if (l == 0 && P.residuals) {
                             T *r4 = P.residuals + 4 * inst[j];
                             r4[0] = r_px; r4[1] = r_dx; r4[2] = r_pu; r4[3] = r_du;
@@ -1104,16 +1137,17 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     return p;
 }
 
-template <typename T, int NX, int NU, int L, int NI, int FAM, bool FAST>
+// FAMH: family mask, plus GPS_HET for per-instance models
+template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
-    const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAM>(*d);
+    const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH & ~GPS_HET>(*d);
     if (plan.L == 0 || !d->gmat || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     d->out_ws_need = plan.ws_bytes;
     if (!d->gps_ws || d->gps_ws_bytes < plan.ws_bytes) return TM_ERR_WORKSPACE;
     KParams<T, NX, NU> P = P0;
     P.gps = plan.ly;
     P.gps_ws = (T *)d->gps_ws;
-    auto kern = gps_solve_kernel<T, NX, NU, L, NI, FAM, FAST>;
+    auto kern = gps_solve_kernel<T, NX, NU, L, NI, FAMH, FAST>;
     if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
     kern<<<plan.ctas, plan.warps * 32, plan.smem, d->stream>>>(P, (const T *)d->gmat, (unsigned long long *)d->work_queue);
     return launch_done(d, plan.warps * 32, plan.ctas, plan.smem, L, plan.warps * (32 / L) * NI);
@@ -1133,6 +1167,16 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     } else {
         constexpr int NIP = gps_pick_NI<T, NX, NU, L>();
         const int fam = gps_family_mask(*d);
+        if (d->io.models) {  // per-instance models: one instance per lane group, the same family variants
+#define TM_GPS_HET_CASE(FF) \
+    if (fam == FF) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_HET, FAST>(d, P0);
+            TM_GPS_HET_CASE(0)
+            TM_GPS_HET_CASE(1)
+            TM_GPS_HET_CASE(6)
+            TM_GPS_HET_CASE(7)
+#undef TM_GPS_HET_CASE
+            return TINYMPC_ERR_UNSUPPORTED;
+        }
         int ni = gps_env_int("TINYMPC_GPS_NI", NIP);
         if (ni != 1 && ni != 2) ni = NIP;
         if (ni > NIP) ni = NIP;
@@ -1157,6 +1201,27 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
         TM_GPS_CASE(7)
 #undef TM_GPS_CASE
         return TINYMPC_ERR_UNSUPPORTED;
+    }
+}
+
+// instances one CTA of the per-instance-model variant holds when the batch fills every SM (the host path rounds its chunks to
+// whole waves of these); 0 = shape not available
+template <typename T, int NX, int NU>
+int gps_het_slots(const LaunchDesc &d0) {
+    constexpr int L = gps_pick_L<T, NX, NU>();
+    if constexpr (L == 0) {
+        return 0;
+    } else {
+        LaunchDesc d = d0;
+        d.sm_count = 1;
+        d.io.B = (int64_t)1 << 40;
+        const int fam = gps_family_mask(d);
+        GpsPlan p;
+        if (fam == 0) p = gps_plan_L<T, NX, NU, L, 1, 0>(d);
+        else if (fam == 1) p = gps_plan_L<T, NX, NU, L, 1, 1>(d);
+        else if (fam == 6) p = gps_plan_L<T, NX, NU, L, 1, 6>(d);
+        else p = gps_plan_L<T, NX, NU, L, 1, 7>(d);
+        return p.L ? p.warps * (32 / L) : 0;
     }
 }
 

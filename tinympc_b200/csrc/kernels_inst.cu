@@ -24,6 +24,7 @@ extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d);
 extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin);
 extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d);
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype);
+extern "C" int TM_SYM(tm_gps_het_slots_)(const tmpc::LaunchDesc *d);
 
 #if TM_PART == 0
 // =========================================================================================================
@@ -46,7 +47,7 @@ int launch_tpi(LaunchDesc *d) {
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->io.models) return TINYMPC_ERR_UNSUPPORTED;  // per-instance models live in the on-chip kernel's per-lane registers only
+    if (d->io.models) return TINYMPC_ERR_UNSUPPORTED;  // per-instance models: the lane-group kernels only
     if (d->ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
     return d->fast ? launch_tpi<T, true, false>(d) : launch_tpi<T, false, false>(d);
 }
@@ -77,7 +78,8 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
                                      &tmpc::launch,
                                      &TM_SYM(tm_gpi_plan_),
                                      &tmpc::precompute_batch,
-                                     &TM_SYM(tm_gps_lanes_)};
+                                     &TM_SYM(tm_gps_lanes_),
+                                     &TM_SYM(tm_gps_het_slots_)};
     return &e;
 }
 
@@ -168,9 +170,9 @@ extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_opt
 namespace tmpc {
 namespace {
 
+// io.models set: the per-instance-model variant (launch_gps)
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->io.models) return TINYMPC_ERR_UNSUPPORTED;
     KParams<T, TM_NX, TM_NU> P;
     fill_params<T, TM_NX, TM_NU>(P, *d);
     return d->fast ? launch_gps<T, TM_NX, TM_NU, true>(d, P) : launch_gps<T, TM_NX, TM_NU, false>(d, P);
@@ -194,5 +196,10 @@ extern "C" int TM_SYM(tm_gps_lanes_)(int dtype) {
         else return L | (tmpc::gps_pick_NI<T, TM_NX, TM_NU, L>() << 8);
     };
     return dtype == TINYMPC_F32 ? lanes(0.f) : (dtype == TINYMPC_F64 ? lanes(0.0) : 0);
+}
+extern "C" int TM_SYM(tm_gps_het_slots_)(const tmpc::LaunchDesc *d) {
+    if (d->dtype == TINYMPC_F32) return tmpc::gps_het_slots<float, TM_NX, TM_NU>(*d);
+    if (d->dtype == TINYMPC_F64) return tmpc::gps_het_slots<double, TM_NX, TM_NU>(*d);
+    return 0;
 }
 #endif

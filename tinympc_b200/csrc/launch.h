@@ -94,6 +94,9 @@ struct DimEntry {
                             const void *rho, void *models_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);
     // streamed lane-group kernel (gps_kernel.cuh): lanes per instance (bits 0-7) | instances per lane group << 8; 0 = shape not available
     int (*gps_lanes)(int dtype);
+    // its per-instance-model variant (io.models): instances per CTA when the batch fills every SM, for the shape and the
+    // constraint families of `d`; 0 = not available
+    int (*gps_het_slots)(const LaunchDesc *d);
 };
 
 }  // namespace tmpc

@@ -78,6 +78,19 @@ def rocket(N=100, cones=True) -> ModelSpec:
     return ModelSpec("rocket_20hz", 6, 3, N, float(d["rho"]), d["A"], d["B"], d["f"], d["Q"], d["R"], cons, s)
 
 
+def rocket_fleet(B, N=100, seed=0, mass_spread=0.2) -> dict:
+    """A fleet of B rockets of different masses: the 20 Hz rocket's model with instance b's input matrix scaled by 1/m_b,
+    m_b = 1 + mass_spread * U(-1, 1) (the thrust acts on a heavier or lighter vehicle; gravity in f does not depend on
+    the mass).  -> per-instance A [B,nx,nx], B [B,nx,nu], f [B,nx], Qdiag [B,nx], Rdiag [B,nu], rho [B] (the arguments
+    of solver.setup_models), the masses m, and the shared spec (constraints, settings) of rocket(N)."""
+    spec = rocket(N=N)
+    rng = np.random.default_rng(seed)
+    m = 1.0 + mass_spread * rng.uniform(-1.0, 1.0, size=B)
+    tile = lambda a: np.tile(np.asarray(a, dtype=np.float64)[None], (B,) + (1,) * np.ndim(a))  # noqa: E731
+    return dict(A=tile(spec.A), B=tile(spec.B) / m[:, None, None], f=tile(spec.f), Qdiag=tile(spec.Qdiag),
+                Rdiag=tile(spec.Rdiag), rho=np.full(B, spec.rho), m=m, spec=spec)
+
+
 def random_lti(nx, nu, N, seed=0) -> ModelSpec:
     """SURVEY §8d C5 generator: A = I + 0.05 G rescaled to spectral radius 1, B ~ N(0, 0.1^2)."""
     rng = np.random.default_rng(1000003 * seed + 7919 * nx + 104729 * nu)
