@@ -350,6 +350,39 @@ def test_max_iter_zero_returns_the_warm_state(kernel):
     assert (g["iter"] == 0).all() and H.bits_equal(g["sol_x"], first["vnew"])
 
 
+@pytest.mark.parametrize("dt", [np.float32, np.float64])
+@pytest.mark.parametrize("dims", [(4, 1), (4, 2), (6, 3), (12, 2), (12, 4), (16, 2), (16, 8)])
+def test_warm_first_iteration_residuals(dims, dt):
+    """max_iter = 1 on a warm start with work->v / work->z: the reported residuals are the first iteration's, whose dual
+    parts compare the new slacks with the caller's v / z.  The on-chip kernel stages v / z in pack layout, padding rows
+    included (shapes whose rows do not fill the lane group: (4,1), (16,2), and (12,4) / (16,8) in fp64 at L = 16).  The
+    scratch is first filled by a solve of other instances, so stale values in the padding rows would show."""
+    nx, nu = dims
+    spec = wl.random_lti(nx, nu, 50, seed=7 * nx + nu)
+    prob = setup_problem(spec, dt)
+    st = abi.Settings.from_buffer_copy(spec.settings)
+    st.max_iter = 12
+    B = 45
+    inst = wl.random_instances(B, nx, 50, seed=nx + nu, dtype=dt)
+    inst["x0"] = (3.0 * inst["x0"]).astype(dt)
+    want = tuple(H.BOX_STATE)
+    o1 = _port(prob, st, inst["x0"], inst["Xref"], None, None, True, want)
+    st1 = abi.Settings.from_buffer_copy(st)
+    st1.max_iter = 1
+    state = {n: o1[n].copy() for n in H.BOX_STATE}
+    x0b = (inst["x0"] * dt(0.9)).astype(dt)
+    o2 = _port(prob, st1, x0b, inst["Xref"], None, {n: a.copy() for n, a in state.items()}, False, want)
+    for kernel in ("gpi", "gps", "tpi"):
+        solver = _mk_solver(prob, st, kernel)
+        other = wl.random_instances(B, nx, 50, seed=99, dtype=dt)  # leaves its own slacks in the v / z scratch
+        solver.solve((5.0 * other["x0"]).astype(dt), other["Xref"], None, cold_start=True, want_state=want)
+        solver.update_settings(max_iter=1)
+        g = solver.solve(x0b, inst["Xref"], None, state={n: a.copy() for n, a in state.items()}, cold_start=False,
+                         want_state=want)
+        for key in H.OUT_KEYS + H.BOX_STATE:
+            assert H.bits_equal(g[key], o2[key]), (dims, kernel, key)
+
+
 @pytest.mark.parametrize("kernel", ALLK)
 @pytest.mark.parametrize("N", [2, 3, 5])
 def test_tiny_horizons(N, kernel):

@@ -398,7 +398,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     na[a] = v;
                     nb[a] = (pb[a] + xo[a]) - v;
                     rpx = absmax(rpx, xo[a] - v);
-                    rdx = absmax(rdx, vo - v);
+                    if (xv[a]) rdx = absmax(rdx, vo - v);  // padding rows: see the STRICT branch below
                 }
                 if (HASU) {
     #pragma unroll
@@ -411,7 +411,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                         na[RX + b] = z;
                         nb[RX + b] = (pb[RX + b] + u[b]) - z;
                         rpu = absmax(rpu, u[b] - z);
-                        rdu = absmax(rdu, zo - z);
+                        if (uv[b]) rdu = absmax(rdu, zo - z);
                     }
                 }
             } else {
@@ -451,7 +451,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     na[a] = v[a];
                     nb[a] = dg[a];
                     rpx = absmax(rpx, dx[a]);
-                    rdx = absmax(rdx, dv[a]);
+                    // padding rows (shapes whose rows do not fill the lane group) are left out of the dual residuals: their
+                    // slack is the same in every iteration, but the caller's work->v / work->z of a warm start's first
+                    // iteration has no padding rows to compare it with.  Exact shapes: xv / uv are constant true.
+                    if (xv[a]) rdx = absmax(rdx, dv[a]);
                 }
                 if (HASU) {
 #pragma unroll
@@ -459,7 +462,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                         na[RX + b] = v[RX + b];
                         nb[RX + b] = dg[RX + b];
                         rpu = absmax(rpu, dx[RX + b]);
-                        rdu = absmax(rdu, dv[RX + b]);
+                        if (uv[b]) rdu = absmax(rdu, dv[RX + b]);
                     }
                 }
             }
