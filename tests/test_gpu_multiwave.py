@@ -5,7 +5,6 @@
     instance a moment ago (state zeroed or warm-loaded, v-scratch staged, per-instance model rows re-read, counters reset).
   * tinympc_b200_solve_host cuts a batch into chunks over three pipeline slots and DMAs straight to / from page-locked
     caller buffers.
-  * TINYMPC_TPI_CHUNK sub-batches a thread-per-instance solve through slice_batch.
 
 Every test sizes its batch from the launch plan (a one-iteration probe solve), asserts that the batch really spans
 several waves in ONE launch (or the expected number of chunks), that instances of a warp retire at different iterations
@@ -472,35 +471,3 @@ def test_disabled_family_state_fields_left_alone(case, kernel, monkeypatch):
         _check(r, o2, want, f"{case} {kernel} {path} warm")
         H.assert_bits_per_instance(r, {n: poisoned(n) for n in off}, off, f"{case} {kernel} {path} warm: disabled families")
 
-
-# ---------------------------------------------------------------------------------------------------------------------
-# F. thread per instance, sub-batched (slice_batch)
-# ---------------------------------------------------------------------------------------------------------------------
-TPI_CASES = {
-    "soc_rocket_N20_f64": (lambda: _rocket(np.float64), lambda B, N, dt: _rocket_instances(B, N, dt, seed=22), H.SOC_STATE),
-    "tvlin_quad_f32": (lambda: _hyperplanes(True, np.float32), lambda B, N, dt: _hyperplane_instances(B, N, dt, seed=23), H.TVLIN_STATE),
-}
-
-
-@pytest.mark.parametrize("case", list(TPI_CASES))
-def test_tpi_sub_batches(case, monkeypatch):
-    """TINYMPC_TPI_CHUNK=128 solves B = 700 in six launches over slice_batch views: every state field (x-shaped and u-shaped
-    alternate in tinympc_state_t) must be advanced by its own per-instance size."""
-    monkeypatch.setenv("TINYMPC_TPI_CHUNK", "128")
-    make, gen, want = TPI_CASES[case]
-    prob, st = make()
-    B = 700
-    inst = gen(B, prob.N, prob.dtype)
-    port = _port(prob, st)
-    solver = BatchedTinySolver(prob, st, kernel=abi.KERNEL_TPI)
-    o1 = port(inst["x0"], inst["Xref"], inst["Uref"], None, True, want)
-    H.assert_mixed_termination(o1)
-    g1, stt = _device_solve(solver, inst["x0"], inst["Xref"], inst["Uref"], None, True, want)
-    assert stt["kernel_family"] == abi.KERNEL_TPI and stt["kernel_launches"] == 6, stt
-    _check(g1, o1, want, f"tpi {case} cold")
-    x0b, state = _warm_inputs(inst["x0"], o1, want, seed=24)
-    o2 = port(x0b, inst["Xref"], inst["Uref"], state, False, want)
-    H.assert_mixed_termination(o2)
-    g2, stt = _device_solve(solver, x0b, inst["Xref"], inst["Uref"], state, False, want)
-    assert stt["kernel_launches"] == 6, stt
-    _check(g2, o2, want, f"tpi {case} warm")

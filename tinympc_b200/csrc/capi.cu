@@ -124,8 +124,7 @@ struct tinympc_b200_solver {
     int nx = 0, nu = 0, N = 0, dtype = 0;
     double rho = 0;
     const tmpc::DimEntry *dim = nullptr;
-    // host copies (native dtype, column-major)
-    std::vector<char> A, Bm, f, Qd, Rd, Kinf, Pinf, Quu, AmBKt, APf, BPf;
+    std::vector<char> blob;  // host copy of the cache blob (model_blob.h), the bytes of d_blob
     std::vector<char> h_xlo, h_xhi, h_ulo, h_uhi;  // column 0 of the bounds
     bool has_xb = false, has_ub = false;
     int ncx = 0, ncu = 0, nlx = 0, nlu = 0, ntvx = 0, ntvu = 0;
@@ -201,62 +200,89 @@ int check_ready(const tinympc_b200_solver *s) {
     return 0;
 }
 
-// Which kernel family serves a solve.  GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane mapping covers); TPI = one thread per instance.
-// `gpi_out`: the on-chip kernel's launch plan (L == 0: not available).  Returns -1 when an explicit request cannot be
-// honoured.
-int resolve_family(const tinympc_b200_solver *s, const Features &ft, tmpc::GpiPlan *gpi_out, int64_t B = 0) {
-    tmpc::GpiPlan gpi;
-    if (!ft.ext && s->dim->gpi_plan) gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin);
-    const bool gpi_ok = gpi.smem > 0;
-    if (gpi_out) *gpi_out = gpi;
-    const bool gps_ok = s->dim->gps_lanes && s->dim->gps_lanes(s->dtype) > 0;
-    if (s->family == TINYMPC_KERNEL_GPI) return gpi_ok ? TINYMPC_KERNEL_GPI : (gps_ok ? TINYMPC_KERNEL_GPS : -1);
-    if (s->family == TINYMPC_KERNEL_GPS) return gps_ok ? TINYMPC_KERNEL_GPS : -1;
-    if (s->family == TINYMPC_KERNEL_TPI) return TINYMPC_KERNEL_TPI;
-    // AUTO (measured rules; evidence: tools/auto_rule_sweep.py, DESIGN.md §5)
-    const bool big_batch = B >= (int64_t)s->sm_count * 384;  // one thread per instance fills the GPU
-    // cones / hyperplanes: streamed lane groups
-    if (ft.ext) return gps_ok ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI;
-    // box constraints, streamed alternative when the state does not stay on chip: one thread per instance for big batches
-    // (it beats the streamed lane groups on every measured shape, fp64 (6,3,100) included: 60.0 vs 63.9 ms); small batches
-    // cannot fill the GPU with one thread per instance
-    const int streamed = (gps_ok && !big_batch) ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI;
-    if (!gpi_ok) return streamed;
-    // Big batches leave the chip when shared memory holds too few instances per SM, except for (16,8), where the
-    // thread-per-instance register footprint costs more than the low on-chip occupancy.  Measured on H100 (B = 131 072 fp32 /
-    // 65 536 fp64, 50 iterations): fp32 on chip wins from 16 instances per SM on ((12,8,50): 45 vs 69 ms thread per instance;
-    // (12,4,100): 85 vs 94 ms) and loses at 8 ((4,8,100): 128 vs 78 ms); fp64 (rows re-read per sweep) on chip wins with three
-    // warps per SM ((4,2,50): 13 vs 19 ms; (16,8,50): 80 vs 197 ms) unless they hold only 6 instances ((12,4,50): 73 vs 60 ms),
-    // and loses badly with one warp ((6,3,100): 143 vs 60 ms thread per instance).
-    const int ipc = gpi.instances_per_cta, gpi_warps = gpi.warps;
-    const bool tpi_heavy = s->nx >= 16 && s->nu >= 8;
-    const bool few = s->dtype == TINYMPC_F64 ? (gpi_warps < 2 || ipc < 8) : ipc < 16;
-    if (ipc > 0 && few && !tpi_heavy && big_batch) return streamed;
-    return TINYMPC_KERNEL_GPI;
+// How a solve runs: the kernel family, the on-chip kernel's launch plan, and the instances one CTA holds when the batch fills
+// every SM (the host path rounds its chunks to whole waves of these).
+struct SolvePlan {
+    int family = -1;
+    tmpc::GpiPlan gpi;    // L == 0: no on-chip plan
+    int64_t per_cta = 0;  // 0: chunks are not rounded
+};
+
+// shared memory the adaptive kernel adds per CTA for its tables
+size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->nx, s->nu, esize(s->dtype)); }
+
+// The plan of a solve of B instances (io->models: per-instance models; ar: adaptive rho, or null).  GPI = lane groups, state
+// on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane
+// mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature cannot be served.
+int plan_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar, int64_t B, SolvePlan *p) {
+    const Features ft = features(s);
+    if (ar) {  // adaptive rho: the on-chip kernel's adaptive variant, whose tables take shared memory
+        if (io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
+        if (!ar->models || !ar->dKinf_drho || !ar->dPinf_drho || ar->reserved != 0)
+            return fail(TINYMPC_ERR_ARG, "adaptive rho: models, dKinf_drho and dPinf_drho are required and reserved must be 0");
+        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho is available in STRICT mode only");
+        if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho covers box constraints only (no cones or hyperplanes)");
+        if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
+            return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs on the on-chip (GPI) kernel family only");
+        const size_t tables = adapt_smem(s);
+        p->gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin - (int)tables);
+        if (p->gpi.smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho: the horizon does not fit the on-chip kernel");
+        p->gpi.smem += tables;
+        p->family = TINYMPC_KERNEL_GPI;
+        p->per_cta = p->gpi.instances_per_cta;
+        return 0;
+    }
+    if (!ft.ext) p->gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin);
+    const bool gpi_ok = p->gpi.smem > 0;
+    const bool gps_ok = s->dim->gps_lanes(s->dtype) > 0;
+    if (s->family == TINYMPC_KERNEL_GPI) {
+        p->family = gpi_ok ? TINYMPC_KERNEL_GPI : (gps_ok ? TINYMPC_KERNEL_GPS : -1);
+    } else if (s->family == TINYMPC_KERNEL_GPS) {
+        p->family = gps_ok ? TINYMPC_KERNEL_GPS : -1;
+    } else if (s->family == TINYMPC_KERNEL_TPI) {
+        p->family = TINYMPC_KERNEL_TPI;
+    } else if (ft.ext) {  // AUTO (measured rules; evidence: tools/auto_rule_sweep.py, DESIGN.md §5).  Cones / hyperplanes: streamed lane groups
+        p->family = gps_ok ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI;
+    } else {
+        const bool big_batch = B >= (int64_t)s->sm_count * 384;  // one thread per instance fills the GPU
+        // box constraints, streamed alternative when the state does not stay on chip: one thread per instance for big batches
+        // (it beats the streamed lane groups on every measured shape, fp64 (6,3,100) included: 60.0 vs 63.9 ms); small batches
+        // cannot fill the GPU with one thread per instance
+        const int streamed = (gps_ok && !big_batch) ? TINYMPC_KERNEL_GPS : TINYMPC_KERNEL_TPI;
+        // Big batches leave the chip when shared memory holds too few instances per SM, except for (16,8), where the
+        // thread-per-instance register footprint costs more than the low on-chip occupancy.  Measured on H100 (B = 131 072 fp32 /
+        // 65 536 fp64, 50 iterations): fp32 on chip wins from 16 instances per SM on ((12,8,50): 45 vs 69 ms thread per instance;
+        // (12,4,100): 85 vs 94 ms) and loses at 8 ((4,8,100): 128 vs 78 ms); fp64 (rows re-read per sweep) on chip wins with three
+        // warps per SM ((4,2,50): 13 vs 19 ms; (16,8,50): 80 vs 197 ms) unless they hold only 6 instances ((12,4,50): 73 vs 60 ms),
+        // and loses badly with one warp ((6,3,100): 143 vs 60 ms thread per instance).
+        const int ipc = p->gpi.instances_per_cta;
+        const bool tpi_heavy = s->nx >= 16 && s->nu >= 8;
+        const bool few = s->dtype == TINYMPC_F64 ? (p->gpi.warps < 2 || ipc < 8) : ipc < 16;
+        p->family = (!gpi_ok || (ipc > 0 && few && !tpi_heavy && big_batch)) ? streamed : TINYMPC_KERNEL_GPI;
+    }
+    if (p->family == TINYMPC_KERNEL_GPI) p->per_cta = p->gpi.instances_per_cta;
+    // Per-instance models: the on-chip kernel, exactly as without models, when the family is AUTO or GPI and the problem has
+    // box constraints only and an on-chip plan (per_cta is left as the rules above set it: the host path rounds such chunks
+    // by the family a shared model would get).  Otherwise the streamed kernel's per-instance-model variant: explicit GPS,
+    // cones or hyperplanes, or a horizon that does not fit on chip.  One thread per instance has no such variant.
+    if (io->models) {
+        if (s->family == TINYMPC_KERNEL_TPI)
+            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models run on the lane-group kernel families (GPI, GPS), not on one thread per instance");
+        if (s->family != TINYMPC_KERNEL_GPS && !ft.ext && gpi_ok) {
+            p->family = TINYMPC_KERNEL_GPI;
+        } else {
+            if (!gps_ok) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models: this problem needs the streamed lane-group kernel, which does not cover this shape");
+            p->family = TINYMPC_KERNEL_GPS;
+            p->per_cta = s->dim->gps_het_slots(s->dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, s->max_smem_optin);
+        }
+    }
+    if (p->family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
+    return 0;
 }
 
-// Which kernel family serves a batch with per-instance models (tinympc_batch_t.models).  The on-chip kernel, exactly as
-// without models, when the family is AUTO or GPI and the problem has box constraints only and an on-chip plan (`gpi`, from
-// resolve_family).  Otherwise the streamed kernel's per-instance-model variant: explicit GPS, cones or hyperplanes, or a
-// horizon that does not fit on chip.  One thread per instance has no such variant.  -1: not available, reason in *why.
-int models_family(const tinympc_b200_solver *s, const Features &ft, const tmpc::GpiPlan &gpi, const char **why) {
-    if (s->family == TINYMPC_KERNEL_TPI) {
-        *why = "per-instance models run on the lane-group kernel families (GPI, GPS), not on one thread per instance";
-        return -1;
-    }
-    if (s->family != TINYMPC_KERNEL_GPS && !ft.ext && gpi.smem > 0) return TINYMPC_KERNEL_GPI;
-    if (!s->dim->gps_lanes || s->dim->gps_lanes(s->dtype) <= 0) {
-        *why = "per-instance models: this problem needs the streamed lane-group kernel, which does not cover this shape";
-        return -1;
-    }
-    return TINYMPC_KERNEL_GPS;
-}
-
-// carve the TPI structure-of-arrays workspace
-int setup_workspace(tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features &ft, int64_t B, int family) {
-    const int64_t Bpad = (B + 31) / 32 * 32;
-    d.Bpad = Bpad;
-    if (family != TINYMPC_KERNEL_TPI) return 0;
+// carve the TPI structure-of-arrays workspace for d.Bpad instances
+int setup_workspace(tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features &ft) {
+    const int64_t Bpad = d.Bpad;
     const int E = s->dtype == TINYMPC_F64 ? 2 : 4;
     const size_t nxv = (s->nx + E - 1) / E, nuv = (s->nu + E - 1) / E;
     const size_t szx = (size_t)s->N * nxv * 16 * Bpad, szu = (size_t)(s->N - 1) * nuv * 16 * Bpad;
@@ -276,7 +302,6 @@ int setup_workspace(tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features 
     };
     d.w_v[0] = take(szx); d.w_v[1] = take(szx); d.w_g = take(szx);
     d.w_z[0] = take(szu); d.w_z[1] = take(szu); d.w_y = take(szu); d.w_d = take(szu);
-    d.w_vc = d.w_gc = d.w_zc = d.w_yc = d.w_vl = d.w_gl = d.w_zl = d.w_yl = d.w_vlt = d.w_glt = d.w_zlt = d.w_ylt = nullptr;
     if (ft.soc_x) { d.w_vc = take(szx); d.w_gc = take(szx); }
     if (ft.soc_u) { d.w_zc = take(szu); d.w_yc = take(szu); }
     if (ft.lin_x) { d.w_vl = take(szx); d.w_gl = take(szx); }
@@ -287,13 +312,11 @@ int setup_workspace(tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features 
 }
 
 void base_desc(const tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features &ft) {
-    std::memset(&d, 0, sizeof(d));
+    d = tmpc::LaunchDesc{};
     d.dtype = s->dtype;
     d.fast = s->mode == TINYMPC_MODE_FAST;
     d.ext = ft.ext;
-    d.A = s->A.data(); d.Bm = s->Bm.data(); d.f = s->f.data(); d.Qd = s->Qd.data(); d.Rd = s->Rd.data();
-    d.Kinf = s->Kinf.data(); d.Pinf = s->Pinf.data(); d.Quu = s->Quu.data(); d.AmBKt = s->AmBKt.data();
-    d.APf = s->APf.data(); d.BPf = s->BPf.data();
+    d.h_blob = s->blob.data();
     d.rho = s->rho;
     const tinympc_settings_t &st = s->settings;
     d.pri_tol = st.abs_pri_tol; d.dua_tol = st.abs_dua_tol;
@@ -317,60 +340,6 @@ void base_desc(const tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features
     d.h_ulo = s->h_ulo.empty() ? nullptr : s->h_ulo.data(); d.h_uhi = s->h_uhi.empty() ? nullptr : s->h_uhi.data();
     d.sm_count = s->sm_count;
     d.max_smem_optin = s->max_smem_optin;
-}
-
-// view of a (device) batch restricted to instances [b0, b0+nb)
-tinympc_batch_t slice_batch(const tinympc_b200_solver *s, const tinympc_batch_t &io, int64_t b0, int64_t nb) {
-    const size_t es = esize(s->dtype);
-    const size_t bx = es * s->nx * s->N, bu = es * s->nu * (s->N - 1);
-    tinympc_batch_t o = io;
-    o.B = nb;
-    auto adv = [&](const void *p, size_t per) -> void * { return p ? (void *)((const char *)p + per * (size_t)b0) : nullptr; };
-    o.x0 = adv(io.x0, es * s->nx);
-    if (io.xref_per_instance) o.Xref = adv(io.Xref, bx);
-    if (io.uref_per_instance) o.Uref = adv(io.Uref, bu);
-    void *const *sp = (void *const *)&io.state;
-    void **dp = (void **)&o.state;
-    const int nfields = sizeof(tinympc_state_t) / sizeof(void *);
-    for (int i = 0; i < nfields; ++i) dp[i] = adv(sp[i], (i % 2) == 0 ? bx : bu);
-    o.sol_x = adv(io.sol_x, bx);
-    o.sol_u = adv(io.sol_u, bu);
-    o.iter = (int32_t *)adv(io.iter, sizeof(int32_t));
-    o.solved = (int32_t *)adv(io.solved, sizeof(int32_t));
-    o.residuals = adv(io.residuals, 4 * es);
-    o.u0 = adv(io.u0, es * s->nu);
-    o.models = adv(io.models, es * (size_t)tinympc_b200_model_blob_elems(s->nx, s->nu));
-    return o;
-}
-
-// TPI streams its per-instance state through global memory every iteration.  TINYMPC_TPI_CHUNK=<n> solves
-// the batch in sub-batches of n instances (an experiment knob: an L2-sized working set did NOT pay off).
-int64_t tpi_chunk_instances(const tinympc_b200_solver *s, const Features &ft, int64_t B) {
-    if (const char *e = std::getenv("TINYMPC_TPI_CHUNK")) {
-        long long v = std::atoll(e);
-        if (v > 0) return std::min<int64_t>(B, (v + 127) / 128 * 128);
-        if (v < 0) return B;  // chunking off
-    }
-    (void)ft;
-    return B;  // sub-batching only lowers occupancy: TPI is latency-, not L2-, limited
-}
-
-// shared memory the adaptive kernel adds per CTA for its tables
-size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->nx, s->nu, esize(s->dtype)); }
-
-// checks of an adaptive-rho solve that need no device; `gpi` = the adaptive kernel's launch plan
-int check_adaptive(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar, tmpc::GpiPlan *gpi) {
-    if (io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
-    if (!ar->models || !ar->dKinf_drho || !ar->dPinf_drho || ar->reserved != 0)
-        return fail(TINYMPC_ERR_ARG, "adaptive rho: models, dKinf_drho and dPinf_drho are required and reserved must be 0");
-    if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho is available in STRICT mode only");
-    if (features(s).ext) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho covers box constraints only (no cones or hyperplanes)");
-    if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
-        return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs on the on-chip (GPI) kernel family only");
-    *gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin - (int)adapt_smem(s));
-    if (gpi->smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho: the horizon does not fit the on-chip kernel");
-    gpi->smem += adapt_smem(s);
-    return 0;
 }
 
 // the adaptive kernel's arguments (GpiAdapt<T>, then the tables) into s->d_adapt, ordered on `stream`: an asynchronous copy
@@ -416,22 +385,15 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
             const tinympc_adaptive_rho_t *ar = nullptr) {
     if (int rc = check_ready(s)) return rc;
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
-    tmpc::GpiPlan gpi;
-    if (ar)
-        if (int rc = check_adaptive(s, io, ar, &gpi)) return rc;
+    SolvePlan plan;
+    if (ar || io->B > 0)  // an adaptive solve is checked whole even when the batch is empty
+        if (int rc = plan_solve(s, io, ar, io->B, &plan)) return rc;
     if (io->B <= 0) return TINYMPC_OK;
-    const Features ft = features(s);
-    int family = ar ? TINYMPC_KERNEL_GPI : resolve_family(s, ft, &gpi, io->B);
-    if (io->models) {
-        const char *why = nullptr;
-        family = models_family(s, ft, gpi, &why);
-        if (family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, why);
-    }
-    if (family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
+    const int family = plan.family;
     // The launch scratch of a handle (work queue, workspaces, timing events) is single-buffered: a solve enqueued on a
     // different stream than the previous one first waits for it.
     if (s->have_last && s->last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, s->ev_last, 0));
-    int64_t launches = 0, ctas = 0;
+    const Features ft = features(s);
     size_t ws_bytes = 0;
     tmpc::LaunchDesc d;
     base_desc(s, d, ft);
@@ -443,46 +405,35 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     if (timed) CUDA_TRY(cudaEventRecord(s->ev0, stream));
     d.family = family;
     d.stream = stream;
-    if (family == TINYMPC_KERNEL_GPI || family == TINYMPC_KERNEL_GPS) {
+    d.io = *io;
+    d.Bpad = (io->B + 31) / 32 * 32;
+    if (family == TINYMPC_KERNEL_TPI) {
+        if (int rc = setup_workspace(s, d, ft)) return rc;
+        ws_bytes = s->ws.bytes;
+    } else {
         if (s->queue.ensure(256)) return fail(TINYMPC_ERR_CUDA, "queue allocation failed");
         CUDA_TRY(cudaMemsetAsync(s->queue.p, 0, 256, stream));
         d.work_queue = s->queue.p;
-        d.gpi_vscratch = nullptr;
+        d.gpi = plan.gpi;
         if (family == TINYMPC_KERNEL_GPI && (io->state.v || io->state.z)) {  // previous-iteration slacks are staged in pack layout, one 16-byte store per knot point
-            if (s->vscratch.ensure((size_t)io->B * gpi.vscratch_per_instance + 256)) return fail(TINYMPC_ERR_CUDA, "GPI v-scratch allocation failed");
+            if (s->vscratch.ensure((size_t)io->B * plan.gpi.vscratch_per_instance + 256)) return fail(TINYMPC_ERR_CUDA, "GPI v-scratch allocation failed");
             d.gpi_vscratch = s->vscratch.p;
         }
-        d.Bpad = (io->B + 31) / 32 * 32;
-        d.io = *io;
         if (ar) d.io.models = ar->models;
         d.gps_ws = s->gps_ws.p;
         d.gps_ws_bytes = s->gps_ws.bytes;
-        int rc = s->dim->launch(&d);
-        if (rc == tmpc::TM_ERR_WORKSPACE) {  // the streamed kernel sizes its workspace by resident slots: grow and retry
-            if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still use the old buffer
-            if (s->gps_ws.ensure(d.out_ws_need + 256)) return fail(TINYMPC_ERR_CUDA, "GPS workspace allocation failed");
-            d.gps_ws = s->gps_ws.p;
-            d.gps_ws_bytes = s->gps_ws.bytes;
-            rc = s->dim->launch(&d);
-        }
-        if (rc == TINYMPC_ERR_CUDA) return fail(rc, std::string("kernel launch failed: ") + cudaGetErrorString(cudaGetLastError()));
-        if (rc) return fail(TINYMPC_ERR_UNSUPPORTED, "no compiled kernel for this (dtype, mode, family) combination");
-        ++launches;
-        ctas += d.out_ctas;
-        if (family == TINYMPC_KERNEL_GPS) ws_bytes = d.out_ws_need;
-    } else {
-        const int64_t chunk = tpi_chunk_instances(s, ft, io->B);
-        if (int rc = setup_workspace(s, d, ft, chunk, TINYMPC_KERNEL_TPI)) return rc;
-        ws_bytes = s->ws.bytes;
-        for (int64_t b0 = 0; b0 < io->B; b0 += chunk) {
-            d.io = slice_batch(s, *io, b0, std::min<int64_t>(chunk, io->B - b0));
-            int rc = s->dim->launch(&d);
-            if (rc == TINYMPC_ERR_CUDA) return fail(rc, std::string("kernel launch failed: ") + cudaGetErrorString(cudaGetLastError()));
-            if (rc) return fail(rc, "no compiled kernel for this (dtype, mode, family) combination");
-            ++launches;
-            ctas += d.out_ctas;
-        }
     }
+    int rc = s->dim->launch(&d);
+    if (rc == tmpc::TM_ERR_WORKSPACE) {  // the streamed kernel sizes its workspace by resident slots: grow and retry
+        if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still use the old buffer
+        if (s->gps_ws.ensure(d.out_ws_need + 256)) return fail(TINYMPC_ERR_CUDA, "GPS workspace allocation failed");
+        d.gps_ws = s->gps_ws.p;
+        d.gps_ws_bytes = s->gps_ws.bytes;
+        rc = s->dim->launch(&d);
+    }
+    if (rc == TINYMPC_ERR_CUDA) return fail(rc, std::string("kernel launch failed: ") + cudaGetErrorString(cudaGetLastError()));
+    if (rc) return fail(TINYMPC_ERR_UNSUPPORTED, "no compiled kernel for this (dtype, mode, family) combination");
+    if (family == TINYMPC_KERNEL_GPS) ws_bytes = d.out_ws_need;
     s->stats.lanes_per_instance = d.out_lanes_per_instance;
     s->stats.instances_per_cta = d.out_instances_per_cta;
     s->stats.smem_bytes_per_cta = d.out_smem;
@@ -493,9 +444,9 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     s->have_last = true;
     s->timed = timed;
     s->stats.instances = io->B;
-    s->stats.kernel_launches = launches;
+    s->stats.kernel_launches = 1;
     s->stats.kernel_family = family;
-    s->stats.ctas = (int)ctas;
+    s->stats.ctas = d.out_ctas;
     s->stats.gpi_instances = family == TINYMPC_KERNEL_TPI ? 0 : io->B;
     s->stats.workspace_bytes = (int64_t)ws_bytes;
     return TINYMPC_OK;
@@ -666,20 +617,16 @@ int tinympc_b200_create(const tinympc_problem_t *p, int32_t device, tinympc_b200
     s->nx = p->nx; s->nu = p->nu; s->N = p->N; s->dtype = p->dtype; s->rho = p->rho;
     s->dim = dim;
     const size_t es = esize(p->dtype), nx = p->nx, nu = p->nu, N = p->N;
-    s->A = copy_bytes(p->Adyn, es * nx * nx); s->Bm = copy_bytes(p->Bdyn, es * nx * nu); s->f = copy_bytes(p->fdyn, es * nx);
-    s->Qd = copy_bytes(p->Q, es * nx); s->Rd = copy_bytes(p->R, es * nu);
-    s->Kinf = copy_bytes(p->Kinf, es * nu * nx); s->Pinf = copy_bytes(p->Pinf, es * nx * nx);
-    s->Quu = copy_bytes(p->Quu_inv, es * nu * nu); s->AmBKt = copy_bytes(p->AmBKt, es * nx * nx);
-    s->APf = copy_bytes(p->APf, es * nx); s->BPf = copy_bytes(p->BPf, es * nu);
     tinympc_b200_default_settings(&s->settings);
     bool ok = true;
-    {   // the cache blob (model_blob.h) the lane-group kernels stage into shared memory
+    {   // the cache blob (model_blob.h): the kernel parameters are filled from it, the lane-group kernels stage it into shared memory
         const tmpc::ModelBlob mb = tmpc::model_blob(p->nx, p->nu);
-        std::vector<char> blob(((size_t)mb.cache * es + 63) / 64 * 64, 0);
-        auto put = [&](int off, const std::vector<char> &v) { std::memcpy(blob.data() + (size_t)off * es, v.data(), v.size()); };
-        put(mb.A, s->A); put(mb.B, s->Bm); put(mb.f, s->f); put(mb.Qd, s->Qd); put(mb.Rd, s->Rd); put(mb.Kinf, s->Kinf);
-        put(mb.Pinf, s->Pinf); put(mb.Quu, s->Quu); put(mb.AmBKt, s->AmBKt); put(mb.APf, s->APf); put(mb.BPf, s->BPf);
-        ok &= !upload(s->d_blob, blob.data(), blob.size());
+        s->blob.assign(((size_t)mb.cache * es + 63) / 64 * 64, 0);
+        auto put = [&](int off, const void *v, size_t elems) { std::memcpy(s->blob.data() + (size_t)off * es, v, elems * es); };
+        put(mb.A, p->Adyn, nx * nx); put(mb.B, p->Bdyn, nx * nu); put(mb.f, p->fdyn, nx); put(mb.Qd, p->Q, nx); put(mb.Rd, p->R, nu);
+        put(mb.Kinf, p->Kinf, nu * nx); put(mb.Pinf, p->Pinf, nx * nx); put(mb.Quu, p->Quu_inv, nu * nu); put(mb.AmBKt, p->AmBKt, nx * nx);
+        put(mb.APf, p->APf, nx); put(mb.BPf, p->BPf, nu);
+        ok &= !upload(s->d_blob, s->blob.data(), s->blob.size());
     }
     auto varies = [&](const void *m, size_t rows, size_t cols) {  // does a (rows x cols) column-major matrix vary along columns?
         if (!m) return false;
@@ -873,10 +820,14 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     CUDA_TRY(cudaSetDevice(s->device));
     if (int rc = check_ready(s)) return rc;
-    tmpc::GpiPlan adapt_plan;
-    if (ar)
-        if (int rc = check_adaptive(s, io, ar, &adapt_plan)) return rc;
     const int64_t B = io->B;
+    // chunking: big enough to fill the GPU several times over, small enough to pipeline
+    int64_t chunk = B;
+    if (B > 16384) chunk = std::max<int64_t>(8192, (B + 7) / 8);
+    chunk = (chunk + 31) / 32 * 32;
+    SolvePlan plan;  // of a chunk
+    if (ar || B > 0)  // an adaptive solve is checked whole even when the batch is empty
+        if (int rc = plan_solve(s, io, ar, chunk, &plan)) return rc;
     if (B <= 0) return TINYMPC_OK;
     const size_t es = esize(s->dtype);
     const size_t bx = es * s->nx * s->N, bu = es * s->nu * (s->N - 1);
@@ -939,34 +890,10 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     if (io->residuals) fields.push_back({nullptr, io->residuals, 4 * es, false, true, (void **)&dev.residuals});
 
     for (Field &f : fields) f.pinned = is_pinned(f.is_out ? f.dst : f.src) && (!f.is_in || !f.src || is_pinned(f.src));
-    // chunking: big enough to fill the GPU several times over, small enough to pipeline
-    int64_t chunk = B;
-    if (B > 16384) chunk = std::max<int64_t>(8192, (B + 7) / 8);
-    chunk = (chunk + 31) / 32 * 32;
-    {   // the persistent GPI kernel holds sm_count * instances_per_cta instances at a time: make a chunk a whole
-        // number of such waves so that no chunk ends on a mostly empty wave (per-instance models: the same for the
-        // streamed kernel's per-instance-model variant when that is what runs)
-        const Features ft = features(s);
-        tmpc::GpiPlan gpi;
-        int fam = resolve_family(s, ft, &gpi, chunk);
-        int64_t per_cta = gpi.instances_per_cta;
-        const char *why = nullptr;
-        if (io->models && models_family(s, ft, gpi, &why) == TINYMPC_KERNEL_GPS) {
-            tmpc::LaunchDesc d;
-            base_desc(s, d, ft);
-            d.io = *io;
-            fam = TINYMPC_KERNEL_GPS;
-            per_cta = s->dim->gps_het_slots(&d);
-        }
-        if (ar) {  // the adaptive kernel's own plan (its tables take shared memory)
-            fam = TINYMPC_KERNEL_GPI;
-            per_cta = adapt_plan.instances_per_cta;
-        }
-        if ((fam == TINYMPC_KERNEL_GPI || (fam == TINYMPC_KERNEL_GPS && io->models)) && B > 16384) {
-            const int64_t wave = (int64_t)s->sm_count * per_cta;
-            if (wave > 0 && wave < B) chunk = std::max<int64_t>(1, (chunk + wave / 2) / wave) * wave;
-        }
-    }
+    // the persistent lane-group kernels hold sm_count * per_cta instances at a time: make a chunk a whole number of such waves
+    // so that no chunk ends on a mostly empty wave
+    const int64_t wave = (int64_t)s->sm_count * plan.per_cta;
+    if (B > 16384 && wave > 0 && wave < B) chunk = std::max<int64_t>(1, (chunk + wave / 2) / wave) * wave;
     if (const char *e = std::getenv("TINYMPC_HOST_CHUNK")) {  // experiment knob
         long long v = std::atoll(e);
         if (v > 0) chunk = std::min<int64_t>(B, (v + 31) / 32 * 32);

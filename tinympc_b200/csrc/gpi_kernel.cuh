@@ -19,7 +19,6 @@
 // Scope: box constraints (admm.cpp:85-98).  Cones / hyperplanes run on the streamed lane-group kernel (gps_kernel.cuh).
 #pragma once
 #include <algorithm>
-#include <cstdlib>
 
 #include "adapt.h"
 #include "common.cuh"
@@ -1168,52 +1167,27 @@ inline void gpi_consider(int N, int max_smem, GpiPlan &best) {
 template <typename T, int NX, int NU>
 inline GpiPlan gpi_plan(int N, int max_smem) {
     GpiPlan p;
+    gpi_consider<T, NX, NU, 4>(N, max_smem, p);
+    gpi_consider<T, NX, NU, 8>(N, max_smem, p);
     // L = 16 is only ever needed in fp64 (two registers per matrix entry: L = 4 / 8 exceed the register ceiling from
-    // nx = 12 on); for fp32 L = 8 covers every (nx, nu) pair of TM_DIMS, so the fp32 L = 16 kernels are compiled only
-    // with -DTM_GPI_L16 (wider states) to keep the build short
-    constexpr bool L16 = sizeof(T) == 8
-#ifdef TM_GPI_L16
-                         || true
-#endif
-        ;
-    // TINYMPC_GPI_LANES=4|8|16 restricts the choice to one group width (A/B switch for measurements)
-    const char *e = std::getenv("TINYMPC_GPI_LANES");
-    const int only = e ? std::atoi(e) : 0;
-    if (!only || only == 4) gpi_consider<T, NX, NU, 4>(N, max_smem, p);
-    if (!only || only == 8) gpi_consider<T, NX, NU, 8>(N, max_smem, p);
-    if constexpr (L16)
-        if (!only || only == 16) gpi_consider<T, NX, NU, 16>(N, max_smem, p);
+    // nx = 12 on); for fp32 L = 8 covers every (nx, nu) pair of TM_DIMS, so no fp32 L = 16 kernel is compiled
+    if constexpr (sizeof(T) == 8) gpi_consider<T, NX, NU, 16>(N, max_smem, p);
     return p;
 }
 
-template <typename T, int NX, int NU, int L, bool FAST, bool HET, bool MM = false>
-int launch_gpi_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P, const T *gmat) {
+// launch the kernel of lane parameter LA (the lane count L, plus GPI_ADAPT for adaptive rho) with the plan d->gpi (d->gpi.L == L;
+// for adaptive rho its smem includes gpi_adapt_bytes)
+template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
+int launch_gpi_L(LaunchDesc *d, const KParams<T, NX, NU> &P, const T *gmat) {
+    constexpr int L = LA % GPI_ADAPT;
     if constexpr (gpi_feasible<T, NX, NU, L>()) {
-        auto kern = gpi_solve_kernel<T, NX, NU, L, FAST, HET, MM>;
+        const GpiPlan &plan = d->gpi;
+        auto kern = gpi_solve_kernel<T, NX, NU, LA, FAST, HET, MM>;
         if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
         const int64_t ngroups = (d->io.B + (32 / L) - 1) / (32 / L);
         // ngroups = warps the batch fills.  A batch smaller than one wave is spread over all SMs with fewer warps per CTA
         // (the kernel's carve-up is per warp, any block size up to plan.warps works): the latency of a solve is set by how
         // many warps share a scheduler.
-        int warps = plan.warps;
-        if ((ngroups + warps - 1) / warps < d->sm_count) warps = (int)std::max<int64_t>(1, (ngroups + d->sm_count - 1) / d->sm_count);
-        const int64_t want = (ngroups + warps - 1) / warps;
-        const int ctas = (int)std::max<int64_t>(1, std::min<int64_t>(d->sm_count, want));
-        kern<<<ctas, warps * 32, plan.smem, d->stream>>>(P, gmat, (unsigned long long *)d->work_queue);
-        return launch_done(d, warps * 32, ctas, plan.smem, L, plan.instances_per_cta);
-    } else {
-        return TINYMPC_ERR_UNSUPPORTED;
-    }
-}
-
-// the adaptive kernel (plan.smem includes gpi_adapt_bytes); same launch geometry as launch_gpi_L
-template <typename T, int NX, int NU, int L>
-int launch_gpi_adapt_L(LaunchDesc *d, const GpiPlan &plan, const KParams<T, NX, NU> &P, const T *gmat) {
-    static_assert(L < GPI_ADAPT, "the lane count must leave GPI_ADAPT free");
-    if constexpr (gpi_feasible<T, NX, NU, L>()) {
-        auto kern = gpi_solve_kernel<T, NX, NU, L + GPI_ADAPT, false, true>;
-        if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
-        const int64_t ngroups = (d->io.B + (32 / L) - 1) / (32 / L);
         int warps = plan.warps;
         if ((ngroups + warps - 1) / warps < d->sm_count) warps = (int)std::max<int64_t>(1, (ngroups + d->sm_count - 1) / d->sm_count);
         const int64_t want = (ngroups + warps - 1) / warps;

@@ -1102,9 +1102,22 @@ struct GpsPlan {
     GpsLayout ly;
 };
 
-inline int gps_env_int(const char *name, int dflt) {
-    const char *e = std::getenv(name);
-    return e ? std::atoi(e) : dflt;
+// shared memory per CTA: the staged blob and the zero image, then one ring per warp
+template <typename T, int NX, int NU, int L, int NI, int FAM>
+inline size_t gps_smem(int warps) {
+    using RINGH = GpsRing<NX, NU, L, (int)sizeof(T), NI, FAM>;
+    return cache_reserve_bytes(NX, NU, sizeof(T)) + RINGH::ZERO_BYTES + RINGH::WARP_BYTES * (size_t)warps;
+}
+
+// most warps per CTA: shared memory, registers (gps_max_warps) and TINYMPC_GPS_WARPS; 0 = not even one warp fits
+template <typename T, int NX, int NU, int L, int NI, int FAM>
+inline int gps_warps_max(int max_smem_optin) {
+    const size_t max_smem = (size_t)(max_smem_optin - 64), fixed = gps_smem<T, NX, NU, L, NI, FAM>(0);
+    const size_t per_warp = gps_smem<T, NX, NU, L, NI, FAM>(1) - fixed;
+    if (fixed + per_warp > max_smem) return 0;
+    const int maxw = (int)std::min<size_t>(gps_max_warps(NI), (max_smem - fixed) / per_warp);
+    const char *e = std::getenv("TINYMPC_GPS_WARPS");  // a cap for tests that need many waves
+    return std::max(1, std::min(maxw, std::max(1, e ? std::atoi(e) : gps_max_warps(NI))));
 }
 
 template <typename T, int NX, int NU, int L, int NI, int FAM>
@@ -1116,13 +1129,8 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     const tinympc_state_t &s = d.io.state;
     // region B: previous box slacks (work->v / work->z) and family slacks, only when the caller wants them back
     p.ly.has_b = (s.v || s.z || s.vcnew || s.zcnew || s.vlnew || s.zlnew || s.vlnew_tv || s.zlnew_tv) ? 1 : 0;
-    const int max_smem = d.max_smem_optin - 64;
-    const size_t blob = cache_reserve_bytes(NX, NU, sizeof(T));
-    using RINGH = GpsRing<NX, NU, L, (int)sizeof(T), NI, FAM>;
-    const size_t per_warp = RINGH::WARP_BYTES, fixed = blob + RINGH::ZERO_BYTES;
-    if (fixed + per_warp > (size_t)max_smem) return p;
-    int maxw = (int)std::min<size_t>(gps_max_warps(NI), ((size_t)max_smem - fixed) / per_warp);
-    maxw = std::max(1, std::min(maxw, std::max(1, gps_env_int("TINYMPC_GPS_WARPS", gps_max_warps(NI)))));
+    const int maxw = gps_warps_max<T, NX, NU, L, NI, FAM>(d.max_smem_optin);
+    if (maxw == 0) return p;
     // balance the waves: with `waves` passes over the resident slots, use just enough warps per SM to hold B / waves
     const int64_t groups = (d.io.B + SPW - 1) / SPW;  // warps' worth of instances
     const int64_t cap = (int64_t)d.sm_count * maxw;
@@ -1132,7 +1140,7 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     p.NI = NI;
     p.warps = warps;
     p.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(d.sm_count, (groups + warps - 1) / warps));
-    p.smem = fixed + per_warp * (size_t)warps;
+    p.smem = gps_smem<T, NX, NU, L, NI, FAM>(warps);
     p.ws_bytes = (size_t)p.ctas * warps * d.N * (REC::recA + (p.ly.has_b ? REC::recB : 0)) * sizeof(T);
     return p;
 }
@@ -1154,10 +1162,7 @@ int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
 }
 
 // family mask of the kernel that serves a feature set: 0 box only, 1 cones only, 6 hyperplanes only, 7 anything else
-inline int gps_family_mask(const LaunchDesc &d) {
-    const bool soc = d.soc_x || d.soc_u, lin = d.lin_x || d.lin_u || d.tvl_x || d.tvl_u;
-    return !soc && !lin ? 0 : (soc && !lin ? 1 : (!soc ? 6 : 7));
-}
+inline int gps_family_mask(bool soc, bool lin) { return !soc && !lin ? 0 : (soc && !lin ? 1 : (!soc ? 6 : 7)); }
 
 template <typename T, int NX, int NU, bool FAST>
 int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
@@ -1165,8 +1170,8 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     if constexpr (L == 0) {
         return TINYMPC_ERR_UNSUPPORTED;
     } else {
-        constexpr int NIP = gps_pick_NI<T, NX, NU, L>();
-        const int fam = gps_family_mask(*d);
+        constexpr int NI = gps_pick_NI<T, NX, NU, L>();
+        const int fam = gps_family_mask(d->soc_x || d->soc_u, d->lin_x || d->lin_u || d->tvl_x || d->tvl_u);
         if (d->io.models) {  // per-instance models: one instance per lane group, the same family variants
 #define TM_GPS_HET_CASE(FF) \
     if (fam == FF) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_HET, FAST>(d, P0);
@@ -1177,24 +1182,8 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
 #undef TM_GPS_HET_CASE
             return TINYMPC_ERR_UNSUPPORTED;
         }
-        int ni = gps_env_int("TINYMPC_GPS_NI", NIP);
-        if (ni != 1 && ni != 2) ni = NIP;
-        if (ni > NIP) ni = NIP;
-        (void)ni;
-// only the planner's instances-per-group variant is compiled; -DTM_GPS_TUNE also builds the one-instance variant of the
-// shapes that default to two (TINYMPC_GPS_NI=1 then selects it: developer sweeps)
-#ifdef TM_GPS_TUNE
-#define TM_GPS_CASE(FF)                                                                   \
-    if (fam == FF) {                                                                      \
-        if constexpr (NIP == 2) {                                                         \
-            if (ni == 2) return launch_gps_cfg<T, NX, NU, L, 2, FF, FAST>(d, P0);         \
-        }                                                                                 \
-        return launch_gps_cfg<T, NX, NU, L, 1, FF, FAST>(d, P0);                          \
-    }
-#else
 #define TM_GPS_CASE(FF) \
-    if (fam == FF) return launch_gps_cfg<T, NX, NU, L, NIP, FF, FAST>(d, P0);
-#endif
+    if (fam == FF) return launch_gps_cfg<T, NX, NU, L, NI, FF, FAST>(d, P0);
         TM_GPS_CASE(0)
         TM_GPS_CASE(1)
         TM_GPS_CASE(6)
@@ -1207,21 +1196,17 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
 // instances one CTA of the per-instance-model variant holds when the batch fills every SM (the host path rounds its chunks to
 // whole waves of these); 0 = shape not available
 template <typename T, int NX, int NU>
-int gps_het_slots(const LaunchDesc &d0) {
+int gps_het_slots(int fam, int max_smem_optin) {
     constexpr int L = gps_pick_L<T, NX, NU>();
     if constexpr (L == 0) {
         return 0;
     } else {
-        LaunchDesc d = d0;
-        d.sm_count = 1;
-        d.io.B = (int64_t)1 << 40;
-        const int fam = gps_family_mask(d);
-        GpsPlan p;
-        if (fam == 0) p = gps_plan_L<T, NX, NU, L, 1, 0>(d);
-        else if (fam == 1) p = gps_plan_L<T, NX, NU, L, 1, 1>(d);
-        else if (fam == 6) p = gps_plan_L<T, NX, NU, L, 1, 6>(d);
-        else p = gps_plan_L<T, NX, NU, L, 1, 7>(d);
-        return p.L ? p.warps * (32 / L) : 0;
+        int warps;
+        if (fam == 0) warps = gps_warps_max<T, NX, NU, L, 1, 0>(max_smem_optin);
+        else if (fam == 1) warps = gps_warps_max<T, NX, NU, L, 1, 1>(max_smem_optin);
+        else if (fam == 6) warps = gps_warps_max<T, NX, NU, L, 1, 6>(max_smem_optin);
+        else warps = gps_warps_max<T, NX, NU, L, 1, 7>(max_smem_optin);
+        return warps * (32 / L);
     }
 }
 

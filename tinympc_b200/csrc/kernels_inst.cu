@@ -24,7 +24,7 @@ extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d);
 extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin);
 extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d);
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype);
-extern "C" int TM_SYM(tm_gps_het_slots_)(const tmpc::LaunchDesc *d);
+extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, int max_smem_optin);
 
 #if TM_PART == 0
 // =========================================================================================================
@@ -90,62 +90,41 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
 namespace tmpc {
 namespace {
 
+// the plan d->gpi comes from the caller (capi.cu: plan_solve, through the DimEntry's gpi_plan)
 template <typename T, int NX, int NU, bool FAST>
 int launch_gpi(LaunchDesc *d) {
-    const GpiPlan plan = gpi_plan<T, NX, NU>(d->N, d->max_smem_optin - 64);
-    if (plan.L == 0 || !d->gmat || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
-    KParams<T, NX, NU> P;
-    fill_params<T, NX, NU>(P, *d);
-    const T *gmat = (const T *)d->gmat;
+    const int L = d->gpi.L;
+    if (L == 0 || !d->gmat || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     const bool het = d->io.models != nullptr;  // heterogeneous batch: per-instance model blobs
-    // STRICT fp32, shared model (the headline path): min / max clamp when no bound is a signed zero
-#define TM_GPI_CASE(LL, HH)                                                                                              \
-    if (plan.L == LL && het == HH) {                                                                                     \
-        if constexpr (!FAST && !HH && sizeof(T) == 4) {                                                                  \
-            if (d->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, FAST, HH, true>(d, plan, P, gmat);               \
-        }                                                                                                                \
-        return launch_gpi_L<T, NX, NU, LL, FAST, HH>(d, plan, P, gmat);                                                  \
-    }
-#define TM_GPI_L(LL) TM_GPI_CASE(LL, false) TM_GPI_CASE(LL, true)
-    TM_GPI_L(4)
-    TM_GPI_L(8)
-#ifdef TM_GPI_L16
-    TM_GPI_L(16)
-#else
-    if constexpr (sizeof(T) == 8) {  // fp64 may need L = 16 for the widest states (see gpi_plan)
-        TM_GPI_L(16)
-    }
-#endif
-#undef TM_GPI_L
-#undef TM_GPI_CASE
-    return TINYMPC_ERR_UNSUPPORTED;
-}
-
-// adaptive rho: heterogeneous STRICT batches; the tables take gpi_adapt_bytes of shared memory per CTA
-template <typename T, int NX, int NU>
-int launch_gpi_adapt(LaunchDesc *d) {
-    const int extra = (int)gpi_adapt_bytes(NX, NU, sizeof(T));
-    GpiPlan plan = gpi_plan<T, NX, NU>(d->N, d->max_smem_optin - 64 - extra);
-    if (plan.L == 0 || d->fast || !d->gmat || !d->work_queue || !d->io.models) return TINYMPC_ERR_UNSUPPORTED;
-    plan.smem += extra;
+    if (d->adapt && (FAST || !het || !d->adapt_args)) return TINYMPC_ERR_UNSUPPORTED;  // adaptive rho: heterogeneous STRICT batches
     KParams<T, NX, NU> P;
     fill_params<T, NX, NU>(P, *d);
-    if (!d->adapt_args) return TINYMPC_ERR_UNSUPPORTED;
-    set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
+    if (d->adapt) set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
     const T *gmat = (const T *)d->gmat;
-    if (plan.L == 4) return launch_gpi_adapt_L<T, NX, NU, 4>(d, plan, P, gmat);
-    if (plan.L == 8) return launch_gpi_adapt_L<T, NX, NU, 8>(d, plan, P, gmat);
-#ifndef TM_GPI_L16
-    if constexpr (sizeof(T) == 8)
-#endif
-        if (plan.L == 16) return launch_gpi_adapt_L<T, NX, NU, 16>(d, plan, P, gmat);
+    // STRICT: adaptive rho has its own variant; fp32 with a shared model (the headline path) clamps with min / max when no bound
+    // is a signed zero
+#define TM_GPI_CASE(LL)                                                                                              \
+    if (L == LL) {                                                                                                   \
+        if constexpr (!FAST) {                                                                                       \
+            if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                   \
+            if constexpr (sizeof(T) == 4)                                                                            \
+                if (!het && d->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, false, false, true>(d, P, gmat); \
+        }                                                                                                            \
+        if (het) return launch_gpi_L<T, NX, NU, LL, FAST, true>(d, P, gmat);                                         \
+        return launch_gpi_L<T, NX, NU, LL, FAST, false>(d, P, gmat);                                                 \
+    }
+    TM_GPI_CASE(4)
+    TM_GPI_CASE(8)
+    if constexpr (sizeof(T) == 8) {  // fp64 may need L = 16 for the widest states (see gpi_plan)
+        TM_GPI_CASE(16)
+    }
+#undef TM_GPI_CASE
     return TINYMPC_ERR_UNSUPPORTED;
 }
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
     if (d->ext) return TINYMPC_ERR_UNSUPPORTED;  // the on-chip kernel covers box constraints; the rest streams (gps)
-    if (d->adapt) return launch_gpi_adapt<T, TM_NX, TM_NU>(d);
     return d->fast ? launch_gpi<T, TM_NX, TM_NU, true>(d) : launch_gpi<T, TM_NX, TM_NU, false>(d);
 }
 
@@ -157,10 +136,10 @@ extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d) {
     if (d->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
     return TINYMPC_ERR_ARG;
 }
+// the on-chip kernel's launch plan; 64 bytes of the opt-in shared memory stay back for the kernel's static shared memory (its mbarrier)
 extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin) {
-    if (dtype == TINYMPC_F32) return tmpc::gpi_plan<float, TM_NX, TM_NU>(N, max_smem_optin - 64);
-    if (dtype == TINYMPC_F64) return tmpc::gpi_plan<double, TM_NX, TM_NU>(N, max_smem_optin - 64);
-    return tmpc::GpiPlan{};
+    auto plan = [&](auto t) { return tmpc::gpi_plan<decltype(t), TM_NX, TM_NU>(N, max_smem_optin - 64); };
+    return dtype == TINYMPC_F32 ? plan(0.f) : (dtype == TINYMPC_F64 ? plan(0.0) : tmpc::GpiPlan{});
 }
 
 #else
@@ -188,18 +167,14 @@ extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d) {
 }
 // lanes per instance of the streamed lane-group kernel for this shape (0 = not available)
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype) {
-    // lanes per instance in bits 0-7, instances per lane group (1 or 2) in bits 8-15
-    auto lanes = [](auto t) {
-        using T = decltype(t);
-        constexpr int L = tmpc::gps_pick_L<T, TM_NX, TM_NU>();
-        if constexpr (L == 0) return 0;
-        else return L | (tmpc::gps_pick_NI<T, TM_NX, TM_NU, L>() << 8);
-    };
-    return dtype == TINYMPC_F32 ? lanes(0.f) : (dtype == TINYMPC_F64 ? lanes(0.0) : 0);
+    if (dtype == TINYMPC_F32) return tmpc::gps_pick_L<float, TM_NX, TM_NU>();
+    if (dtype == TINYMPC_F64) return tmpc::gps_pick_L<double, TM_NX, TM_NU>();
+    return 0;
 }
-extern "C" int TM_SYM(tm_gps_het_slots_)(const tmpc::LaunchDesc *d) {
-    if (d->dtype == TINYMPC_F32) return tmpc::gps_het_slots<float, TM_NX, TM_NU>(*d);
-    if (d->dtype == TINYMPC_F64) return tmpc::gps_het_slots<double, TM_NX, TM_NU>(*d);
+extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, int max_smem_optin) {
+    const int fam = tmpc::gps_family_mask(soc, lin);
+    if (dtype == TINYMPC_F32) return tmpc::gps_het_slots<float, TM_NX, TM_NU>(fam, max_smem_optin);
+    if (dtype == TINYMPC_F64) return tmpc::gps_het_slots<double, TM_NX, TM_NU>(fam, max_smem_optin);
     return 0;
 }
 #endif

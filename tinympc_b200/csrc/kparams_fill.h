@@ -12,17 +12,19 @@ namespace tmpc {
 template <typename T, int NX, int NU>
 inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
     std::memset(&P, 0, sizeof(P));
-    std::memcpy(P.A, d.A, sizeof(T) * NX * NX);
-    std::memcpy(P.Bm, d.Bm, sizeof(T) * NX * NU);
-    std::memcpy(P.f, d.f, sizeof(T) * NX);
-    std::memcpy(P.Qd, d.Qd, sizeof(T) * NX);
-    std::memcpy(P.Rd, d.Rd, sizeof(T) * NU);
-    std::memcpy(P.Kinf, d.Kinf, sizeof(T) * NU * NX);
-    std::memcpy(P.Pinf, d.Pinf, sizeof(T) * NX * NX);
-    std::memcpy(P.Quu, d.Quu, sizeof(T) * NU * NU);
-    std::memcpy(P.AmBKt, d.AmBKt, sizeof(T) * NX * NX);
-    std::memcpy(P.APf, d.APf, sizeof(T) * NX);
-    std::memcpy(P.BPf, d.BPf, sizeof(T) * NU);
+    const ModelBlob mb = model_blob(NX, NU);
+    const T *blob = (const T *)d.h_blob;
+    std::memcpy(P.A, blob + mb.A, sizeof(P.A));
+    std::memcpy(P.Bm, blob + mb.B, sizeof(P.Bm));
+    std::memcpy(P.f, blob + mb.f, sizeof(P.f));
+    std::memcpy(P.Qd, blob + mb.Qd, sizeof(P.Qd));
+    std::memcpy(P.Rd, blob + mb.Rd, sizeof(P.Rd));
+    std::memcpy(P.Kinf, blob + mb.Kinf, sizeof(P.Kinf));
+    std::memcpy(P.Pinf, blob + mb.Pinf, sizeof(P.Pinf));
+    std::memcpy(P.Quu, blob + mb.Quu, sizeof(P.Quu));
+    std::memcpy(P.AmBKt, blob + mb.AmBKt, sizeof(P.AmBKt));
+    std::memcpy(P.APf, blob + mb.APf, sizeof(P.APf));
+    std::memcpy(P.BPf, blob + mb.BPf, sizeof(P.BPf));
     P.rho = (T)d.rho;
     P.pri_tol = (T)d.pri_tol;
     P.dua_tol = (T)d.dua_tol;
@@ -56,7 +58,7 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
             P.uhi[j] = (d.en_input_bound && d.h_uhi) ? ((const T *)d.h_uhi)[j] : inf;
         }
     }
-    P.Pinf_g = d.gmat ? (const T *)d.gmat + model_blob(NX, NU).Pinf : nullptr;
+    P.Pinf_g = d.gmat ? (const T *)d.gmat + mb.Pinf : nullptr;
     P.xref_pi = io.xref_per_instance;
     P.uref_pi = io.uref_per_instance;
     P.x0 = (const T *)io.x0; P.Xref = (const T *)io.Xref; P.Uref = (const T *)io.Uref;

@@ -9,14 +9,21 @@
 
 namespace tmpc {
 
+// launch plan of the on-chip lane-group kernel (gpi_kernel.cuh: gpi_plan) for one (dtype, N); L == 0: not available
+struct GpiPlan {
+    int L = 0, warps = 0;              // lanes per instance, warps per CTA
+    size_t smem = 0;                   // dynamic shared memory per CTA (bytes)
+    int instances_per_cta = 0;         // instances resident per CTA (warps * 32 / L)
+    size_t vscratch_per_instance = 0;  // bytes of work->v / work->z scratch per instance (launch.h: gpi_vscratch)
+};
+
 struct LaunchDesc {
     int dtype;   // TINYMPC_F32 / F64
     int fast;    // TINYMPC_MODE_FAST ?
     int family;  // TINYMPC_KERNEL_TPI / GPI / GPS (resolved, never AUTO)
     int ext;     // any of soc / linear / tv-linear enabled
 
-    // host copies of the model + cache in the native dtype (column-major)
-    const void *A, *Bm, *f, *Qd, *Rd, *Kinf, *Pinf, *Quu, *AmBKt, *APf, *BPf;
+    const void *h_blob;  // host copy of the cache blob (model_blob.h), the bytes of gmat
     double rho, pri_tol, dua_tol;
     int N, max_iter, check_termination;
     int en_state_bound, en_input_bound;
@@ -38,6 +45,7 @@ struct LaunchDesc {
     int bounds_zero_free;  // no element of the box bounds is +-0 (lets STRICT kernels clamp with min / max instructions)
     const void *h_xlo, *h_xhi, *h_ulo, *h_uhi;  // host copies of column 0 of the bounds (native dtype), may be null
     void *work_queue;  // GPI: device int64 counter (zeroed by the caller)
+    GpiPlan gpi;       // GPI: the launch plan (for adaptive rho the adaptive kernel's, its tables' shared memory included)
     void *gpi_vscratch;  // GPI: scratch for work->v / work->z persistence (allocated by the caller when state.v/z given)
     void *gps_ws;        // GPS: streamed state records of the resident slots (allocated by the caller, see out_ws_need)
     size_t gps_ws_bytes;
@@ -76,14 +84,6 @@ constexpr int TM_ERR_WORKSPACE = -100;
 // per-(nx,nu) entry: returns 0 on success, TINYMPC_ERR_UNSUPPORTED when (dtype,family,...) is not compiled
 typedef int (*launch_fn)(LaunchDesc *);
 
-// launch plan of the on-chip lane-group kernel (gpi_kernel.cuh: gpi_plan) for one (dtype, N); L == 0: not available
-struct GpiPlan {
-    int L = 0, warps = 0;              // lanes per instance, warps per CTA
-    size_t smem = 0;                   // dynamic shared memory per CTA (bytes)
-    int instances_per_cta = 0;         // instances resident per CTA (warps * 32 / L)
-    size_t vscratch_per_instance = 0;  // bytes of work->v / work->z scratch per instance (launch.h: gpi_vscratch)
-};
-
 struct DimEntry {
     int nx, nu;
     launch_fn launch;
@@ -92,11 +92,11 @@ struct DimEntry {
     // batched cache precompute on the device (precompute_kernel.cuh): device pointers, one model blob per instance
     int (*precompute_batch)(int dtype, int64_t B, const void *A, const void *Bm, const void *f, const void *Qdiag, const void *Rdiag,
                             const void *rho, void *models_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);
-    // streamed lane-group kernel (gps_kernel.cuh): lanes per instance (bits 0-7) | instances per lane group << 8; 0 = shape not available
+    // streamed lane-group kernel (gps_kernel.cuh): lanes per instance; 0 = shape not available
     int (*gps_lanes)(int dtype);
     // its per-instance-model variant (io.models): instances per CTA when the batch fills every SM, for the shape and the
-    // constraint families of `d`; 0 = not available
-    int (*gps_het_slots)(const LaunchDesc *d);
+    // constraint families (cones, hyperplanes); 0 = not available
+    int (*gps_het_slots)(int dtype, bool soc, bool lin, int max_smem_optin);
 };
 
 }  // namespace tmpc
