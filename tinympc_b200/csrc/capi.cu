@@ -15,7 +15,7 @@
 
 #include "adapt.h"
 #include "host_precompute.h"
-#include "launch.h"
+#include "kparams_fill.h"
 #include "model_blob.h"
 
 #define TM_DECL(nx, nu) extern "C" const tmpc::DimEntry *tm_dim_entry_##nx##_##nu();
@@ -71,48 +71,33 @@ const tmpc::DimEntry *find_dim(int nx, int nu) {
 
 size_t esize(int dtype) { return dtype == TINYMPC_F64 ? 8 : 4; }
 
-struct DevBuf {
+// a growable buffer of device memory or of page-locked host memory, released with the handle
+template <bool PINNED>
+struct Buf {
     void *p = nullptr;
     size_t bytes = 0;
+    Buf() = default;
+    Buf(const Buf &) = delete;
+    Buf &operator=(const Buf &) = delete;
+    ~Buf() { release(); }
     int ensure(size_t n) {
         if (n <= bytes) return 0;
-        if (p) cudaFree(p);
-        p = nullptr;
-        bytes = 0;
-        if (cudaMalloc(&p, n) != cudaSuccess) return -1;
+        release();
+        if ((PINNED ? cudaMallocHost(&p, n) : cudaMalloc(&p, n)) != cudaSuccess) {
+            p = nullptr;
+            return -1;
+        }
         bytes = n;
         return 0;
     }
     void release() {
-        if (p) cudaFree(p);
+        if (p) PINNED ? cudaFreeHost(p) : cudaFree(p);
         p = nullptr;
         bytes = 0;
     }
 };
-struct PinBuf {
-    void *p = nullptr;
-    size_t bytes = 0;
-    int ensure(size_t n) {
-        if (n <= bytes) return 0;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        bytes = 0;
-        if (cudaMallocHost(&p, n) != cudaSuccess) return -1;
-        bytes = n;
-        return 0;
-    }
-    void release() {
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        bytes = 0;
-    }
-};
-
-std::vector<char> copy_bytes(const void *p, size_t n) {
-    std::vector<char> v(n);
-    if (n) std::memcpy(v.data(), p, n);
-    return v;
-}
+using DevBuf = Buf<false>;
+using PinBuf = Buf<true>;
 
 }  // namespace
 
@@ -121,20 +106,9 @@ struct tinympc_b200_solver {
     int sm_count = 0;
     int max_smem_optin = 0;
     int l2_bytes = 0;
-    int nx = 0, nu = 0, N = 0, dtype = 0;
-    double rho = 0;
     const tmpc::DimEntry *dim = nullptr;
-    std::vector<char> blob;  // host copy of the cache blob (model_blob.h), the bytes of d_blob
-    std::vector<char> h_xlo, h_xhi, h_ulo, h_uhi;  // column 0 of the bounds
-    bool has_xb = false, has_ub = false;
-    int ncx = 0, ncu = 0, nlx = 0, nlu = 0, ntvx = 0, ntvu = 0;
-    int cone_x_start[4] = {0, 0, 0, 0}, cone_u_start[4] = {0, 0, 0, 0};
-    double cone_x_mu[4] = {0, 0, 0, 0}, cone_u_mu[4] = {0, 0, 0, 0};
-    // device copies
-    DevBuf d_xmin, d_xmax, d_umin, d_umax, d_blob;
-    int bounds_tv = 0;
-    int bounds_zero_free = 1;
-    DevBuf d_Alin_x, d_blin_x, d_Alin_u, d_blin_u, d_tvA_x, d_tvb_x, d_tvA_u, d_tvb_u;
+    tmpc::ProblemDesc pd;
+    DevBuf problem;  // the device arrays of pd
     tinympc_settings_t settings;
     int mode = TINYMPC_MODE_STRICT;
     int family = TINYMPC_KERNEL_AUTO;
@@ -167,20 +141,11 @@ struct tinympc_b200_solver {
 
 namespace {
 
-int upload(DevBuf &b, const void *src, size_t n) {
-    if (!src || n == 0) return 0;
-    if (b.ensure(n)) return -1;
-    return cudaMemcpy(b.p, src, n, cudaMemcpyHostToDevice) == cudaSuccess ? 0 : -1;
-}
-
-struct Features {
-    int soc_x, soc_u, lin_x, lin_u, tvl_x, tvl_u, ext;
-};
-Features features(const tinympc_b200_solver *s) {
-    Features f;
+tmpc::Features features(const tinympc_b200_solver *s) {
+    tmpc::Features f;
     const tinympc_settings_t &st = s->settings;
-    f.soc_x = st.en_state_soc && s->ncx > 0;
-    f.soc_u = st.en_input_soc && s->ncu > 0;
+    f.soc_x = st.en_state_soc && s->pd.ncx > 0;
+    f.soc_u = st.en_input_soc && s->pd.ncu > 0;
     f.lin_x = st.en_state_linear != 0;
     f.lin_u = st.en_input_linear != 0;
     f.tvl_x = st.en_tv_state_linear != 0;
@@ -189,14 +154,17 @@ Features features(const tinympc_b200_solver *s) {
     return f;
 }
 
-int check_ready(const tinympc_b200_solver *s) {
+// The checks of a solve before it is planned: the handle's state, then the arguments (ar: adaptive rho, or null).  Their
+// order decides which error a caller sees.
+int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
     const tinympc_settings_t &st = s->settings;
-    if ((st.en_state_bound && !s->has_xb) || (st.en_input_bound && !s->has_ub))
+    if ((st.en_state_bound && !s->pd.x_min) || (st.en_input_bound && !s->pd.u_min))
         return fail(TINYMPC_ERR_NO_BOUNDS, "en_state_bound/en_input_bound set but bounds were never provided");
-    if ((st.en_state_linear && s->nlx > 0 && (!s->d_Alin_x.p || !s->d_blin_x.p)) || (st.en_input_linear && s->nlu > 0 && (!s->d_Alin_u.p || !s->d_blin_u.p)) ||
-        (st.en_tv_state_linear && s->ntvx > 0 && (!s->d_tvA_x.p || !s->d_tvb_x.p)) || (st.en_tv_input_linear && s->ntvu > 0 && (!s->d_tvA_u.p || !s->d_tvb_u.p)))
-        return fail(TINYMPC_ERR_ARG, "linear constraints enabled but their matrices were not uploaded");
     if (st.check_termination <= 0) return fail(TINYMPC_ERR_ARG, "check_termination must be >= 1");
+    if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
+    if (ar && io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
+    if (ar && (!ar->models || !ar->dKinf_drho || !ar->dPinf_drho || ar->reserved != 0))
+        return fail(TINYMPC_ERR_ARG, "adaptive rho: models, dKinf_drho and dPinf_drho are required and reserved must be 0");
     return 0;
 }
 
@@ -209,32 +177,29 @@ struct SolvePlan {
 };
 
 // shared memory the adaptive kernel adds per CTA for its tables
-size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->nx, s->nu, esize(s->dtype)); }
+size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->pd.nx, s->pd.nu, esize(s->pd.dtype)); }
 
-// The plan of a solve of B instances (io->models: per-instance models; ar: adaptive rho, or null).  GPI = lane groups, state
+// The plan of a solve of B instances (models: per-instance models; adapt: adaptive rho).  GPI = lane groups, state
 // on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane
 // mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature cannot be served.
-int plan_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar, int64_t B, SolvePlan *p) {
-    const Features ft = features(s);
-    if (ar) {  // adaptive rho: the on-chip kernel's adaptive variant, whose tables take shared memory
-        if (io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
-        if (!ar->models || !ar->dKinf_drho || !ar->dPinf_drho || ar->reserved != 0)
-            return fail(TINYMPC_ERR_ARG, "adaptive rho: models, dKinf_drho and dPinf_drho are required and reserved must be 0");
+int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B, SolvePlan *p) {
+    const tmpc::Features ft = features(s);
+    if (adapt) {  // adaptive rho: the on-chip kernel's adaptive variant, whose tables take shared memory
         if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho is available in STRICT mode only");
         if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho covers box constraints only (no cones or hyperplanes)");
         if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
             return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs on the on-chip (GPI) kernel family only");
         const size_t tables = adapt_smem(s);
-        p->gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin - (int)tables);
+        p->gpi = s->dim->gpi_plan(s->pd.dtype, s->pd.N, s->max_smem_optin - (int)tables);
         if (p->gpi.smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho: the horizon does not fit the on-chip kernel");
         p->gpi.smem += tables;
         p->family = TINYMPC_KERNEL_GPI;
         p->per_cta = p->gpi.instances_per_cta;
         return 0;
     }
-    if (!ft.ext) p->gpi = s->dim->gpi_plan(s->dtype, s->N, s->max_smem_optin);
+    if (!ft.ext) p->gpi = s->dim->gpi_plan(s->pd.dtype, s->pd.N, s->max_smem_optin);
     const bool gpi_ok = p->gpi.smem > 0;
-    const bool gps_ok = s->dim->gps_lanes(s->dtype) > 0;
+    const bool gps_ok = s->dim->gps_lanes(s->pd.dtype) > 0;
     if (s->family == TINYMPC_KERNEL_GPI) {
         p->family = gpi_ok ? TINYMPC_KERNEL_GPI : (gps_ok ? TINYMPC_KERNEL_GPS : -1);
     } else if (s->family == TINYMPC_KERNEL_GPS) {
@@ -256,8 +221,8 @@ int plan_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const ti
         // warps per SM ((4,2,50): 13 vs 19 ms; (16,8,50): 80 vs 197 ms) unless they hold only 6 instances ((12,4,50): 73 vs 60 ms),
         // and loses badly with one warp ((6,3,100): 143 vs 60 ms thread per instance).
         const int ipc = p->gpi.instances_per_cta;
-        const bool tpi_heavy = s->nx >= 16 && s->nu >= 8;
-        const bool few = s->dtype == TINYMPC_F64 ? (p->gpi.warps < 2 || ipc < 8) : ipc < 16;
+        const bool tpi_heavy = s->pd.nx >= 16 && s->pd.nu >= 8;
+        const bool few = s->pd.dtype == TINYMPC_F64 ? (p->gpi.warps < 2 || ipc < 8) : ipc < 16;
         p->family = (!gpi_ok || (ipc > 0 && few && !tpi_heavy && big_batch)) ? streamed : TINYMPC_KERNEL_GPI;
     }
     if (p->family == TINYMPC_KERNEL_GPI) p->per_cta = p->gpi.instances_per_cta;
@@ -265,7 +230,7 @@ int plan_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const ti
     // box constraints only and an on-chip plan (per_cta is left as the rules above set it: the host path rounds such chunks
     // by the family a shared model would get).  Otherwise the streamed kernel's per-instance-model variant: explicit GPS,
     // cones or hyperplanes, or a horizon that does not fit on chip.  One thread per instance has no such variant.
-    if (io->models) {
+    if (models) {
         if (s->family == TINYMPC_KERNEL_TPI)
             return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models run on the lane-group kernel families (GPI, GPS), not on one thread per instance");
         if (s->family != TINYMPC_KERNEL_GPS && !ft.ext && gpi_ok) {
@@ -273,80 +238,18 @@ int plan_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const ti
         } else {
             if (!gps_ok) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models: this problem needs the streamed lane-group kernel, which does not cover this shape");
             p->family = TINYMPC_KERNEL_GPS;
-            p->per_cta = s->dim->gps_het_slots(s->dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, s->max_smem_optin);
+            p->per_cta = s->dim->gps_het_slots(s->pd.dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, s->max_smem_optin);
         }
     }
     if (p->family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
     return 0;
 }
 
-// carve the TPI structure-of-arrays workspace for d.Bpad instances
-int setup_workspace(tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features &ft) {
-    const int64_t Bpad = d.Bpad;
-    const int E = s->dtype == TINYMPC_F64 ? 2 : 4;
-    const size_t nxv = (s->nx + E - 1) / E, nuv = (s->nu + E - 1) / E;
-    const size_t szx = (size_t)s->N * nxv * 16 * Bpad, szu = (size_t)(s->N - 1) * nuv * 16 * Bpad;
-    size_t total = 3 * szx + 4 * szu;
-    if (ft.soc_x) total += 2 * szx;
-    if (ft.soc_u) total += 2 * szu;
-    if (ft.lin_x) total += 2 * szx;
-    if (ft.lin_u) total += 2 * szu;
-    if (ft.tvl_x) total += 2 * szx;
-    if (ft.tvl_u) total += 2 * szu;
-    if (s->ws.ensure(total + 256)) return fail(TINYMPC_ERR_CUDA, "workspace allocation failed");
-    char *c = (char *)s->ws.p;
-    auto take = [&](size_t n) {
-        void *r = c;
-        c += n;
-        return r;
-    };
-    d.w_v[0] = take(szx); d.w_v[1] = take(szx); d.w_g = take(szx);
-    d.w_z[0] = take(szu); d.w_z[1] = take(szu); d.w_y = take(szu); d.w_d = take(szu);
-    if (ft.soc_x) { d.w_vc = take(szx); d.w_gc = take(szx); }
-    if (ft.soc_u) { d.w_zc = take(szu); d.w_yc = take(szu); }
-    if (ft.lin_x) { d.w_vl = take(szx); d.w_gl = take(szx); }
-    if (ft.lin_u) { d.w_zl = take(szu); d.w_yl = take(szu); }
-    if (ft.tvl_x) { d.w_vlt = take(szx); d.w_glt = take(szx); }
-    if (ft.tvl_u) { d.w_zlt = take(szu); d.w_ylt = take(szu); }
-    return 0;
-}
-
-void base_desc(const tinympc_b200_solver *s, tmpc::LaunchDesc &d, const Features &ft) {
-    d = tmpc::LaunchDesc{};
-    d.dtype = s->dtype;
-    d.fast = s->mode == TINYMPC_MODE_FAST;
-    d.ext = ft.ext;
-    d.h_blob = s->blob.data();
-    d.rho = s->rho;
-    const tinympc_settings_t &st = s->settings;
-    d.pri_tol = st.abs_pri_tol; d.dua_tol = st.abs_dua_tol;
-    d.N = s->N; d.max_iter = st.max_iter; d.check_termination = st.check_termination;
-    d.en_state_bound = st.en_state_bound; d.en_input_bound = st.en_input_bound;
-    d.soc_x = ft.soc_x; d.soc_u = ft.soc_u;
-    d.ncx = st.en_state_soc ? s->ncx : 0; d.ncu = st.en_input_soc ? s->ncu : 0;
-    d.lin_x = ft.lin_x; d.lin_u = ft.lin_u; d.nlx = s->nlx; d.nlu = s->nlu;
-    d.tvl_x = ft.tvl_x; d.tvl_u = ft.tvl_u; d.ntvx = s->ntvx; d.ntvu = s->ntvu;
-    for (int c = 0; c < 4; ++c) {
-        d.cone_x_start[c] = s->cone_x_start[c]; d.cone_u_start[c] = s->cone_u_start[c];
-        d.cone_x_mu[c] = s->cone_x_mu[c]; d.cone_u_mu[c] = s->cone_u_mu[c];
-    }
-    d.x_min = s->d_xmin.p; d.x_max = s->d_xmax.p; d.u_min = s->d_umin.p; d.u_max = s->d_umax.p;
-    d.Alin_x = s->d_Alin_x.p; d.blin_x = s->d_blin_x.p; d.Alin_u = s->d_Alin_u.p; d.blin_u = s->d_blin_u.p;
-    d.tv_Alin_x = s->d_tvA_x.p; d.tv_blin_x = s->d_tvb_x.p; d.tv_Alin_u = s->d_tvA_u.p; d.tv_blin_u = s->d_tvb_u.p;
-    d.gmat = s->d_blob.p;
-    d.bounds_tv = s->bounds_tv;
-    d.bounds_zero_free = s->bounds_zero_free;
-    d.h_xlo = s->h_xlo.empty() ? nullptr : s->h_xlo.data(); d.h_xhi = s->h_xhi.empty() ? nullptr : s->h_xhi.data();
-    d.h_ulo = s->h_ulo.empty() ? nullptr : s->h_ulo.data(); d.h_uhi = s->h_uhi.empty() ? nullptr : s->h_uhi.data();
-    d.sm_count = s->sm_count;
-    d.max_smem_optin = s->max_smem_optin;
-}
-
 // the adaptive kernel's arguments (GpiAdapt<T>, then the tables) into s->d_adapt, ordered on `stream`: an asynchronous copy
 // from a page-locked staging slot (the host returns without waiting for earlier work on the stream)
 template <typename T>
-int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, cudaStream_t stream) {
-    const size_t nk = (size_t)s->nu * s->nx, np = (size_t)s->nx * s->nx;
+int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, const void *models, cudaStream_t stream) {
+    const size_t nk = (size_t)s->pd.nu * s->pd.nx, np = (size_t)s->pd.nx * s->pd.nx;
     const size_t bytes = tmpc::GPI_ADAPT_HDR + (nk + np) * sizeof(T);
     if (s->d_adapt.bytes < bytes) {
         if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still read the old buffer
@@ -363,14 +266,14 @@ int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, cu
     std::memcpy(tab, ar->dKinf_drho, nk * sizeof(T));
     std::memcpy(tab + nk, ar->dPinf_drho, np * sizeof(T));
     tmpc::GpiAdapt<T> a{};
-    a.models = (T *)ar->models;
+    a.models = (T *)models;
     a.dK = (const T *)((char *)s->d_adapt.p + tmpc::GPI_ADAPT_HDR);
     a.dP = a.dK + nk;
     a.rho_min = (T)ar->rho_min;
     a.rho_max = (T)ar->rho_max;
     a.clip = ar->enable_clipping != 0;
-    const long cols = (long)s->nx * s->N + (long)s->nu * (s->N - 1);
-    a.maskA = tmpc::gemv_block_mask((long)(s->nx + s->nu) * (s->N - 1), cols, sizeof(T));
+    const long cols = (long)s->pd.nx * s->pd.N + (long)s->pd.nu * (s->pd.N - 1);
+    a.maskA = tmpc::gemv_block_mask((long)(s->pd.nx + s->pd.nu) * (s->pd.N - 1), cols, sizeof(T));
     a.maskP = tmpc::gemv_block_mask(cols, cols, sizeof(T));
     static_assert(sizeof(a) <= tmpc::GPI_ADAPT_HDR, "GpiAdapt must fit its header");
     std::memcpy(h, &a, sizeof(a));
@@ -380,25 +283,30 @@ int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, cu
     return 0;
 }
 
-// enqueue one batched solve on `stream` (device pointers); fills stats.  ar: adaptive rho (device model blobs), or null
+// enqueue one batched solve on `stream` (device pointers, checked by check_solve); fills stats.  io->models: the model blobs
+// the kernel reads, the per-instance models or, with ar (adaptive rho, else null), the blobs it adapts in place
 int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stream, bool timed,
             const tinympc_adaptive_rho_t *ar = nullptr) {
-    if (int rc = check_ready(s)) return rc;
-    if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     SolvePlan plan;
     if (ar || io->B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io, ar, io->B, &plan)) return rc;
+        if (int rc = plan_solve(s, io->models != nullptr, ar != nullptr, io->B, &plan)) return rc;
     if (io->B <= 0) return TINYMPC_OK;
     const int family = plan.family;
     // The launch scratch of a handle (work queue, workspaces, timing events) is single-buffered: a solve enqueued on a
     // different stream than the previous one first waits for it.
     if (s->have_last && s->last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, s->ev_last, 0));
-    const Features ft = features(s);
     size_t ws_bytes = 0;
-    tmpc::LaunchDesc d;
-    base_desc(s, d, ft);
+    tmpc::LaunchDesc d{};
+    d.pd = &s->pd;
+    d.st = s->settings;
+    d.ft = features(s);
+    d.fast = s->mode == TINYMPC_MODE_FAST;
+    d.sm_count = s->sm_count;
+    d.max_smem_optin = s->max_smem_optin;
     if (ar) {
-        if (int rc = s->dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, stream) : upload_adaptive<float>(s, ar, stream)) return rc;
+        if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, io->models, stream)
+                                                : upload_adaptive<float>(s, ar, io->models, stream))
+            return rc;
         d.adapt = 1;
         d.adapt_args = s->d_adapt.p;
     }
@@ -408,7 +316,9 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     d.io = *io;
     d.Bpad = (io->B + 31) / 32 * 32;
     if (family == TINYMPC_KERNEL_TPI) {
-        if (int rc = setup_workspace(s, d, ft)) return rc;
+        const tmpc::ProblemDesc &pd = s->pd;
+        if (s->ws.ensure(tmpc::tpi_workspace(pd.nx, pd.nu, pd.N, pd.dtype, d.Bpad, d.ft) + 256)) return fail(TINYMPC_ERR_CUDA, "workspace allocation failed");
+        d.tpi_ws = s->ws.p;
         ws_bytes = s->ws.bytes;
     } else {
         if (s->queue.ensure(256)) return fail(TINYMPC_ERR_CUDA, "queue allocation failed");
@@ -419,7 +329,6 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
             if (s->vscratch.ensure((size_t)io->B * plan.gpi.vscratch_per_instance + 256)) return fail(TINYMPC_ERR_CUDA, "GPI v-scratch allocation failed");
             d.gpi_vscratch = s->vscratch.p;
         }
-        if (ar) d.io.models = ar->models;
         d.gps_ws = s->gps_ws.p;
         d.gps_ws_bytes = s->gps_ws.bytes;
     }
@@ -569,7 +478,7 @@ int tinympc_b200_precompute_cache_batch_device(tinympc_b200_solver_t *s, int64_t
     if (!A || !Bm || !f || !Qdiag || !Rdiag || !rho || !models_out || B < 0) return fail(TINYMPC_ERR_ARG, "null pointer or bad size");
     if (B == 0) return TINYMPC_OK;
     CUDA_TRY(cudaSetDevice(s->device));
-    const int rc = s->dim->precompute_batch(s->dtype, B, A, Bm, f, Qdiag, Rdiag, rho, models_out, sweeps_out, s->sm_count,
+    const int rc = s->dim->precompute_batch(s->pd.dtype, B, A, Bm, f, Qdiag, Rdiag, rho, models_out, sweeps_out, s->sm_count,
                                             (cudaStream_t)stream);
     if (rc == TINYMPC_ERR_CUDA) return fail(rc, std::string("precompute kernel launch failed: ") + cudaGetErrorString(cudaGetLastError()));
     if (rc) return fail(rc, "precompute kernel unavailable for this dtype");
@@ -614,19 +523,18 @@ int tinympc_b200_create(const tinympc_problem_t *p, int32_t device, tinympc_b200
     s->sm_count = prop.multiProcessorCount;
     s->max_smem_optin = (int)prop.sharedMemPerBlockOptin;
     s->l2_bytes = prop.l2CacheSize;
-    s->nx = p->nx; s->nu = p->nu; s->N = p->N; s->dtype = p->dtype; s->rho = p->rho;
     s->dim = dim;
     const size_t es = esize(p->dtype), nx = p->nx, nu = p->nu, N = p->N;
     tinympc_b200_default_settings(&s->settings);
-    bool ok = true;
+    tmpc::ProblemDesc &pd = s->pd;
+    pd.nx = p->nx; pd.nu = p->nu; pd.N = p->N; pd.dtype = p->dtype; pd.rho = p->rho;
     {   // the cache blob (model_blob.h): the kernel parameters are filled from it, the lane-group kernels stage it into shared memory
         const tmpc::ModelBlob mb = tmpc::model_blob(p->nx, p->nu);
-        s->blob.assign(((size_t)mb.cache * es + 63) / 64 * 64, 0);
-        auto put = [&](int off, const void *v, size_t elems) { std::memcpy(s->blob.data() + (size_t)off * es, v, elems * es); };
+        pd.h_blob.assign(((size_t)mb.cache * es + 63) / 64 * 64, 0);
+        auto put = [&](int off, const void *v, size_t elems) { std::memcpy(pd.h_blob.data() + (size_t)off * es, v, elems * es); };
         put(mb.A, p->Adyn, nx * nx); put(mb.B, p->Bdyn, nx * nu); put(mb.f, p->fdyn, nx); put(mb.Qd, p->Q, nx); put(mb.Rd, p->R, nu);
         put(mb.Kinf, p->Kinf, nu * nx); put(mb.Pinf, p->Pinf, nx * nx); put(mb.Quu, p->Quu_inv, nu * nu); put(mb.AmBKt, p->AmBKt, nx * nx);
         put(mb.APf, p->APf, nx); put(mb.BPf, p->BPf, nu);
-        ok &= !upload(s->d_blob, s->blob.data(), s->blob.size());
     }
     auto varies = [&](const void *m, size_t rows, size_t cols) {  // does a (rows x cols) column-major matrix vary along columns?
         if (!m) return false;
@@ -641,29 +549,42 @@ int tinympc_b200_create(const tinympc_problem_t *p, int32_t device, tinympc_b200
             if ((es == 8 ? ((const double *)m)[i] : (double)((const float *)m)[i]) == 0.0) return true;
         return false;
     };
-    s->bounds_zero_free = !(has_zero(p->x_min, (size_t)nx * N) || has_zero(p->x_max, (size_t)nx * N) ||
+    pd.bounds_zero_free = !(has_zero(p->x_min, (size_t)nx * N) || has_zero(p->x_max, (size_t)nx * N) ||
                             has_zero(p->u_min, (size_t)nu * (N - 1)) || has_zero(p->u_max, (size_t)nu * (N - 1)));
-    s->bounds_tv = varies(p->x_min, nx, N) || varies(p->x_max, nx, N) || varies(p->u_min, nu, N - 1) || varies(p->u_max, nu, N - 1);
-    if (p->x_min && p->x_max) {
-        ok &= !upload(s->d_xmin, p->x_min, es * nx * N) && !upload(s->d_xmax, p->x_max, es * nx * N);
-        s->has_xb = true;
-        s->h_xlo = copy_bytes(p->x_min, es * nx); s->h_xhi = copy_bytes(p->x_max, es * nx);
-    }
-    if (p->u_min && p->u_max) {
-        ok &= !upload(s->d_umin, p->u_min, es * nu * (N - 1)) && !upload(s->d_umax, p->u_max, es * nu * (N - 1));
-        s->has_ub = true;
-        s->h_ulo = copy_bytes(p->u_min, es * nu); s->h_uhi = copy_bytes(p->u_max, es * nu);
-    }
+    pd.bounds_tv = varies(p->x_min, nx, N) || varies(p->x_max, nx, N) || varies(p->u_min, nu, N - 1) || varies(p->u_max, nu, N - 1);
+    const bool xb = p->x_min && p->x_max, ub = p->u_min && p->u_max;
+    auto col0 = [&](std::vector<char> &h, const void *m, size_t rows) { h.assign((const char *)m, (const char *)m + rows * es); };
+    if (xb) { col0(pd.h_xlo, p->x_min, nx); col0(pd.h_xhi, p->x_max, nx); }
+    if (ub) { col0(pd.h_ulo, p->u_min, nu); col0(pd.h_uhi, p->u_max, nu); }
     auto rd = [&](const void *base, int i) { return p->dtype == TINYMPC_F64 ? ((const double *)base)[i] : (double)((const float *)base)[i]; };
-    s->ncx = p->num_state_cones; s->ncu = p->num_input_cones;
-    for (int c = 0; c < s->ncx; ++c) { s->cone_x_start[c] = p->Acx[c]; s->cone_x_mu[c] = rd(p->cx, c); }
-    for (int c = 0; c < s->ncu; ++c) { s->cone_u_start[c] = p->Acu[c]; s->cone_u_mu[c] = rd(p->cu, c); }
-    s->nlx = p->num_state_linear; s->nlu = p->num_input_linear;
-    if (s->nlx > 0) ok &= !upload(s->d_Alin_x, p->Alin_x, es * s->nlx * nx) && !upload(s->d_blin_x, p->blin_x, es * s->nlx);
-    if (s->nlu > 0) ok &= !upload(s->d_Alin_u, p->Alin_u, es * s->nlu * nu) && !upload(s->d_blin_u, p->blin_u, es * s->nlu);
-    s->ntvx = p->num_tv_state_linear; s->ntvu = p->num_tv_input_linear;
-    if (s->ntvx > 0) ok &= !upload(s->d_tvA_x, p->tv_Alin_x, es * s->ntvx * N * nx) && !upload(s->d_tvb_x, p->tv_blin_x, es * s->ntvx * N);
-    if (s->ntvu > 0) ok &= !upload(s->d_tvA_u, p->tv_Alin_u, es * s->ntvu * (N - 1) * nu) && !upload(s->d_tvb_u, p->tv_blin_u, es * s->ntvu * (N - 1));
+    pd.ncx = p->num_state_cones; pd.ncu = p->num_input_cones;
+    for (int c = 0; c < pd.ncx; ++c) { pd.cone_x_start[c] = p->Acx[c]; pd.cone_x_mu[c] = rd(p->cx, c); }
+    for (int c = 0; c < pd.ncu; ++c) { pd.cone_u_start[c] = p->Acu[c]; pd.cone_u_mu[c] = rd(p->cu, c); }
+    pd.nlx = p->num_state_linear; pd.nlu = p->num_input_linear;
+    pd.ntvx = p->num_tv_state_linear; pd.ntvu = p->num_tv_input_linear;
+    // the device arrays, in one allocation: the cache blob at offset 0 (cudaMalloc's alignment for its bulk copy), then each
+    // array 256-byte aligned; an array that is not given stays null
+    const struct { const void *src; size_t bytes; const void **dev; } arrays[] = {
+        {pd.h_blob.data(), pd.h_blob.size(), &pd.blob},
+        {xb ? p->x_min : nullptr, es * nx * N, &pd.x_min}, {xb ? p->x_max : nullptr, es * nx * N, &pd.x_max},
+        {ub ? p->u_min : nullptr, es * nu * (N - 1), &pd.u_min}, {ub ? p->u_max : nullptr, es * nu * (N - 1), &pd.u_max},
+        {p->Alin_x, es * pd.nlx * nx, &pd.Alin_x}, {p->blin_x, es * pd.nlx, &pd.blin_x},
+        {p->Alin_u, es * pd.nlu * nu, &pd.Alin_u}, {p->blin_u, es * pd.nlu, &pd.blin_u},
+        {p->tv_Alin_x, es * pd.ntvx * N * nx, &pd.tv_Alin_x}, {p->tv_blin_x, es * pd.ntvx * N, &pd.tv_blin_x},
+        {p->tv_Alin_u, es * pd.ntvu * (N - 1) * nu, &pd.tv_Alin_u}, {p->tv_blin_u, es * pd.ntvu * (N - 1), &pd.tv_blin_u},
+    };
+    auto aligned = [](size_t n) { return (n + 255) / 256 * 256; };
+    size_t bytes = 0;
+    for (const auto &a : arrays)
+        if (a.src && a.bytes) bytes += aligned(a.bytes);
+    bool ok = !s->problem.ensure(bytes);
+    size_t off = 0;
+    for (const auto &a : arrays) {
+        if (!ok || !a.src || !a.bytes) continue;
+        *a.dev = (char *)s->problem.p + off;
+        ok &= cudaMemcpy((char *)s->problem.p + off, a.src, a.bytes, cudaMemcpyHostToDevice) == cudaSuccess;
+        off += aligned(a.bytes);
+    }
     ok &= cudaEventCreate(&s->ev0) == cudaSuccess && cudaEventCreate(&s->ev1) == cudaSuccess &&
           cudaEventCreateWithFlags(&s->ev_last, cudaEventDisableTiming) == cudaSuccess;
     if (!ok) {
@@ -678,18 +599,9 @@ int tinympc_b200_create(const tinympc_problem_t *p, int32_t device, tinympc_b200
 int tinympc_b200_destroy(tinympc_b200_solver_t *s) {
     if (!s) return TINYMPC_OK;
     cudaSetDevice(s->device);
-    DevBuf *bufs[] = {&s->d_xmin, &s->d_xmax, &s->d_umin, &s->d_umax, &s->d_Alin_x, &s->d_blin_x, &s->d_Alin_u,
-                      &s->d_blin_u, &s->d_tvA_x, &s->d_tvb_x, &s->d_tvA_u, &s->d_tvb_u, &s->ws, &s->queue, &s->d_blob, &s->vscratch,
-                      &s->gps_ws, &s->shared_ref, &s->d_adapt};
-    for (DevBuf *b : bufs) b->release();
-    for (int i = 0; i < 3; ++i) {
-        s->adapt_pin[i].release();
+    for (int i = 0; i < 3; ++i)
         if (s->ev_adapt[i]) cudaEventDestroy(s->ev_adapt[i]);
-    }
     for (int i = 0; i < tinympc_b200_solver::SLOTS; ++i) {
-        s->dio[i].release();
-        s->pin_in[i].release();
-        s->pin_out[i].release();
         if (s->ev_in[i]) cudaEventDestroy(s->ev_in[i]);
         if (s->ev_k[i]) cudaEventDestroy(s->ev_k[i]);
         if (s->ev_out[i]) cudaEventDestroy(s->ev_out[i]);
@@ -700,7 +612,7 @@ int tinympc_b200_destroy(tinympc_b200_solver_t *s) {
     if (s->ev_last) cudaEventDestroy(s->ev_last);
     if (s->ev0) cudaEventDestroy(s->ev0);
     if (s->ev1) cudaEventDestroy(s->ev1);
-    delete s;
+    delete s;  // the buffers free their memory
     return TINYMPC_OK;
 }
 
@@ -730,6 +642,7 @@ int tinympc_b200_set_mode(tinympc_b200_solver_t *s, int32_t mode, int32_t family
 int tinympc_b200_solve(tinympc_b200_solver_t *s, const tinympc_batch_t *io, void *cuda_stream) {
     if (!s || !io) return fail(TINYMPC_ERR_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(s->device));
+    if (int rc = check_solve(s, io, nullptr)) return rc;
     return enqueue(s, io, (cudaStream_t)cuda_stream, true);
 }
 
@@ -737,7 +650,10 @@ int tinympc_b200_solve_adaptive(tinympc_b200_solver_t *s, const tinympc_batch_t 
                                 void *cuda_stream) {
     if (!s || !io || !ar) return fail(TINYMPC_ERR_ARG, "null argument");
     CUDA_TRY(cudaSetDevice(s->device));
-    return enqueue(s, io, (cudaStream_t)cuda_stream, true, ar);
+    if (int rc = check_solve(s, io, ar)) return rc;
+    tinympc_batch_t adapted = *io;
+    adapted.models = ar->models;  // the blobs the kernel adapts in place
+    return enqueue(s, &adapted, (cudaStream_t)cuda_stream, true, ar);
 }
 
 namespace {
@@ -747,14 +663,14 @@ int advance_impl(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, i
     if (B <= 0) return TINYMPC_OK;
     CUDA_TRY(cudaSetDevice(s->device));
     // threads per block = a multiple of nx so that all rows of an instance read x0 before any row writes it
-    const int per = std::max(1, 256 / s->nx) * s->nx;
-    const int64_t total = B * s->nx;
+    const int per = std::max(1, 256 / s->pd.nx) * s->pd.nx;
+    const int64_t total = B * s->pd.nx;
     const unsigned blocks = (unsigned)((total + per - 1) / per);
     cudaStream_t st = (cudaStream_t)cuda_stream;
-    if (s->dtype == TINYMPC_F32)
-        advance_kernel<float><<<blocks, per, 0, st>>>(s->nx, s->nu, u_stride, B, (const float *)blob, bstride, (float *)x0, (const float *)u);
+    if (s->pd.dtype == TINYMPC_F32)
+        advance_kernel<float><<<blocks, per, 0, st>>>(s->pd.nx, s->pd.nu, u_stride, B, (const float *)blob, bstride, (float *)x0, (const float *)u);
     else
-        advance_kernel<double><<<blocks, per, 0, st>>>(s->nx, s->nu, u_stride, B, (const double *)blob, bstride, (double *)x0, (const double *)u);
+        advance_kernel<double><<<blocks, per, 0, st>>>(s->pd.nx, s->pd.nu, u_stride, B, (const double *)blob, bstride, (double *)x0, (const double *)u);
     CUDA_TRY(cudaGetLastError());
     return TINYMPC_OK;
 }
@@ -762,13 +678,13 @@ int advance_impl(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, i
 
 int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, void *cuda_stream) {
     if (!s || !x0 || !u) return fail(TINYMPC_ERR_ARG, "null argument");
-    return advance_impl(s, B, x0, u, u_stride, s->d_blob.p, 0, cuda_stream);
+    return advance_impl(s, B, x0, u, u_stride, s->pd.blob, 0, cuda_stream);
 }
 
 int tinympc_b200_advance_models(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *models,
                                 void *cuda_stream) {
     if (!s || !x0 || !u || !models) return fail(TINYMPC_ERR_ARG, "null argument");
-    return advance_impl(s, B, x0, u, u_stride, models, tinympc_b200_model_blob_elems(s->nx, s->nu), cuda_stream);
+    return advance_impl(s, B, x0, u, u_stride, models, tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), cuda_stream);
 }
 
 int tinympc_b200_get_stats(const tinympc_b200_solver_t *s, tinympc_b200_stats_t *out) {
@@ -819,7 +735,7 @@ namespace {
 int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     CUDA_TRY(cudaSetDevice(s->device));
-    if (int rc = check_ready(s)) return rc;
+    if (int rc = check_solve(s, io, ar)) return rc;
     const int64_t B = io->B;
     // chunking: big enough to fill the GPU several times over, small enough to pipeline
     int64_t chunk = B;
@@ -827,10 +743,10 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     chunk = (chunk + 31) / 32 * 32;
     SolvePlan plan;  // of a chunk
     if (ar || B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io, ar, chunk, &plan)) return rc;
+        if (int rc = plan_solve(s, io->models != nullptr, ar != nullptr, chunk, &plan)) return rc;
     if (B <= 0) return TINYMPC_OK;
-    const size_t es = esize(s->dtype);
-    const size_t bx = es * s->nx * s->N, bu = es * s->nu * (s->N - 1);
+    const size_t es = esize(s->pd.dtype);
+    const size_t bx = es * s->pd.nx * s->pd.N, bu = es * s->pd.nu * (s->pd.N - 1);
     constexpr int SLOTS = tinympc_b200_solver::SLOTS;
     if (!s->st_h2d) {
         CUDA_TRY(cudaStreamCreateWithFlags(&s->st_h2d, cudaStreamNonBlocking));
@@ -848,13 +764,12 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     tinympc_batch_t dev = *io;  // template for the device-side descriptor
     const bool cold = io->cold_start != 0;
     std::vector<Field> fields;
-    fields.push_back({io->x0, nullptr, es * s->nx, true, false, (void **)&dev.x0});
+    fields.push_back({io->x0, nullptr, es * s->pd.nx, true, false, (void **)&dev.x0});
     if (io->xref_per_instance) fields.push_back({io->Xref, nullptr, bx, true, false, (void **)&dev.Xref});
     if (io->Uref && io->uref_per_instance) fields.push_back({io->Uref, nullptr, bu, true, false, (void **)&dev.Uref});
-    if (io->models) fields.push_back({io->models, nullptr, es * (size_t)tinympc_b200_model_blob_elems(s->nx, s->nu), true, false, (void **)&dev.models});
-    // adaptive rho: the model blobs are in/out; they travel in dev.models (io->models is NULL) and are handed to the kernel as
-    // the adaptive argument's blobs
-    if (ar) fields.push_back({ar->models, ar->models, es * (size_t)tinympc_b200_model_blob_elems(s->nx, s->nu), true, true, (void **)&dev.models});
+    if (io->models) fields.push_back({io->models, nullptr, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, false, (void **)&dev.models});
+    // adaptive rho: the model blobs are in/out; they travel in dev.models (io->models is NULL), where the kernel adapts them
+    if (ar) fields.push_back({ar->models, ar->models, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, true, (void **)&dev.models});
     {
         size_t need = (io->xref_per_instance ? 0 : bx) + ((io->Uref && !io->uref_per_instance) ? bu : 0);
         if (need) {
@@ -884,7 +799,7 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     }
     if (io->sol_x) fields.push_back({nullptr, io->sol_x, bx, false, true, (void **)&dev.sol_x});
     if (io->sol_u) fields.push_back({nullptr, io->sol_u, bu, false, true, (void **)&dev.sol_u});
-    if (io->u0) fields.push_back({nullptr, io->u0, es * s->nu, false, true, (void **)&dev.u0});
+    if (io->u0) fields.push_back({nullptr, io->u0, es * s->pd.nu, false, true, (void **)&dev.u0});
     if (io->iter) fields.push_back({nullptr, io->iter, sizeof(int32_t), false, true, (void **)&dev.iter});
     if (io->solved) fields.push_back({nullptr, io->solved, sizeof(int32_t), false, true, (void **)&dev.solved});
     if (io->residuals) fields.push_back({nullptr, io->residuals, 4 * es, false, true, (void **)&dev.residuals});
@@ -962,14 +877,7 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
         }
         CUDA_TRY(cudaEventRecord(s->ev_in[slot], s->st_h2d));
         CUDA_TRY(cudaStreamWaitEvent(s->st_k, s->ev_in[slot], 0));
-        if (ar) {
-            tinympc_adaptive_rho_t a = *ar;
-            a.models = (void *)d.models;
-            d.models = nullptr;
-            if (int rc = enqueue(s, &d, s->st_k, false, &a)) return rc;
-        } else if (int rc = enqueue(s, &d, s->st_k, false)) {
-            return rc;
-        }
+        if (int rc = enqueue(s, &d, s->st_k, false, ar)) return rc;
         launches += s->stats.kernel_launches;
         CUDA_TRY(cudaEventRecord(s->ev_k[slot], s->st_k));
         CUDA_TRY(cudaStreamWaitEvent(s->st_d2h, s->ev_k[slot], 0));

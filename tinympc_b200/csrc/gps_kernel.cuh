@@ -1141,7 +1141,7 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     p.warps = warps;
     p.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(d.sm_count, (groups + warps - 1) / warps));
     p.smem = gps_smem<T, NX, NU, L, NI, FAM>(warps);
-    p.ws_bytes = (size_t)p.ctas * warps * d.N * (REC::recA + (p.ly.has_b ? REC::recB : 0)) * sizeof(T);
+    p.ws_bytes = (size_t)p.ctas * warps * d.pd->N * (REC::recA + (p.ly.has_b ? REC::recB : 0)) * sizeof(T);
     return p;
 }
 
@@ -1149,7 +1149,7 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH & ~GPS_HET>(*d);
-    if (plan.L == 0 || !d->gmat || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
+    if (plan.L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     d->out_ws_need = plan.ws_bytes;
     if (!d->gps_ws || d->gps_ws_bytes < plan.ws_bytes) return TM_ERR_WORKSPACE;
     KParams<T, NX, NU> P = P0;
@@ -1157,7 +1157,7 @@ int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     P.gps_ws = (T *)d->gps_ws;
     auto kern = gps_solve_kernel<T, NX, NU, L, NI, FAMH, FAST>;
     if (!set_dynamic_smem(kern, plan.smem)) return TINYMPC_ERR_CUDA;
-    kern<<<plan.ctas, plan.warps * 32, plan.smem, d->stream>>>(P, (const T *)d->gmat, (unsigned long long *)d->work_queue);
+    kern<<<plan.ctas, plan.warps * 32, plan.smem, d->stream>>>(P, (const T *)d->pd->blob, (unsigned long long *)d->work_queue);
     return launch_done(d, plan.warps * 32, plan.ctas, plan.smem, L, plan.warps * (32 / L) * NI);
 }
 
@@ -1171,7 +1171,7 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
         return TINYMPC_ERR_UNSUPPORTED;
     } else {
         constexpr int NI = gps_pick_NI<T, NX, NU, L>();
-        const int fam = gps_family_mask(d->soc_x || d->soc_u, d->lin_x || d->lin_u || d->tvl_x || d->tvl_u);
+        const int fam = gps_family_mask(d->ft.soc_x || d->ft.soc_u, d->ft.lin_x || d->ft.lin_u || d->ft.tvl_x || d->ft.tvl_u);
         if (d->io.models) {  // per-instance models: one instance per lane group, the same family variants
 #define TM_GPS_HET_CASE(FF) \
     if (fam == FF) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_HET, FAST>(d, P0);

@@ -48,15 +48,15 @@ int launch_tpi(LaunchDesc *d) {
 template <typename T>
 int launch_T(LaunchDesc *d) {
     if (d->io.models) return TINYMPC_ERR_UNSUPPORTED;  // per-instance models: the lane-group kernels only
-    if (d->ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
+    if (d->ft.ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
     return d->fast ? launch_tpi<T, true, false>(d) : launch_tpi<T, false, false>(d);
 }
 
 int launch(LaunchDesc *d) {
     if (d->family == TINYMPC_KERNEL_GPI) return TM_SYM(tm_gpi_launch_)(d);
     if (d->family == TINYMPC_KERNEL_GPS) return TM_SYM(tm_gps_launch_)(d);
-    if (d->dtype == TINYMPC_F32) return launch_T<float>(d);
-    if (d->dtype == TINYMPC_F64) return launch_T<double>(d);
+    if (d->pd->dtype == TINYMPC_F32) return launch_T<float>(d);
+    if (d->pd->dtype == TINYMPC_F64) return launch_T<double>(d);
     return TINYMPC_ERR_ARG;
 }
 
@@ -94,24 +94,24 @@ namespace {
 template <typename T, int NX, int NU, bool FAST>
 int launch_gpi(LaunchDesc *d) {
     const int L = d->gpi.L;
-    if (L == 0 || !d->gmat || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
+    if (L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     const bool het = d->io.models != nullptr;  // heterogeneous batch: per-instance model blobs
     if (d->adapt && (FAST || !het || !d->adapt_args)) return TINYMPC_ERR_UNSUPPORTED;  // adaptive rho: heterogeneous STRICT batches
     KParams<T, NX, NU> P;
     fill_params<T, NX, NU>(P, *d);
     if (d->adapt) set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
-    const T *gmat = (const T *)d->gmat;
+    const T *gmat = (const T *)d->pd->blob;
     // STRICT: adaptive rho has its own variant; fp32 with a shared model (the headline path) clamps with min / max when no bound
     // is a signed zero
-#define TM_GPI_CASE(LL)                                                                                              \
-    if (L == LL) {                                                                                                   \
-        if constexpr (!FAST) {                                                                                       \
-            if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                   \
-            if constexpr (sizeof(T) == 4)                                                                            \
-                if (!het && d->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, false, false, true>(d, P, gmat); \
-        }                                                                                                            \
-        if (het) return launch_gpi_L<T, NX, NU, LL, FAST, true>(d, P, gmat);                                         \
-        return launch_gpi_L<T, NX, NU, LL, FAST, false>(d, P, gmat);                                                 \
+#define TM_GPI_CASE(LL)                                                                                                  \
+    if (L == LL) {                                                                                                       \
+        if constexpr (!FAST) {                                                                                           \
+            if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                       \
+            if constexpr (sizeof(T) == 4)                                                                                \
+                if (!het && d->pd->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, false, false, true>(d, P, gmat); \
+        }                                                                                                                \
+        if (het) return launch_gpi_L<T, NX, NU, LL, FAST, true>(d, P, gmat);                                             \
+        return launch_gpi_L<T, NX, NU, LL, FAST, false>(d, P, gmat);                                                     \
     }
     TM_GPI_CASE(4)
     TM_GPI_CASE(8)
@@ -124,7 +124,7 @@ int launch_gpi(LaunchDesc *d) {
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->ext) return TINYMPC_ERR_UNSUPPORTED;  // the on-chip kernel covers box constraints; the rest streams (gps)
+    if (d->ft.ext) return TINYMPC_ERR_UNSUPPORTED;  // the on-chip kernel covers box constraints; the rest streams (gps)
     return d->fast ? launch_gpi<T, TM_NX, TM_NU, true>(d) : launch_gpi<T, TM_NX, TM_NU, false>(d);
 }
 
@@ -132,8 +132,8 @@ int launch_T(LaunchDesc *d) {
 }  // namespace tmpc
 
 extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d) {
-    if (d->dtype == TINYMPC_F32) return tmpc::launch_T<float>(d);
-    if (d->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
+    if (d->pd->dtype == TINYMPC_F32) return tmpc::launch_T<float>(d);
+    if (d->pd->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
     return TINYMPC_ERR_ARG;
 }
 // the on-chip kernel's launch plan; 64 bytes of the opt-in shared memory stay back for the kernel's static shared memory (its mbarrier)
@@ -161,8 +161,8 @@ int launch_T(LaunchDesc *d) {
 }  // namespace tmpc
 
 extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d) {
-    if (d->dtype == TINYMPC_F32) return tmpc::launch_T<float>(d);
-    if (d->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
+    if (d->pd->dtype == TINYMPC_F32) return tmpc::launch_T<float>(d);
+    if (d->pd->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
     return TINYMPC_ERR_ARG;
 }
 // lanes per instance of the streamed lane-group kernel for this shape (0 = not available)

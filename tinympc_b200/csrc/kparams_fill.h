@@ -1,5 +1,7 @@
-// kparams_fill.h — LaunchDesc (type-erased, host) -> KParams<T,NX,NU> (the kernels' parameter block).
+// kparams_fill.h — LaunchDesc (type-erased, host) -> KParams<T,NX,NU> (the kernels' parameter block), and the layout of the
+// thread-per-instance workspace.
 #pragma once
+#include <cstddef>
 #include <cstring>
 #include <limits>
 
@@ -9,11 +11,37 @@
 
 namespace tmpc {
 
+// The thread-per-instance workspace (tpi_kernel.cuh) for Bpad instances: structure-of-arrays slabs of 16-byte vectors,
+// [k][vec][Bpad], back to back.  Slab i backs the i-th of KParams' w_* pointers: v[0] v[1] z[0] z[1] g y d, then vc zc gc yc,
+// vl zl gl yl and vlt zlt glt ylt, each pair of a constraint family present only when the family is enabled.  Returns the
+// bytes; with `w` given, also points w[i] at slab i in `base` (null for an absent slab).
+constexpr int TPI_SLABS = 19;
+inline size_t tpi_workspace(int nx, int nu, int N, int dtype, int64_t Bpad, const Features &ft, char *base = nullptr,
+                            void **w = nullptr) {
+    const int E = dtype == TINYMPC_F64 ? 2 : 4;
+    const size_t szx = (size_t)N * ((nx + E - 1) / E) * 16 * Bpad, szu = (size_t)(N - 1) * ((nu + E - 1) / E) * 16 * Bpad;
+    const bool state[TPI_SLABS] = {1, 1, 0, 0, 1, 0, 0, 1, 0, 1, 0, 1, 0, 1, 0, 1, 0, 1, 0};
+    const bool on[TPI_SLABS] = {1, 1, 1, 1, 1, 1, 1,
+                                (bool)ft.soc_x, (bool)ft.soc_u, (bool)ft.soc_x, (bool)ft.soc_u,
+                                (bool)ft.lin_x, (bool)ft.lin_u, (bool)ft.lin_x, (bool)ft.lin_u,
+                                (bool)ft.tvl_x, (bool)ft.tvl_u, (bool)ft.tvl_x, (bool)ft.tvl_u};
+    size_t bytes = 0;
+    for (int i = 0; i < TPI_SLABS; ++i) {
+        if (w) w[i] = on[i] ? base + bytes : nullptr;
+        if (on[i]) bytes += state[i] ? szx : szu;
+    }
+    return bytes;
+}
+
 template <typename T, int NX, int NU>
 inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
+    using KP = KParams<T, NX, NU>;
     std::memset(&P, 0, sizeof(P));
+    const ProblemDesc &pd = *d.pd;
+    const tinympc_settings_t &st = d.st;
+    const Features &ft = d.ft;
     const ModelBlob mb = model_blob(NX, NU);
-    const T *blob = (const T *)d.h_blob;
+    const T *blob = (const T *)pd.h_blob.data();
     std::memcpy(P.A, blob + mb.A, sizeof(P.A));
     std::memcpy(P.Bm, blob + mb.B, sizeof(P.Bm));
     std::memcpy(P.f, blob + mb.f, sizeof(P.f));
@@ -25,47 +53,48 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
     std::memcpy(P.AmBKt, blob + mb.AmBKt, sizeof(P.AmBKt));
     std::memcpy(P.APf, blob + mb.APf, sizeof(P.APf));
     std::memcpy(P.BPf, blob + mb.BPf, sizeof(P.BPf));
-    P.rho = (T)d.rho;
-    P.pri_tol = (T)d.pri_tol;
-    P.dua_tol = (T)d.dua_tol;
-    P.N = d.N;
-    P.max_iter = d.max_iter;
-    P.check_termination = d.check_termination;
-    P.en_state_bound = d.en_state_bound;
-    P.en_input_bound = d.en_input_bound;
-    P.soc_x = d.soc_x; P.soc_u = d.soc_u; P.ncx = d.ncx; P.ncu = d.ncu;
-    P.lin_x = d.lin_x; P.lin_u = d.lin_u; P.nlx = d.nlx; P.nlu = d.nlu;
-    P.tvl_x = d.tvl_x; P.tvl_u = d.tvl_u; P.ntvx = d.ntvx; P.ntvu = d.ntvu;
+    P.rho = (T)pd.rho;
+    P.pri_tol = (T)st.abs_pri_tol;
+    P.dua_tol = (T)st.abs_dua_tol;
+    P.N = pd.N;
+    P.max_iter = st.max_iter;
+    P.check_termination = st.check_termination;
+    P.en_state_bound = st.en_state_bound;
+    P.en_input_bound = st.en_input_bound;
+    P.soc_x = ft.soc_x; P.soc_u = ft.soc_u; P.ncx = st.en_state_soc ? pd.ncx : 0; P.ncu = st.en_input_soc ? pd.ncu : 0;
+    P.lin_x = ft.lin_x; P.lin_u = ft.lin_u; P.nlx = pd.nlx; P.nlu = pd.nlu;
+    P.tvl_x = ft.tvl_x; P.tvl_u = ft.tvl_u; P.ntvx = pd.ntvx; P.ntvu = pd.ntvu;
     for (int c = 0; c < MAX_CONES; ++c) {
-        P.cone_x_start[c] = d.cone_x_start[c];
-        P.cone_u_start[c] = d.cone_u_start[c];
-        P.cone_x_mu[c] = (T)d.cone_x_mu[c];
-        P.cone_u_mu[c] = (T)d.cone_u_mu[c];
+        P.cone_x_start[c] = pd.cone_x_start[c];
+        P.cone_u_start[c] = pd.cone_u_start[c];
+        P.cone_x_mu[c] = (T)pd.cone_x_mu[c];
+        P.cone_u_mu[c] = (T)pd.cone_u_mu[c];
     }
     const tinympc_batch_t &io = d.io;
     P.B = io.B;
     P.Bpad = d.Bpad;
     P.cold = io.cold_start;
-    P.bounds_tv = d.bounds_tv;
+    P.bounds_tv = pd.bounds_tv;
     {
         const T inf = std::numeric_limits<T>::infinity();
+        auto col0 = [&](const std::vector<char> &h, int i, bool en, T dflt) { return en && !h.empty() ? ((const T *)h.data())[i] : dflt; };
         for (int i = 0; i < NX; ++i) {
-            P.xlo[i] = (d.en_state_bound && d.h_xlo) ? ((const T *)d.h_xlo)[i] : -inf;
-            P.xhi[i] = (d.en_state_bound && d.h_xhi) ? ((const T *)d.h_xhi)[i] : inf;
+            P.xlo[i] = col0(pd.h_xlo, i, st.en_state_bound, -inf);
+            P.xhi[i] = col0(pd.h_xhi, i, st.en_state_bound, inf);
         }
         for (int j = 0; j < NU; ++j) {
-            P.ulo[j] = (d.en_input_bound && d.h_ulo) ? ((const T *)d.h_ulo)[j] : -inf;
-            P.uhi[j] = (d.en_input_bound && d.h_uhi) ? ((const T *)d.h_uhi)[j] : inf;
+            P.ulo[j] = col0(pd.h_ulo, j, st.en_input_bound, -inf);
+            P.uhi[j] = col0(pd.h_uhi, j, st.en_input_bound, inf);
         }
     }
-    P.Pinf_g = d.gmat ? (const T *)d.gmat + mb.Pinf : nullptr;
+    P.Pinf_g = (const T *)pd.blob + mb.Pinf;
     P.xref_pi = io.xref_per_instance;
     P.uref_pi = io.uref_per_instance;
     P.x0 = (const T *)io.x0; P.Xref = (const T *)io.Xref; P.Uref = (const T *)io.Uref;
-    P.x_min = (const T *)d.x_min; P.x_max = (const T *)d.x_max; P.u_min = (const T *)d.u_min; P.u_max = (const T *)d.u_max;
-    P.Alin_x = (const T *)d.Alin_x; P.blin_x = (const T *)d.blin_x; P.Alin_u = (const T *)d.Alin_u; P.blin_u = (const T *)d.blin_u;
-    P.tv_Alin_x = (const T *)d.tv_Alin_x; P.tv_blin_x = (const T *)d.tv_blin_x;
-    P.tv_Alin_u = (const T *)d.tv_Alin_u; P.tv_blin_u = (const T *)d.tv_blin_u;
+    P.x_min = (const T *)pd.x_min; P.x_max = (const T *)pd.x_max; P.u_min = (const T *)pd.u_min; P.u_max = (const T *)pd.u_max;
+    P.Alin_x = (const T *)pd.Alin_x; P.blin_x = (const T *)pd.blin_x; P.Alin_u = (const T *)pd.Alin_u; P.blin_u = (const T *)pd.blin_u;
+    P.tv_Alin_x = (const T *)pd.tv_Alin_x; P.tv_blin_x = (const T *)pd.tv_blin_x;
+    P.tv_Alin_u = (const T *)pd.tv_Alin_u; P.tv_blin_u = (const T *)pd.tv_blin_u;
     const tinympc_state_t &s = io.state;
     P.s_x = (T *)s.x; P.s_u = (T *)s.u; P.s_v = (T *)s.v; P.s_z = (T *)s.z;
     P.s_vnew = (T *)s.vnew; P.s_znew = (T *)s.znew; P.s_g = (T *)s.g; P.s_y = (T *)s.y;
@@ -77,11 +106,12 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
     P.u0 = (T *)io.u0;
     P.models = (const T *)io.models;
     P.gpi_vscratch = (T *)d.gpi_vscratch;
-    P.w_v[0] = d.w_v[0]; P.w_v[1] = d.w_v[1]; P.w_z[0] = d.w_z[0]; P.w_z[1] = d.w_z[1];
-    P.w_g = d.w_g; P.w_y = d.w_y; P.w_d = d.w_d;
-    P.w_vc = d.w_vc; P.w_zc = d.w_zc; P.w_gc = d.w_gc; P.w_yc = d.w_yc;
-    P.w_vl = d.w_vl; P.w_zl = d.w_zl; P.w_gl = d.w_gl; P.w_yl = d.w_yl;
-    P.w_vlt = d.w_vlt; P.w_zlt = d.w_zlt; P.w_glt = d.w_glt; P.w_ylt = d.w_ylt;
+    if (d.tpi_ws) {
+        static_assert(offsetof(KP, w_ylt) == offsetof(KP, w_v) + (TPI_SLABS - 1) * sizeof(void *), "w_* are the slab pointers in order");
+        void *w[TPI_SLABS];
+        tpi_workspace(NX, NU, pd.N, pd.dtype, d.Bpad, ft, (char *)d.tpi_ws, w);
+        std::memcpy((char *)&P + offsetof(KP, w_v), w, sizeof(w));
+    }
 }
 
 }  // namespace tmpc

@@ -1,9 +1,11 @@
-// launch.h — type-erased launch descriptor between the C-ABI layer (capi.cu) and the per-(nx,nu)
+// launch.h — type-erased problem and launch descriptors between the C-ABI layer (capi.cu) and the per-(nx,nu)
 // kernel translation units (kernels_inst.cu compiled once per supported dimension pair).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
 #include <stdint.h>
+
+#include <vector>
 
 #include "../../include/tinympc_b200.h"
 
@@ -17,33 +19,39 @@ struct GpiPlan {
     size_t vscratch_per_instance = 0;  // bytes of work->v / work->z scratch per instance (launch.h: gpi_vscratch)
 };
 
+// The problem a handle solves, described once by tinympc_b200_create.  Arrays are in the native dtype.
+struct ProblemDesc {
+    int nx = 0, nu = 0, N = 0, dtype = 0;  // dtype: TINYMPC_F32 / F64
+    double rho = 0;
+    std::vector<char> h_blob;                      // host copy of the cache blob (model_blob.h), the bytes at `blob`
+    std::vector<char> h_xlo, h_xhi, h_ulo, h_uhi;  // column 0 of the bounds; empty when the bounds were not given
+    int bounds_tv = 0;         // the bounds vary along the horizon
+    int bounds_zero_free = 1;  // no element of the box bounds is +-0 (lets STRICT kernels clamp with min / max instructions)
+    int ncx = 0, ncu = 0, nlx = 0, nlu = 0, ntvx = 0, ntvu = 0;  // cones, hyperplanes, time-varying hyperplanes per side
+    int cone_x_start[4] = {}, cone_u_start[4] = {};
+    double cone_x_mu[4] = {}, cone_u_mu[4] = {};  // already rounded to the native dtype
+    // device arrays: pieces of one allocation, the cache blob at offset 0 and every piece 256-byte aligned; null when not given
+    const void *blob = nullptr;
+    const void *x_min = nullptr, *x_max = nullptr, *u_min = nullptr, *u_max = nullptr;
+    const void *Alin_x = nullptr, *blin_x = nullptr, *Alin_u = nullptr, *blin_u = nullptr;
+    const void *tv_Alin_x = nullptr, *tv_blin_x = nullptr, *tv_Alin_u = nullptr, *tv_blin_u = nullptr;
+};
+
+// the constraint families a solve runs with (the problem's cones and hyperplanes under the current settings)
+struct Features {
+    int soc_x, soc_u, lin_x, lin_u, tvl_x, tvl_u, ext;  // ext: any of them
+};
+
 struct LaunchDesc {
-    int dtype;   // TINYMPC_F32 / F64
+    const ProblemDesc *pd;
+    tinympc_settings_t st;
+    Features ft;
     int fast;    // TINYMPC_MODE_FAST ?
     int family;  // TINYMPC_KERNEL_TPI / GPI / GPS (resolved, never AUTO)
-    int ext;     // any of soc / linear / tv-linear enabled
 
-    const void *h_blob;  // host copy of the cache blob (model_blob.h), the bytes of gmat
-    double rho, pri_tol, dua_tol;
-    int N, max_iter, check_termination;
-    int en_state_bound, en_input_bound;
-    int soc_x, soc_u, ncx, ncu;
-    int lin_x, lin_u, nlx, nlu;
-    int tvl_x, tvl_u, ntvx, ntvu;
-    int cone_x_start[4], cone_u_start[4];
-    double cone_x_mu[4], cone_u_mu[4];  // already rounded to the native dtype
-
-    // device pointers
-    const void *x_min, *x_max, *u_min, *u_max;
-    const void *Alin_x, *blin_x, *Alin_u, *blin_u, *tv_Alin_x, *tv_blin_x, *tv_Alin_u, *tv_blin_u;
     tinympc_batch_t io;  // device pointers
     int64_t Bpad;
-    void *w_v[2], *w_z[2], *w_g, *w_y, *w_d;
-    void *w_vc, *w_zc, *w_gc, *w_yc, *w_vl, *w_zl, *w_gl, *w_yl, *w_vlt, *w_zlt, *w_glt, *w_ylt;
-    const void *gmat;  // device blob: A,B,f,Qd,Rd,Kinf,Pinf,Quu,AmBKt,APf,BPf packed (native dtype)
-    int bounds_tv;
-    int bounds_zero_free;  // no element of the box bounds is +-0 (lets STRICT kernels clamp with min / max instructions)
-    const void *h_xlo, *h_xhi, *h_ulo, *h_uhi;  // host copies of column 0 of the bounds (native dtype), may be null
+    void *tpi_ws;      // TPI: the workspace (kparams_fill.h: tpi_workspace)
     void *work_queue;  // GPI: device int64 counter (zeroed by the caller)
     GpiPlan gpi;       // GPI: the launch plan (for adaptive rho the adaptive kernel's, its tables' shared memory included)
     void *gpi_vscratch;  // GPI: scratch for work->v / work->z persistence (allocated by the caller when state.v/z given)
