@@ -243,6 +243,38 @@ int tinympc_b200_precompute_cache_batch_device(tinympc_b200_solver_t *h, int64_t
                                                const void *Qdiag, const void *Rdiag, const void *rho, void *models_out,
                                                int32_t *sweeps_out, void *stream);
 
+/*
+ * Sensitivity tables for adaptive rho (tinympc_adaptive_rho_t below), for B different models at once, on the host with
+ * `nthreads` threads.  The reference ships one hard-coded pair for one quadrotor (tiny_api.cpp:479-540, applied by
+ * update_matrices_with_derivatives, rho_benchmark.cpp:215-229); here the tables of model b are DEFINED as the forward-mode
+ * derivative, with respect to rho[b], of tinympc_b200_precompute_cache_batch as it runs: the Riccati recursion of
+ * tiny_precompute_and_set_cache (tiny_api.cpp:307-381) with its tangent carried alongside,
+ *     Q1 = Qdiag + 2 rho, R1 = Rdiag + 2 rho (the "double rho"):  dQ1 = dR1 = 2 I;    P <- rho I:  dP = I
+ *     per sweep, S = R1 + B'PB, K = S^-1 B'PA:
+ *         dS = dR1 + B'dP B;   dK = S^-1 (B'dP A - dS K);   dP+ = (dQ1 + A'dP (A - BK)) - A'P (B dK)
+ * for exactly the sweeps the primal recursion of that model takes (the primal's stop test ends both), so the tables are
+ * the derivative of the Kinf / Pinf the cache call returns, sweep count held fixed.  Ascending-k sums, separate multiply
+ * and add, like the cache.  Inputs as in tinympc_b200_precompute_cache_batch (f is accepted for symmetry and not read: it
+ * does not enter Kinf / Pinf).  dK_out [B][nu*nx], dP_out [B][nx*nx], column-major per instance, in `dtype`.
+ * In fp32 a model whose recursion never meets the stop test (typically few inputs for many states) runs all 1000 sweeps, and
+ * its tangent can overflow to Inf / NaN on the way; compute such tables in fp64 and round them.
+ * Returns 0, or TINYMPC_ERR_SINGULAR under the same condition, and with the same message, as the cache call.
+ */
+int tinympc_b200_precompute_sensitivity_batch(int32_t dtype, int32_t nx, int32_t nu, int64_t B, const void *A, const void *Bm,
+                                              const void *f, const void *Qdiag, const void *Rdiag, const void *rho, void *dK_out,
+                                              void *dP_out, int32_t nthreads);
+
+/*
+ * The same tables ON THE DEVICE of handle `h` (one warp per instance, precompute_kernel.cuh): device pointers of the
+ * handle's dtype, nx, nu are the handle's, asynchronous on `stream`.  Bit-identical to the host routine's.  sweeps_out
+ * (optional, [B]): sweeps used per instance, -1 where a matrix was singular (the same instances as in
+ * tinympc_b200_precompute_cache_batch_device; their tables are not written).  dK_out / dP_out can be passed straight to
+ * tinympc_b200_solve_adaptive with tables_per_instance = 1.
+ */
+int tinympc_b200_precompute_sensitivity_batch_device(tinympc_b200_solver_t *h, int64_t B, const void *A, const void *Bm, const void *f,
+                                                     const void *Qdiag, const void *Rdiag, const void *rho, void *dK_out, void *dP_out,
+                                                     int32_t *sweeps_out, void *stream);
+
 /* tiny_setup (tiny_api.hpp:10-12) minus the precompute: uploads the problem to `device`. */
 int tinympc_b200_create(const tinympc_problem_t *problem, int32_t device, tinympc_b200_solver_t **out);
 int tinympc_b200_destroy(tinympc_b200_solver_t *s);
@@ -281,7 +313,12 @@ int tinympc_b200_get_stats(const tinympc_b200_solver_t *s, tinympc_b200_stats_t 
  * The reference declares its RhoAdapter uninitialised (admm.cpp:340) and then reads it (rho_benchmark.cpp:56), which
  * makes its adaptive solve undefined behaviour; this library implements the value-initialised adapter.
  *
- *   dKinf_drho (nu x nx), dPinf_drho (nx x nx): HOST pointers of the handle's dtype, column-major, read during the call.
+ *   dKinf_drho (nu x nx), dPinf_drho (nx x nx): HOST pointers of the handle's dtype, column-major, read during the call
+ *           (tables_per_instance = 0: one pair adapts every instance, right when all instances share one model).
+ *           tables_per_instance = 1: dKinf_drho is [B][nu*nx] and dPinf_drho [B][nx*nx], instance b adapts with its own
+ *           pair (a fleet of different models; build them with tinympc_b200_precompute_sensitivity_batch[_device]).  They
+ *           are then DEVICE pointers for tinympc_b200_solve_adaptive (read by the kernel, like `models`) and host pointers
+ *           for tinympc_b200_solve_adaptive_host (chunked and staged with the models).
  *   models: [B][tinympc_b200_model_blob_elems(nx,nu)] (layout: tinympc_batch_t.models), IN/OUT: every instance starts from
  *           its blob's model, cache and rho, and its adapted rho / Kinf / Pinf are written back, so passing the same
  *           buffer to the next solve continues the adaptation (the reference's one-TinySolver-per-robot semantics).
@@ -294,6 +331,8 @@ typedef struct tinympc_adaptive_rho {
     const void *dKinf_drho;   /* nu x nx */
     const void *dPinf_drho;   /* nx x nx */
     void *models;             /* [B][blob] in/out */
+    int32_t tables_per_instance; /* 0: one table pair for the batch; 1: one pair per instance */
+    int32_t reserved1;
 } tinympc_adaptive_rho_t;
 
 /* tinympc_b200_solve with adaptive rho: io and ar->models are DEVICE pointers; asynchronous on `cuda_stream` */

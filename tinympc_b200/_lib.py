@@ -41,6 +41,8 @@ def load():
     lib.tinympc_b200_model_blob_elems.argtypes = [C.c_int32, C.c_int32]
     lib.tinympc_b200_precompute_cache_batch.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [vp] * 7 + [C.c_int32]
     lib.tinympc_b200_precompute_cache_batch_device.argtypes = [vp, C.c_int64] + [vp] * 9
+    lib.tinympc_b200_precompute_sensitivity_batch.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [vp] * 8 + [C.c_int32]
+    lib.tinympc_b200_precompute_sensitivity_batch_device.argtypes = [vp, C.c_int64] + [vp] * 10
     lib.tinympc_b200_create.argtypes = [C.POINTER(abi.Problem), C.c_int32, C.POINTER(vp)]
     lib.tinympc_b200_destroy.argtypes = [vp]
     lib.tinympc_b200_update_settings.argtypes = [vp, C.POINTER(abi.Settings)]

@@ -86,12 +86,13 @@ class Stats(C.Structure):
 
 
 class AdaptiveRho(C.Structure):
-    """tinympc_adaptive_rho_t: adaptive-rho settings, sensitivity tables (host pointers) and the in/out model blobs."""
+    """tinympc_adaptive_rho_t: adaptive-rho settings, sensitivity tables (host pointers; per instance: see the header) and the in/out model blobs."""
     _fields_ = [
         ("rho_min", C.c_double), ("rho_max", C.c_double),
         ("enable_clipping", C.c_int32), ("reserved", C.c_int32),
         ("dKinf_drho", vp), ("dPinf_drho", vp),
         ("models", vp),
+        ("tables_per_instance", C.c_int32), ("reserved1", C.c_int32),
     ]
 
 
@@ -102,6 +103,8 @@ EXPORTS = [
     "tinympc_b200_model_blob_elems",
     "tinympc_b200_precompute_cache_batch",
     "tinympc_b200_precompute_cache_batch_device",
+    "tinympc_b200_precompute_sensitivity_batch",
+    "tinympc_b200_precompute_sensitivity_batch_device",
     "tinympc_b200_create",
     "tinympc_b200_destroy",
     "tinympc_b200_update_settings",

@@ -31,7 +31,8 @@ class DeviceMPCLoop:
         """models ([B, blob], tinympc_batch_t.models, e.g. from setup_models): a heterogeneous fleet, one model, cache and rho
         per plant.  Every step solves with them and advances plant b with its own A, B, f (tinympc_b200_advance_models).
         adaptive_rho: every plant adapts its own rho / Kinf / Pinf, kept on the device across steps in self.models
-        (starting from `models` or the problem's own cache), as one TinySolver per robot would."""
+        (starting from `models` or the problem's own cache), as one TinySolver per robot would; with `models`, give it
+        per-instance tables (solver.setup_sensitivity_device), which stay on the GPU with the models."""
         import torch
 
         self.solver = solver
@@ -47,6 +48,11 @@ class DeviceMPCLoop:
         self._first = True
         self.want_solution = True  # also return solution->x / solution->u (= vnew / znew) every step
         self.adaptive_rho = adaptive_rho
+        if adaptive_rho is not None and adaptive_rho.per_instance:
+            # per-instance tables live on the GPU across steps, in the column-major storage the solve reads (no copy per step)
+            cm = lambda a: torch.as_tensor(a, device=self.dev).to(self._tdt).transpose(1, 2).contiguous().transpose(1, 2)  # noqa: E731
+            self.adaptive_rho = AdaptiveRho(cm(adaptive_rho.dKinf_drho), cm(adaptive_rho.dPinf_drho), adaptive_rho.rho_min,
+                                            adaptive_rho.rho_max, adaptive_rho.enable_clipping)
         self.models = None
         if adaptive_rho is not None or models is not None:
             m = pack_models(p, self.B) if models is None else models

@@ -118,7 +118,7 @@ struct tinympc_b200_solver {
     DevBuf vscratch;
     DevBuf gps_ws;
     DevBuf shared_ref;  // host path: references shared by the whole batch
-    DevBuf d_adapt;     // adaptive rho: GpiAdapt arguments + dKinf_drho + dPinf_drho (adapt.h)
+    DevBuf d_adapt;     // adaptive rho: GpiAdapt arguments + the shared dKinf_drho + dPinf_drho (adapt.h)
     // page-locked staging of d_adapt's contents, a ring so that the copy stays asynchronous: slot i is rewritten only once
     // the copy three solves back (ev_adapt[i]) has read it
     PinBuf adapt_pin[3];
@@ -165,6 +165,8 @@ int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const t
     if (ar && io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
     if (ar && (!ar->models || !ar->dKinf_drho || !ar->dPinf_drho || ar->reserved != 0))
         return fail(TINYMPC_ERR_ARG, "adaptive rho: models, dKinf_drho and dPinf_drho are required and reserved must be 0");
+    if (ar && ar->tables_per_instance != 0 && ar->tables_per_instance != 1)
+        return fail(TINYMPC_ERR_ARG, "adaptive rho: tables_per_instance must be 0 (one table pair for the batch) or 1 (one pair per instance)");
     return 0;
 }
 
@@ -245,12 +247,14 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B,
     return 0;
 }
 
-// the adaptive kernel's arguments (GpiAdapt<T>, then the tables) into s->d_adapt, ordered on `stream`: an asynchronous copy
-// from a page-locked staging slot (the host returns without waiting for earlier work on the stream)
+// the adaptive kernel's arguments (GpiAdapt<T>, then the shared tables) into s->d_adapt, ordered on `stream`: an asynchronous
+// copy from a page-locked staging slot (the host returns without waiting for earlier work on the stream).  Per-instance
+// tables are device arrays already: the arguments point at them and nothing follows the header.
 template <typename T>
 int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, const void *models, cudaStream_t stream) {
     const size_t nk = (size_t)s->pd.nu * s->pd.nx, np = (size_t)s->pd.nx * s->pd.nx;
-    const size_t bytes = tmpc::GPI_ADAPT_HDR + (nk + np) * sizeof(T);
+    const bool per = ar->tables_per_instance != 0;
+    const size_t bytes = tmpc::GPI_ADAPT_HDR + (per ? 0 : (nk + np) * sizeof(T));
     if (s->d_adapt.bytes < bytes) {
         if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still read the old buffer
         if (s->d_adapt.ensure(bytes)) return fail(TINYMPC_ERR_CUDA, "adaptive-rho argument allocation failed");
@@ -262,13 +266,18 @@ int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, co
     if (s->adapt_pin[slot].ensure(bytes)) return fail(TINYMPC_ERR_CUDA, "adaptive-rho staging allocation failed");
     char *h = (char *)s->adapt_pin[slot].p;
     std::memset(h, 0, bytes);
-    T *tab = (T *)(h + tmpc::GPI_ADAPT_HDR);
-    std::memcpy(tab, ar->dKinf_drho, nk * sizeof(T));
-    std::memcpy(tab + nk, ar->dPinf_drho, np * sizeof(T));
     tmpc::GpiAdapt<T> a{};
     a.models = (T *)models;
-    a.dK = (const T *)((char *)s->d_adapt.p + tmpc::GPI_ADAPT_HDR);
-    a.dP = a.dK + nk;
+    if (per) {  // [B][nu*nx], [B][nx*nx] device arrays, read by the GPI_ADAPT_TABLES kernel variant
+        a.dK = (const T *)ar->dKinf_drho;
+        a.dP = (const T *)ar->dPinf_drho;
+    } else {
+        T *tab = (T *)(h + tmpc::GPI_ADAPT_HDR);
+        std::memcpy(tab, ar->dKinf_drho, nk * sizeof(T));
+        std::memcpy(tab + nk, ar->dPinf_drho, np * sizeof(T));
+        a.dK = (const T *)((char *)s->d_adapt.p + tmpc::GPI_ADAPT_HDR);
+        a.dP = a.dK + nk;
+    }
     a.rho_min = (T)ar->rho_min;
     a.rho_max = (T)ar->rho_max;
     a.clip = ar->enable_clipping != 0;
@@ -307,7 +316,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
         if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, io->models, stream)
                                                 : upload_adaptive<float>(s, ar, io->models, stream))
             return rc;
-        d.adapt = 1;
+        d.adapt = ar->tables_per_instance ? 2 : 1;
         d.adapt_args = s->d_adapt.p;
     }
     if (timed) CUDA_TRY(cudaEventRecord(s->ev0, stream));
@@ -405,6 +414,29 @@ int precompute_batch_T(int nx, int nu, int64_t B, const T *A, const T *Bm, const
     if (bad_index) *bad_index = -1;
     return 0;
 }
+
+template <typename T>
+int sensitivity_batch_T(int nx, int nu, int64_t B, const T *A, const T *Bm, const T *Qd, const T *Rd, const T *rho, T *dK, T *dP,
+                        int nthreads) {
+    nthreads = (int)std::max<int64_t>(1, std::min<int64_t>(nthreads, B));
+    std::vector<int64_t> bad(nthreads, 0);
+    auto work = [&](int t) {
+        for (int64_t b = t; b < B; b += nthreads) {
+            const int rc = tmpc::precompute_sensitivity<T>(nx, nu, rho[b], A + b * nx * nx, Bm + b * nx * nu, Qd + b * nx, Rd + b * nu,
+                                                           dK + b * nu * nx, dP + b * nx * nx);
+            if (rc < 0 && bad[t] == 0) bad[t] = b + 1;
+        }
+    };
+    std::vector<std::thread> th;
+    for (int t = 1; t < nthreads; ++t) th.emplace_back(work, t);
+    work(0);
+    for (auto &x : th) x.join();
+    int64_t first = 0;
+    for (int64_t v : bad)
+        if (v && (!first || v < first)) first = v;
+    if (first) return fail(TINYMPC_ERR_SINGULAR, "singular R + B'PB in the Riccati recursion of instance " + std::to_string(first - 1));
+    return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -482,6 +514,36 @@ int tinympc_b200_precompute_cache_batch_device(tinympc_b200_solver_t *s, int64_t
                                             (cudaStream_t)stream);
     if (rc == TINYMPC_ERR_CUDA) return fail(rc, std::string("precompute kernel launch failed: ") + cudaGetErrorString(cudaGetLastError()));
     if (rc) return fail(rc, "precompute kernel unavailable for this dtype");
+    return TINYMPC_OK;
+}
+
+int tinympc_b200_precompute_sensitivity_batch(int32_t dtype, int32_t nx, int32_t nu, int64_t B, const void *A, const void *Bm,
+                                              const void *f, const void *Qdiag, const void *Rdiag, const void *rho, void *dK_out,
+                                              void *dP_out, int32_t nthreads) {
+    (void)f;  // the affine term does not enter Kinf / Pinf
+    if (!A || !Bm || !Qdiag || !Rdiag || !rho || !dK_out || !dP_out || nx <= 0 || nu <= 0 || B < 0)
+        return fail(TINYMPC_ERR_ARG, "null pointer or bad size");
+    if (dtype == TINYMPC_F64)
+        return sensitivity_batch_T<double>(nx, nu, B, (const double *)A, (const double *)Bm, (const double *)Qdiag, (const double *)Rdiag,
+                                           (const double *)rho, (double *)dK_out, (double *)dP_out, nthreads);
+    if (dtype == TINYMPC_F32)
+        return sensitivity_batch_T<float>(nx, nu, B, (const float *)A, (const float *)Bm, (const float *)Qdiag, (const float *)Rdiag,
+                                          (const float *)rho, (float *)dK_out, (float *)dP_out, nthreads);
+    return fail(TINYMPC_ERR_ARG, "bad dtype");
+}
+
+int tinympc_b200_precompute_sensitivity_batch_device(tinympc_b200_solver_t *s, int64_t B, const void *A, const void *Bm, const void *f,
+                                                     const void *Qdiag, const void *Rdiag, const void *rho, void *dK_out, void *dP_out,
+                                                     int32_t *sweeps_out, void *stream) {
+    (void)f;
+    if (!s) return fail(TINYMPC_ERR_ARG, "null handle");
+    if (!A || !Bm || !Qdiag || !Rdiag || !rho || !dK_out || !dP_out || B < 0) return fail(TINYMPC_ERR_ARG, "null pointer or bad size");
+    if (B == 0) return TINYMPC_OK;
+    CUDA_TRY(cudaSetDevice(s->device));
+    const int rc = s->dim->sensitivity_batch(s->pd.dtype, B, A, Bm, Qdiag, Rdiag, rho, dK_out, dP_out, sweeps_out, s->sm_count,
+                                             (cudaStream_t)stream);
+    if (rc == TINYMPC_ERR_CUDA) return fail(rc, std::string("sensitivity kernel launch failed: ") + cudaGetErrorString(cudaGetLastError()));
+    if (rc) return fail(rc, "sensitivity kernel unavailable for this dtype");
     return TINYMPC_OK;
 }
 
@@ -714,7 +776,7 @@ struct Field {
     void *dst;         // host output (may be null)
     size_t per_inst;   // bytes per instance
     bool is_in, is_out;
-    void **dev_slot;   // where the device pointer goes in the device-side tinympc_batch_t
+    void **dev_slot;   // where the device pointer goes in the device-side descriptors
     bool pinned = false;  // the caller's buffer is page-locked: DMA straight from/to it, no staging copy
 };
 
@@ -761,7 +823,12 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
 
     // shared (not per-instance) references are uploaded once, into a buffer the handle keeps
     DevBuf &shared_ref = s->shared_ref;
-    tinympc_batch_t dev = *io;  // template for the device-side descriptor
+    // template for the device-side descriptors: the batch, and the adaptive-rho arguments whose per-instance tables are staged
+    struct {
+        tinympc_batch_t io;
+        tinympc_adaptive_rho_t ar;
+    } args{*io, ar ? *ar : tinympc_adaptive_rho_t{}};
+    tinympc_batch_t &dev = args.io;
     const bool cold = io->cold_start != 0;
     std::vector<Field> fields;
     fields.push_back({io->x0, nullptr, es * s->pd.nx, true, false, (void **)&dev.x0});
@@ -770,6 +837,10 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     if (io->models) fields.push_back({io->models, nullptr, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, false, (void **)&dev.models});
     // adaptive rho: the model blobs are in/out; they travel in dev.models (io->models is NULL), where the kernel adapts them
     if (ar) fields.push_back({ar->models, ar->models, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, true, (void **)&dev.models});
+    if (ar && ar->tables_per_instance) {  // sliced per chunk like the models
+        fields.push_back({ar->dKinf_drho, nullptr, es * s->pd.nu * s->pd.nx, true, false, (void **)&args.ar.dKinf_drho});
+        fields.push_back({ar->dPinf_drho, nullptr, es * s->pd.nx * s->pd.nx, true, false, (void **)&args.ar.dPinf_drho});
+    }
     {
         size_t need = (io->xref_per_instance ? 0 : bx) + ((io->Uref && !io->uref_per_instance) ? bu : 0);
         if (need) {
@@ -848,15 +919,16 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
         if (drain(slot)) return fail(TINYMPC_ERR_CUDA, "event sync failed");
         // stage inputs into pinned memory, then one async copy per field
         char *pi = (char *)s->pin_in[slot].p, *pd = (char *)s->dio[slot].p;
-        tinympc_batch_t d = dev;
+        auto da = args;
+        tinympc_batch_t &d = da.io;
         d.B = nb;
         // device layout
         {
             char *cur = pd;
-            const char *base = (const char *)&dev;
+            const char *base = (const char *)&args;
             for (const Field &f : fields) {
                 size_t off = (const char *)f.dev_slot - base;
-                *(void **)((char *)&d + off) = cur;
+                *(void **)((char *)&da + off) = cur;
                 cur += padded(f.per_inst * chunk);
             }
         }
@@ -877,7 +949,7 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
         }
         CUDA_TRY(cudaEventRecord(s->ev_in[slot], s->st_h2d));
         CUDA_TRY(cudaStreamWaitEvent(s->st_k, s->ev_in[slot], 0));
-        if (int rc = enqueue(s, &d, s->st_k, false, ar)) return rc;
+        if (int rc = enqueue(s, &d, s->st_k, false, ar ? &da.ar : nullptr)) return rc;
         launches += s->stats.kernel_launches;
         CUDA_TRY(cudaEventRecord(s->ev_k[slot], s->st_k));
         CUDA_TRY(cudaStreamWaitEvent(s->st_d2h, s->ev_k[slot], 0));

@@ -69,15 +69,21 @@ constexpr int GPI_MAX_WARPS = 8;
 // parameter or kernel argument would rename the existing kernels, a shared __device__ body or a larger KParams changes their
 // machine code.)
 constexpr int GPI_ADAPT = 64;
+// ... with per-instance sensitivity tables (tinympc_adaptive_rho_t.tables_per_instance): added on top of GPI_ADAPT.  A variant of
+// its own, so that the shared-table adaptive kernel keeps its machine code (a run-time choice between the staged and the
+// per-instance tables cost it 2-3 %, DESIGN.md §5.5).
+constexpr int GPI_ADAPT_TABLES = 128;
 
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
 template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
 __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     gpi_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
-    constexpr bool ADAPT = LA >= GPI_ADAPT;  // adaptive rho
+    constexpr bool ADAPT = (LA & GPI_ADAPT) != 0;       // adaptive rho
+    constexpr bool PERTAB = LA >= GPI_ADAPT_TABLES;     // ... with per-instance tables
     constexpr int L = LA % GPI_ADAPT;
-    static_assert(LA < 2 * GPI_ADAPT && L > 0, "lane count: 4, 8 or 16, plus GPI_ADAPT for the adaptive variant");
+    static_assert(LA < 2 * GPI_ADAPT_TABLES && L > 0 && (ADAPT || !PERTAB),
+                  "lane count: 4, 8 or 16, plus GPI_ADAPT (and GPI_ADAPT_TABLES) for the adaptive variants");
     static_assert(!ADAPT || (HET && !FAST && !MM), "adaptive rho runs on heterogeneous STRICT batches");
     GpiAdapt<T> AP{};
     if constexpr (ADAPT) AP = *gpi_adapt_args<T>(P);
@@ -220,13 +226,15 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     const unsigned aPB = (unsigned)__cvta_generic_to_shared(gPB) + (unsigned)(lane * PVP) * ES;
     const unsigned aD = (unsigned)__cvta_generic_to_shared(gD) + (unsigned)lane * ES;
     const unsigned aGB = (unsigned)__cvta_generic_to_shared(gGB);
-    // ADAPT: dKinf_drho / dPinf_drho staged behind the state regions of all warps (and behind the dead blob staging area)
+    // ADAPT: dKinf_drho / dPinf_drho staged behind the state regions of all warps (and behind the dead blob staging area);
+    // per-instance tables (PERTAB) stay in global memory (adapt_blob)
     const T *sdK = nullptr, *sdP = nullptr;
     if constexpr (ADAPT) {
         size_t off = BLOB_KEEP + (size_t)(blockDim.x >> 5) * warp_elems * ES;
         off = ((off > BLOB_BYTES ? off : (size_t)BLOB_BYTES) + 15) / 16 * 16;
         T *t = reinterpret_cast<T *>(smem_raw + off);
-        for (int e = threadIdx.x; e < NU * NX + NX * NX; e += blockDim.x) t[e] = AP.dK[e];  // dP follows dK
+        if constexpr (!PERTAB)
+            for (int e = threadIdx.x; e < NU * NX + NX * NX; e += blockDim.x) t[e] = AP.dK[e];  // dP follows dK
         __syncthreads();
         sdK = t;
         sdP = t + NU * NX;
@@ -700,11 +708,16 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // Kinf += delta*dK; Kinf += delta2*dK (and Pinf) in this slot's blob for a pending slot, elements split over its L lanes
     auto adapt_blob = [&](const bool on) {
         T *mb = AP.models + (inst < 0 ? 0 : inst) * (int64_t)MB.model;
+        const T *tK = sdK, *tP = sdP;
+        if constexpr (PERTAB) {  // this instance's own pair, in global memory: AP.dK is [B][nu*nx], AP.dP [B][nx*nx]
+            tK = AP.dK + (inst < 0 ? 0 : inst) * (int64_t)(NU * NX);
+            tP = AP.dP + (inst < 0 ? 0 : inst) * (int64_t)(NX * NX);
+        }
         for (int e0 = 0; e0 < NU * NX + NX * NX; e0 += L) {
             const int e = e0 + l;
             if (on && e < NU * NX + NX * NX) {
                 const int o = e < NU * NX ? MB.Kinf + e : MB.Pinf + (e - NU * NX);
-                const T dv = e < NU * NX ? sdK[e] : sdP[e - NU * NX];
+                const T dv = e < NU * NX ? tK[e] : tP[e - NU * NX];
                 const T v1 = __ldcg(mb + o) + adelta * dv;
                 mb[o] = v1 + adelta2 * dv;
             }
@@ -717,12 +730,14 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         __syncwarp();
         if (pend) {
             if constexpr (!PS) {
+                const T *tK = sdK;
+                if constexpr (PERTAB) tK = AP.dK + inst * (int64_t)(NU * NX);
 #pragma unroll
                 for (int a = 0; a < RX; ++a) {
                     const int ii = xv[a] ? l * RX + a : 0;
 #pragma unroll
                     for (int j = 0; j < NU; ++j) {
-                        const T dv = sdK[j + NU * ii];
+                        const T dv = tK[j + NU * ii];
                         mKt[a][j] = xv[a] ? (mKt[a][j] + adelta * dv) + adelta2 * dv : T(0);
                     }
                 }
@@ -731,7 +746,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     const int jj = uv[b] ? l * RU + b : 0;
 #pragma unroll
                     for (int m = 0; m < NX; ++m) {
-                        const T dv = sdK[jj + NU * m];
+                        const T dv = tK[jj + NU * m];
                         mS1f[RX + b][m] = uv[b] ? (mS1f[RX + b][m] + adelta * dv) + adelta2 * dv : T(0);
                     }
                 }
@@ -1175,7 +1190,7 @@ inline GpiPlan gpi_plan(int N, int max_smem) {
     return p;
 }
 
-// launch the kernel of lane parameter LA (the lane count L, plus GPI_ADAPT for adaptive rho) with the plan d->gpi (d->gpi.L == L;
+// launch the kernel of lane parameter LA (the lane count L, plus GPI_ADAPT [+ GPI_ADAPT_TABLES] for adaptive rho) with the plan d->gpi (d->gpi.L == L;
 // for adaptive rho its smem includes gpi_adapt_bytes)
 template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
 int launch_gpi_L(LaunchDesc *d, const KParams<T, NX, NU> &P, const T *gmat) {

@@ -129,4 +129,53 @@ int precompute_cache(int nx, int nu, double rho_d, const T *Ap, const T *Bp, con
     return sweeps;
 }
 
+// Sensitivity tables dKinf/drho (nu x nx) and dPinf/drho (nx x nx) of one model: the forward-mode derivative, with respect
+// to rho, of the batched precompute as it runs (tinympc_b200_precompute_cache_batch: Q = Qdiag + rho, R = Rdiag + rho, then
+// precompute_cache above), tangent carried next to the same primal recursion and ended by the primal's own stop test:
+//   dQ1 = dR1 = 2 I (rho enters Q1, R1 twice), dP = I (P starts at rho I)
+//   per sweep, S = R1 + B'PB:  dS = dR1 + B'dP B ;  dK = S^-1 (B'dP A - dS K) ;  dPn = (dQ1 + A'dP (A - BK)) - A'P (B dK)
+// (the role rho_benchmark.cpp:215-229's tables play for the reference's one hard-coded quadrotor).  Q, R here are the
+// USER's diagonals, without rho.  Returns the sweeps used, or -1 exactly when precompute_cache would.
+template <typename T>
+int precompute_sensitivity(int nx, int nu, T rho, const T *Ap, const T *Bp, const T *Q, const T *R, T *dK_o, T *dP_o) {
+    Mat<T> A(nx, nx), B(nx, nu), Q1(nx, nx), R1(nu, nu), dR1(nu, nu), P(nx, nx), Kprev(nu, nx), K(nu, nx), Pn(nx, nx);
+    Mat<T> dP(nx, nx), dK(nu, nx), dPn(nx, nx);
+    A.a.assign(Ap, Ap + (size_t)nx * nx);
+    B.a.assign(Bp, Bp + (size_t)nx * nu);
+    for (int i = 0; i < nx; ++i) {
+        Q1(i, i) = (Q[i] + rho) + rho;
+        P(i, i) = rho;
+        dP(i, i) = T(1);
+    }
+    for (int j = 0; j < nu; ++j) {
+        R1(j, j) = (R[j] + rho) + rho;
+        dR1(j, j) = T(2);
+    }
+    const Mat<T> Bt = tr(B), At = tr(A);
+    for (int it = 0;; ++it) {
+        const Mat<T> BtP = mul(Bt, P), dBtP = mul(Bt, dP);
+        Mat<T> Sinv(nu, nu);
+        if (!invert(add(R1, mul(BtP, B)), Sinv)) return -1;
+        K = mul(Sinv, mul(BtP, A));
+        dK = mul(Sinv, sub(mul(dBtP, A), mul(add(dR1, mul(dBtP, B)), K)));
+        const Mat<T> AmBK = sub(A, mul(B, K)), AtP = mul(At, P);
+        Pn = add(Q1, mul(AtP, AmBK));
+        dPn = mul(mul(At, dP), AmBK);
+        for (int i = 0; i < nx; ++i) dPn(i, i) = T(2) + dPn(i, i);
+        dPn = sub(dPn, mul(AtP, mul(B, dK)));
+        T md = T(0);
+        for (size_t e = 0; e < K.a.size(); ++e) md = std::max(md, (T)std::fabs(K.a[e] - Kprev.a[e]));
+        if (md < (T)1e-5 || it == 999) {
+            Mat<T> Quu(nu, nu);
+            if (!invert(add(R1, mul(mul(Bt, Pn), B)), Quu)) return -1;
+            std::copy(dK.a.begin(), dK.a.end(), dK_o);
+            std::copy(dPn.a.begin(), dPn.a.end(), dP_o);
+            return it + 1;
+        }
+        Kprev = K;
+        P = Pn;
+        dP = dPn;
+    }
+}
+
 }  // namespace tmpc

@@ -69,6 +69,15 @@ int precompute_batch(int dtype, int64_t B, const void *A, const void *Bm, const 
     return TINYMPC_ERR_ARG;
 }
 
+int sensitivity_batch(int dtype, int64_t B, const void *A, const void *Bm, const void *Qdiag, const void *Rdiag, const void *rho,
+                      void *dK_out, void *dP_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream) {
+    if (dtype == TINYMPC_F32)
+        return launch_sensitivity_T<float, TM_NX, TM_NU>(B, A, Bm, Qdiag, Rdiag, rho, dK_out, dP_out, sweeps_out, sm_count, stream);
+    if (dtype == TINYMPC_F64)
+        return launch_sensitivity_T<double, TM_NX, TM_NU>(B, A, Bm, Qdiag, Rdiag, rho, dK_out, dP_out, sweeps_out, sm_count, stream);
+    return TINYMPC_ERR_ARG;
+}
+
 }  // namespace
 }  // namespace tmpc
 
@@ -78,6 +87,7 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
                                      &tmpc::launch,
                                      &TM_SYM(tm_gpi_plan_),
                                      &tmpc::precompute_batch,
+                                     &tmpc::sensitivity_batch,
                                      &TM_SYM(tm_gps_lanes_),
                                      &TM_SYM(tm_gps_het_slots_)};
     return &e;
@@ -106,6 +116,8 @@ int launch_gpi(LaunchDesc *d) {
 #define TM_GPI_CASE(LL)                                                                                                  \
     if (L == LL) {                                                                                                       \
         if constexpr (!FAST) {                                                                                           \
+            if (d->adapt == 2) /* per-instance tables */                                                                 \
+                return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT + GPI_ADAPT_TABLES, false, true>(d, P, gmat);              \
             if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                       \
             if constexpr (sizeof(T) == 4)                                                                                \
                 if (!het && d->pd->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, false, false, true>(d, P, gmat); \

@@ -60,7 +60,7 @@ struct LaunchDesc {
 
     // adaptive rho (tinympc_b200_solve_adaptive): io.models is then the in/out blob array; adapt_args = device copy of
     // GpiAdapt<T> (adapt.h) followed by dKinf_drho and dPinf_drho
-    int adapt;
+    int adapt;  // 0: no; 1: one shared table pair; 2: per-instance tables
     const void *adapt_args;
 
     cudaStream_t stream;
@@ -100,6 +100,9 @@ struct DimEntry {
     // batched cache precompute on the device (precompute_kernel.cuh): device pointers, one model blob per instance
     int (*precompute_batch)(int dtype, int64_t B, const void *A, const void *Bm, const void *f, const void *Qdiag, const void *Rdiag,
                             const void *rho, void *models_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);
+    // batched sensitivity tables on the device (precompute_kernel.cuh): device pointers, dK [B][nu*nx], dP [B][nx*nx]
+    int (*sensitivity_batch)(int dtype, int64_t B, const void *A, const void *Bm, const void *Qdiag, const void *Rdiag, const void *rho,
+                             void *dK_out, void *dP_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);
     // streamed lane-group kernel (gps_kernel.cuh): lanes per instance; 0 = shape not available
     int (*gps_lanes)(int dtype);
     // its per-instance-model variant (io.models): instances per CTA when the batch fills every SM, for the shape and the

@@ -236,4 +236,134 @@ int launch_precompute_T(int64_t Bn, const void *A, const void *Bm, const void *f
     return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
 }
 
+// ---- sensitivity tables dKinf/drho, dPinf/drho (host_precompute.h: precompute_sensitivity) ----
+// The same primal recursion with its tangent carried alongside, one warp per instance, every element by the host routine's
+// operation sequence: the tables are BIT-IDENTICAL to tinympc_b200_precompute_sensitivity_batch's.  A singular S is found by
+// the same pc_invert calls as in precompute_cache_kernel, so sweeps_out is -1 for exactly the same models.
+template <int NX, int NU>
+struct PsLayout : PcLayout<NX, NU> {
+    using Pc = PcLayout<NX, NU>;
+    // the tangent's scratch behind the primal's
+    static constexpr int DP = Pc::TOTAL, DPN = DP + Pc::XX, DATP = DPN + Pc::XX, BDK = DATP + Pc::XX, DBTP = BDK + Pc::XX, T1 = DBTP + Pc::XU,
+                         T2 = T1 + Pc::XU, DK = T2 + Pc::XU, DS = DK + Pc::XU, TOTAL = DS + Pc::UU;
+};
+
+template <typename T, int NX, int NU>
+__global__ void __launch_bounds__(PC_WARPS * 32)
+    precompute_sensitivity_kernel(int64_t Bn, const T *__restrict__ Ag, const T *__restrict__ Bg, const T *__restrict__ Qg,
+                                  const T *__restrict__ Rg, const T *__restrict__ rhog, T *__restrict__ dK_out, T *__restrict__ dP_out,
+                                  int32_t *__restrict__ sweeps_out) {
+    using Lo = PsLayout<NX, NU>;
+    extern __shared__ __align__(16) unsigned char pc_smem_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T *w = reinterpret_cast<T *>(pc_smem_raw) + (size_t)warp * Lo::TOTAL;
+    T *A = w + Lo::A, *Bm = w + Lo::B, *P = w + Lo::P, *Pn = w + Lo::PN, *BtP = w + Lo::BTP, *BtPA = w + Lo::BTPA, *K = w + Lo::K,
+      *Kp = w + Lo::KP, *S = w + Lo::S, *Si = w + Lo::SI, *AmBK = w + Lo::AMBK, *AtP = w + Lo::ATP, *Q1 = w + Lo::Q1, *R1 = w + Lo::R1;
+    T *dP = w + Lo::DP, *dPn = w + Lo::DPN, *dAtP = w + Lo::DATP, *BdK = w + Lo::BDK, *dBtP = w + Lo::DBTP, *T1 = w + Lo::T1,
+      *T2 = w + Lo::T2, *dK = w + Lo::DK, *dS = w + Lo::DS;
+
+    for (int64_t b = (int64_t)blockIdx.x * PC_WARPS + warp; b < Bn; b += (int64_t)gridDim.x * PC_WARPS) {
+        const T rho = rhog[b];
+        for (int e = lane; e < Lo::XX; e += 32) {
+            const bool diag = e % NX == e / NX;
+            A[e] = Ag[b * Lo::XX + e];
+            P[e] = diag ? rho : T(0);    // P <- rho I
+            dP[e] = diag ? T(1) : T(0);  // dP <- I
+        }
+        for (int e = lane; e < Lo::XU; e += 32) {
+            Bm[e] = Bg[b * Lo::XU + e];
+            Kp[e] = T(0);
+        }
+        for (int e = lane; e < NX; e += 32) Q1[e] = (Qg[b * NX + e] + rho) + rho;  // tiny_api.cpp:117, :317
+        for (int e = lane; e < NU; e += 32) R1[e] = (Rg[b * NU + e] + rho) + rho;  // :118, :318
+        __syncwarp();
+        auto a_ = [&](int i, int j) { return A[i + j * NX]; };
+        auto at_ = [&](int i, int j) { return A[j + i * NX]; };
+        auto b_ = [&](int i, int j) { return Bm[i + j * NX]; };
+        auto bt_ = [&](int i, int j) { return Bm[j + i * NX]; };
+        auto mat = [](const T *M, int rows) { return [M, rows](int i, int j) { return M[i + j * rows]; }; };
+        // Z = diag(d) + (BtX) B, as add(diagonal matrix, mul(..)): off-diagonal entries are 0 + product
+        auto form_S = [&](T *Z, const T *BtX, auto d) {
+            pc_mul<T, NU, NU, NX>(Z, mat(BtX, NU), b_, lane);
+            for (int e = lane; e < Lo::UU; e += 32) Z[e] = ((e % NU == e / NU) ? d(e % NU) : T(0)) + Z[e];
+            __syncwarp();
+        };
+        auto r1_ = [&](int j) { return R1[j]; };
+        int sweeps = 0;
+        bool ok = true;
+        for (int it = 0; it < 1000; ++it) {
+            pc_mul<T, NU, NX, NX>(BtP, bt_, mat(P, NX), lane);
+            pc_mul<T, NU, NX, NX>(dBtP, bt_, mat(dP, NX), lane);
+            form_S(S, BtP, r1_);
+            if (!pc_invert<T, NU>(S, Si, lane)) {
+                ok = false;
+                break;
+            }
+            pc_mul<T, NU, NX, NX>(BtPA, mat(BtP, NU), a_, lane);
+            pc_mul<T, NU, NX, NU>(K, mat(Si, NU), mat(BtPA, NU), lane);
+            // dK = S^-1 (B'dP A - dS K), dS = 2 I + B'dP B
+            pc_mul<T, NU, NX, NX>(T1, mat(dBtP, NU), a_, lane);
+            form_S(dS, dBtP, [](int) { return T(2); });
+            pc_mul<T, NU, NX, NU>(T2, mat(dS, NU), mat(K, NU), lane);
+            for (int e = lane; e < Lo::XU; e += 32) T1[e] = T1[e] - T2[e];
+            __syncwarp();
+            pc_mul<T, NU, NX, NU>(dK, mat(Si, NU), mat(T1, NU), lane);
+            // AmBK = A - B K ; Pn = Q1 + A'P AmBK
+            pc_mul<T, NX, NX, NU>(AmBK, b_, mat(K, NU), lane);
+            for (int e = lane; e < Lo::XX; e += 32) AmBK[e] = A[e] - AmBK[e];
+            __syncwarp();
+            pc_mul<T, NX, NX, NX>(AtP, at_, mat(P, NX), lane);
+            pc_mul<T, NX, NX, NX>(Pn, mat(AtP, NX), mat(AmBK, NX), lane);
+            for (int e = lane; e < Lo::XX; e += 32) Pn[e] = ((e % NX == e / NX) ? Q1[e % NX] : T(0)) + Pn[e];
+            // dPn = (2 I + A'dP AmBK) - A'P (B dK)
+            pc_mul<T, NX, NX, NX>(dAtP, at_, mat(dP, NX), lane);
+            pc_mul<T, NX, NX, NX>(dPn, mat(dAtP, NX), mat(AmBK, NX), lane);
+            pc_mul<T, NX, NX, NU>(BdK, b_, mat(dK, NU), lane);
+            pc_mul<T, NX, NX, NX>(dAtP, mat(AtP, NX), mat(BdK, NX), lane);  // dAtP is free again: A'P (B dK)
+            for (int e = lane; e < Lo::XX; e += 32) {
+                const T v = (e % NX == e / NX) ? T(2) + dPn[e] : dPn[e];
+                dPn[e] = v - dAtP[e];
+            }
+            __syncwarp();
+            sweeps = it + 1;
+            T md = T(0);
+            for (int e = lane; e < Lo::XU; e += 32) md = fmax(md, fabs(K[e] - Kp[e]));
+#pragma unroll
+            for (int m = 16; m >= 1; m >>= 1) md = fmax(md, __shfl_xor_sync(0xffffffffu, md, m));
+            if (md < (T)1e-5) break;
+            for (int e = lane; e < Lo::XU; e += 32) Kp[e] = K[e];
+            for (int e = lane; e < Lo::XX; e += 32) {
+                P[e] = Pn[e];
+                dP[e] = dPn[e];
+            }
+            __syncwarp();
+        }
+        if (ok) {  // the cache's Quu_inv = (R1 + B' Pinf B)^-1 must exist too
+            pc_mul<T, NU, NX, NX>(BtP, bt_, mat(Pn, NX), lane);
+            form_S(S, BtP, r1_);
+            ok = pc_invert<T, NU>(S, Si, lane);
+        }
+        if (ok) {
+            for (int e = lane; e < Lo::XU; e += 32) dK_out[b * Lo::XU + e] = dK[e];
+            for (int e = lane; e < Lo::XX; e += 32) dP_out[b * Lo::XX + e] = dPn[e];
+        }
+        if (lane == 0 && sweeps_out) sweeps_out[b] = ok ? sweeps : -1;
+        __syncwarp();
+    }
+}
+
+template <typename T, int NX, int NU>
+int launch_sensitivity_T(int64_t Bn, const void *A, const void *Bm, const void *Q, const void *R, const void *rho, void *dK, void *dP,
+                         int32_t *sweeps, int sm_count, cudaStream_t stream) {
+    using Lo = PsLayout<NX, NU>;
+    auto kern = precompute_sensitivity_kernel<T, NX, NU>;
+    const size_t smem = (size_t)PC_WARPS * Lo::TOTAL * sizeof(T);
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return TINYMPC_ERR_CUDA;
+    const int64_t want = (Bn + PC_WARPS - 1) / PC_WARPS;
+    const int ctas = (int)std::max<int64_t>(1, std::min<int64_t>((int64_t)sm_count * 8, want));
+    kern<<<ctas, PC_WARPS * 32, smem, stream>>>(Bn, (const T *)A, (const T *)Bm, (const T *)Q, (const T *)R, (const T *)rho, (T *)dK,
+                                                (T *)dP, sweeps);
+    return cudaGetLastError() == cudaSuccess ? TINYMPC_OK : TINYMPC_ERR_CUDA;
+}
+
 }  // namespace tmpc

@@ -80,6 +80,29 @@ def setup_models(nx, nu, A, B, f, Qdiag, Rdiag, rho, dtype=np.float32, nthreads=
     return out
 
 
+def setup_sensitivity(nx, nu, A, B, f, Qdiag, Rdiag, rho, dtype=np.float32, nthreads=0):
+    """The adaptive-rho sensitivity tables of Bn models (tinympc_b200_precompute_sensitivity_batch): the derivative with
+    respect to rho of the Kinf / Pinf setup_models computes, inputs as in setup_models.  Returns (dKinf_drho [Bn, nu, nx],
+    dPinf_drho [Bn, nx, nx]) indexed (instance, row, column), as AdaptiveRho takes them."""
+    import os
+
+    lib = load()
+    dt = np.dtype(dtype).type
+    A = np.asarray(A, dtype=dt)
+    Bn = A.shape[0]
+    A_ = np.ascontiguousarray(np.transpose(A.reshape(Bn, nx, nx), (0, 2, 1)))          # column-major per instance
+    B_ = np.ascontiguousarray(np.transpose(np.asarray(B, dtype=dt).reshape(Bn, nx, nu), (0, 2, 1)))
+    f_ = np.ascontiguousarray(np.asarray(f, dtype=dt).reshape(Bn, nx))
+    Q_ = np.ascontiguousarray(np.asarray(Qdiag, dtype=dt).reshape(Bn, nx))
+    R_ = np.ascontiguousarray(np.asarray(Rdiag, dtype=dt).reshape(Bn, nu))
+    r_ = np.ascontiguousarray(np.broadcast_to(np.asarray(rho, dtype=dt), (Bn,)))
+    dK, dP = np.zeros((Bn, nx, nu), dtype=dt), np.zeros((Bn, nx, nx), dtype=dt)  # column-major per instance
+    vp = lambda a: C.c_void_p(a.ctypes.data)  # noqa: E731
+    check(lib.tinympc_b200_precompute_sensitivity_batch(dtype_code(dt), nx, nu, Bn, vp(A_), vp(B_), vp(f_), vp(Q_), vp(R_), vp(r_),
+                                                        vp(dK), vp(dP), nthreads or (os.cpu_count() or 1)))
+    return np.transpose(dK, (0, 2, 1)), np.transpose(dP, (0, 2, 1))
+
+
 def unpack_model(blob, nx, nu):
     """One per-instance blob -> dict of column-major pieces (for building the equivalent single-model MPCProblem)."""
     sizes = [("A", (nx, nx)), ("B", (nx, nu)), ("f", (nx,)), ("Q", (nx,)), ("R", (nu,)), ("Kinf", (nu, nx)), ("Pinf", (nx, nx)),
@@ -105,21 +128,49 @@ def pack_models(problem: MPCProblem, B: int):
 
 class AdaptiveRho:
     """The reference's adaptive-rho settings (settings->adaptive_rho_min / _max / _enable_clipping) and sensitivity tables
-    (cache->dKinf_drho nu x nx, dPinf_drho nx x nx), for BatchedTinySolver.solve(..., adaptive_rho=...)."""
+    (cache->dKinf_drho nu x nx, dPinf_drho nx x nx), for BatchedTinySolver.solve(..., adaptive_rho=...).  Tables with a
+    leading batch dimension ([B, nu, nx], [B, nx, nx], e.g. from setup_sensitivity[_device]) give every instance its own
+    pair: what a fleet of different models needs."""
 
     def __init__(self, dKinf_drho, dPinf_drho, rho_min=1.0, rho_max=100.0, enable_clipping=True):
         self.dKinf_drho, self.dPinf_drho = dKinf_drho, dPinf_drho
         self.rho_min, self.rho_max, self.enable_clipping = float(rho_min), float(rho_max), bool(enable_clipping)
+        self.per_instance = len(dKinf_drho.shape) == 3 if hasattr(dKinf_drho, "shape") else np.ndim(dKinf_drho) == 3
 
-    def to_c(self, problem: MPCProblem, models_ptr) -> abi.AdaptiveRho:
-        dt = problem.dtype
-        dK = np.asfortranarray(np.asarray(self.dKinf_drho, dtype=dt).reshape(problem.nu, problem.nx))
-        dP = np.asfortranarray(np.asarray(self.dPinf_drho, dtype=dt).reshape(problem.nx, problem.nx))
+    def to_c(self, problem: MPCProblem, models_ptr, B=None, device=None) -> abi.AdaptiveRho:
+        """device: None = the host entry point (tables as host arrays); a torch device = tinympc_b200_solve_adaptive, whose
+        per-instance tables are device arrays (CUDA tensors already in place are passed without a copy)."""
+        dt, nx, nu = problem.dtype, problem.nx, problem.nu
         a = abi.AdaptiveRho()
         a.rho_min, a.rho_max, a.enable_clipping, a.reserved = self.rho_min, self.rho_max, int(self.enable_clipping), 0
-        a.dKinf_drho, a.dPinf_drho, a.models = dK.ctypes.data, dP.ctypes.data, models_ptr
+        a.tables_per_instance = int(self.per_instance)
+        if not self.per_instance:
+            dK = np.asfortranarray(_host(self.dKinf_drho, dt).reshape(nu, nx))
+            dP = np.asfortranarray(_host(self.dPinf_drho, dt).reshape(nx, nx))
+            a.dKinf_drho, a.dPinf_drho = dK.ctypes.data, dP.ctypes.data
+        else:
+            B = self.dKinf_drho.shape[0] if B is None else B
+            if tuple(self.dKinf_drho.shape) != (B, nu, nx) or tuple(self.dPinf_drho.shape) != (B, nx, nx):
+                raise ValueError(f"per-instance tables must be [{B}, {nu}, {nx}] and [{B}, {nx}, {nx}]")
+            if device is None:  # column-major per instance
+                dK = np.ascontiguousarray(np.transpose(_host(self.dKinf_drho, dt), (0, 2, 1)))
+                dP = np.ascontiguousarray(np.transpose(_host(self.dPinf_drho, dt), (0, 2, 1)))
+                a.dKinf_drho, a.dPinf_drho = dK.ctypes.data, dP.ctypes.data
+            else:
+                import torch
+
+                tdt = torch.float32 if dt == np.float32 else torch.float64
+                dK = torch.as_tensor(self.dKinf_drho, device=device).to(tdt).transpose(1, 2).contiguous()
+                dP = torch.as_tensor(self.dPinf_drho, device=device).to(tdt).transpose(1, 2).contiguous()
+                a.dKinf_drho, a.dPinf_drho = dK.data_ptr(), dP.data_ptr()
+        a.models = models_ptr
         a._owner = (dK, dP)
         return a
+
+
+def _host(a, dt):
+    """numpy array of dtype dt from a numpy array or a torch tensor on any device"""
+    return np.asarray(a.detach().cpu().numpy() if hasattr(a, "detach") else a, dtype=dt)
 
 
 class BatchedTinySolver:
@@ -178,7 +229,7 @@ class BatchedTinySolver:
             return hb.result()
         hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state)
         m = pack_models(self.problem, hb.B) if models is None else np.array(models, dtype=self.problem.dtype).reshape(hb.B, -1)
-        cb, ar = hb.to_c(), adaptive_rho.to_c(self.problem, m.ctypes.data)
+        cb, ar = hb.to_c(), adaptive_rho.to_c(self.problem, m.ctypes.data, hb.B)
         check(self._lib.tinympc_b200_solve_adaptive_host(self._h, C.byref(cb), C.byref(ar)))
         out = hb.result()
         out["models"] = m
@@ -213,6 +264,32 @@ class BatchedTinySolver:
             self._h, Bn, A_.data_ptr(), B_.data_ptr(), f_.data_ptr(), Q_.data_ptr(), R_.data_ptr(), r_.data_ptr(), out.data_ptr(),
             None if sweeps is None else sweeps.data_ptr(), C.c_void_p(stream)))
         return (out, sweeps) if want_sweeps else out
+
+    def setup_sensitivity_device(self, A, B, f, Qdiag, Rdiag, rho, want_sweeps=False):
+        """setup_sensitivity on the GPU (tinympc_b200_precompute_sensitivity_batch_device), inputs as in setup_models_device:
+        torch CUDA tensors (dKinf_drho [Bn, nu, nx], dPinf_drho [Bn, nx, nx]) indexed (instance, row, column), views of the
+        column-major storage the adaptive solve reads: AdaptiveRho passes them on without a copy.  Bit-identical to the host
+        routine."""
+        import torch
+
+        p = self.problem
+        tdt = torch.float32 if p.dtype == np.float32 else torch.float64
+        dev = torch.device("cuda", self.device)
+        t = lambda a: torch.as_tensor(a, device=dev).to(tdt)  # noqa: E731
+        A_ = t(A).reshape(-1, p.nx, p.nx).transpose(1, 2).contiguous()  # column-major per instance
+        Bn = A_.shape[0]
+        B_ = t(B).reshape(Bn, p.nx, p.nu).transpose(1, 2).contiguous()
+        f_, Q_, R_ = t(f).reshape(Bn, p.nx).contiguous(), t(Qdiag).reshape(Bn, p.nx).contiguous(), t(Rdiag).reshape(Bn, p.nu).contiguous()
+        r_ = t(rho).reshape(-1).expand(Bn).contiguous()
+        dK = torch.zeros((Bn, p.nx, p.nu), dtype=tdt, device=dev)
+        dP = torch.zeros((Bn, p.nx, p.nx), dtype=tdt, device=dev)
+        sweeps = torch.zeros(Bn, dtype=torch.int32, device=dev) if want_sweeps else None
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        check(self._lib.tinympc_b200_precompute_sensitivity_batch_device(
+            self._h, Bn, A_.data_ptr(), B_.data_ptr(), f_.data_ptr(), Q_.data_ptr(), R_.data_ptr(), r_.data_ptr(), dK.data_ptr(),
+            dP.data_ptr(), None if sweeps is None else sweeps.data_ptr(), C.c_void_p(stream)))
+        dK, dP = dK.transpose(1, 2), dP.transpose(1, 2)
+        return (dK, dP, sweeps) if want_sweeps else (dK, dP)
 
     # ---- device buffers (torch tensors on cuda:<device>) ---------------------------------------------
     def make_device_batch(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), want_residuals=True,
@@ -291,5 +368,5 @@ class BatchedTinySolver:
                 and models.dtype == (torch.float32 if p.dtype == np.float32 else torch.float64)):
             raise ValueError(f"models must be a contiguous CUDA tensor of {batch.B} x {M} elements of the problem dtype")
         s = stream if stream is not None else torch.cuda.current_stream(self.device)
-        ar = adaptive_rho.to_c(p, models.data_ptr())
+        ar = adaptive_rho.to_c(p, models.data_ptr(), batch.B, models.device)
         check(self._lib.tinympc_b200_solve_adaptive(self._h, C.byref(batch), C.byref(ar), C.c_void_p(s.cuda_stream)))
