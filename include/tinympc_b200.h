@@ -342,6 +342,47 @@ int tinympc_b200_solve_adaptive(tinympc_b200_solver_t *s, const tinympc_batch_t 
 int tinympc_b200_solve_adaptive_host(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar);
 
 /*
+ * Closed-loop rollout: T warm-started MPC steps per instance in one launch, the loop of the reference's examples
+ * (examples/quadrotor_tracking.cpp:77-106).  For every instance b and step t = 0 ... T-1 the result is bit-identical to
+ *     solve (warm start from step t-1; the first step is cold or warm from io->state per io->cold_start) with
+ *         x0 = the plant state, Xref = knot points t ... t+N-1 of Xref, Uref = knot points t ... t+N-2 of Uref;
+ *     u0 = work->u.col(0);  x0 <- (Adyn x0 + Bdyn u0) + fdyn  (tinympc_b200_advance[_models]);  x0 <- x0 + w[b][t]
+ * with the warm state kept on chip from one step to the next.  reset_duals = 1 zeroes g, y before every step after the first
+ * (zero io->state.g / y yourself to reset them before the first).  carry_v = 1 carries work->v / work->z (the slack of the
+ * previous iteration, which feeds the first iteration's dual residual) from one step to the next, as a solve with state.v / z
+ * would; carry_v = 0 reads them as zeros at every step and needs io->state.v / z NULL.
+ *
+ *   io: B, x0 (the initial plant states, not modified), cold_start, state (in: the first step's warm start; out: the state
+ *       after the last step; x and u must be NULL), models (a fleet: every instance solves and advances with its own blob),
+ *       optional sol_x / sol_u (solution of the last step).  Xref, Uref, iter, solved, residuals and u0 must be NULL.
+ *   Xref: [B][T+N-1][nx] (xref_per_instance) or [T+N-1][nx]; Uref: [B][T+N-2][nu] / [T+N-2][nu], or NULL = zeros.
+ *   Outputs, each may be NULL: x_traj [B][T+1][nx] the plant state before step t and after the last one; u_traj [B][T][nu];
+ *   iter_traj, solved_traj [B][T]; residuals_traj [B][T][4].  T = 0 writes nothing.
+ * All pointers are DEVICE pointers; asynchronous on `cuda_stream`.  Served by the on-chip (GPI) kernel in STRICT mode with box
+ * constraints only, with the launch plan a solve of the same batch gets on it (stats() reports it); FAST mode, cones,
+ * hyperplanes, a horizon that does not fit on chip and an explicit TPI or GPS family return TINYMPC_ERR_UNSUPPORTED.
+ */
+typedef struct tinympc_rollout {
+    int32_t T;            /* steps per instance, >= 0 */
+    int32_t reset_duals;  /* 0 / 1 */
+    int32_t carry_v;      /* 0 / 1 */
+    int32_t xref_per_instance;
+    const void *Xref;
+    const void *Uref;
+    int32_t uref_per_instance;
+    int32_t reserved;     /* must be 0 */
+    const void *w;        /* [B][T][nx] disturbance, or NULL */
+    void *x_traj;         /* [B][T+1][nx] */
+    void *u_traj;         /* [B][T][nu] */
+    int32_t *iter_traj;   /* [B][T] */
+    int32_t *solved_traj; /* [B][T] */
+    void *residuals_traj; /* [B][T][4] */
+    int64_t reserved1[2]; /* must be 0 */
+} tinympc_rollout_t;
+
+int tinympc_b200_rollout(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_rollout_t *ro, void *cuda_stream);
+
+/*
  * Closed-loop helper (the caller of the hot path, e.g. examples/quadrotor_tracking.cpp:105):
  *     x0[b] <- (Adyn * x0[b] + Bdyn * u[b][:,0]) + fdyn        for b in [0, B)
  * with x0 [B][nx] (in/out) and u pointing at the first control of instance 0, consecutive instances `u_stride`

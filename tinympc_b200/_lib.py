@@ -50,6 +50,7 @@ def load():
     lib.tinympc_b200_set_mode.argtypes = [vp, C.c_int32, C.c_int32]
     lib.tinympc_b200_solve.argtypes = [vp, C.POINTER(abi.Batch), vp]
     lib.tinympc_b200_solve_host.argtypes = [vp, C.POINTER(abi.Batch)]
+    lib.tinympc_b200_rollout.argtypes = [vp, C.POINTER(abi.Batch), C.POINTER(abi.Rollout), vp]
     lib.tinympc_b200_get_stats.argtypes = [vp, C.POINTER(abi.Stats)]
     lib.tinympc_b200_advance.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp]
     lib.tinympc_b200_advance_models.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, vp]

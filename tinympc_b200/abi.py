@@ -96,6 +96,18 @@ class AdaptiveRho(C.Structure):
     ]
 
 
+class Rollout(C.Structure):
+    """tinympc_rollout_t: T closed-loop steps per instance, their reference trajectories, disturbance and per-step outputs."""
+    _fields_ = [
+        ("T", C.c_int32), ("reset_duals", C.c_int32), ("carry_v", C.c_int32), ("xref_per_instance", C.c_int32),
+        ("Xref", vp), ("Uref", vp),
+        ("uref_per_instance", C.c_int32), ("reserved", C.c_int32),
+        ("w", vp),
+        ("x_traj", vp), ("u_traj", vp), ("iter_traj", vp), ("solved_traj", vp), ("residuals_traj", vp),
+        ("reserved1", C.c_int64 * 2),
+    ]
+
+
 # every entry point declared in include/tinympc_b200.h
 EXPORTS = [
     "tinympc_b200_default_settings",
@@ -114,6 +126,7 @@ EXPORTS = [
     "tinympc_b200_solve_host",
     "tinympc_b200_solve_adaptive",
     "tinympc_b200_solve_adaptive_host",
+    "tinympc_b200_rollout",
     "tinympc_b200_get_stats",
     "tinympc_b200_advance",
     "tinympc_b200_advance_models",

@@ -85,3 +85,76 @@ class DeviceMPCLoop:
             check(s._lib.tinympc_b200_advance_models(s._h, self.B, x0p, u0p, s.problem.nu, C.c_void_p(self.models.data_ptr()),
                                                      C.c_void_p(st.cuda_stream)))
         return out
+
+    def rollout(self, Xref_traj, T: int, Uref_traj=None, w=None, stream=None):
+        """T steps in one launch (tinympc_b200_rollout): bit-identical to
+            for t in range(T): self.step(Xref_traj[..., t:t+N, :], Uref_traj[..., t:t+N-1, :]); self.x0 += w[:, t]
+        with the warm state kept on chip between steps.  Xref_traj: [B, >= T+N-1, nx] or [>= T+N-1, nx]; Uref_traj: [B, >= T+N-2, nu]
+        or [>= T+N-2, nu] or None; w: [B, T, nx] or None.  Returns device tensors with a step axis: x [B, T+1, nx] (the plant
+        state before every step and after the last), u [B, T, nu], iter / solved [B, T], residuals [B, T, 4].  Leaves x0,
+        state and out as the T steps would.  Box constraints only, without adaptive rho (the on-chip kernel's rollout variant)."""
+        import torch
+
+        if self.adaptive_rho is not None:
+            raise ValueError("rollout: adaptive rho is not available in a rollout; use step()")
+        if len(self.fields) != len(WARM_FIELDS if "v" in self.fields else WARM_FIELDS_FAST):
+            raise ValueError("rollout: covers box constraints only (no extra_state); use step()")
+        T = int(T)
+        if T < 0:
+            raise ValueError("rollout: T must be >= 0")
+        s, p = self.solver, self.solver.problem
+        B, N = self.B, p.N
+        st = stream if stream is not None else torch.cuda.current_stream(s.device)
+
+        def traj(a, knots, width, name):
+            a = torch.as_tensor(a, device=self.dev).to(self._tdt)
+            if a.dim() not in (2, 3) or a.shape[-2] < knots or a.shape[-1] != width or (a.dim() == 3 and a.shape[0] != B):
+                raise ValueError(f"rollout: {name} must be [{B}, >= {knots}, {width}] or [>= {knots}, {width}]")
+            return a[..., :knots, :].contiguous()
+
+        X = traj(Xref_traj, T + N - 1, p.nx, "Xref_traj")
+        U = None if Uref_traj is None else traj(Uref_traj, T + N - 2, p.nu, "Uref_traj")
+        W = None
+        if w is not None:
+            W = torch.as_tensor(w, device=self.dev).to(self._tdt).contiguous()
+            if tuple(W.shape) != (B, T, p.nx):
+                raise ValueError(f"rollout: w must be [{B}, {T}, {p.nx}]")
+        if self.state is not None and self.reset_duals:
+            self.state["g"].zero_()
+            self.state["y"].zero_()
+        kw = dict(dtype=self._tdt, device=self.dev)
+        state = self.state
+        if state is None:
+            state = {n: torch.zeros((B, N, p.nx) if abi.STATE_IS_X[n] else (B, N - 1, p.nu), **kw) for n in self.fields}
+        het = self.models is not None
+        res = dict(x=torch.empty((B, T + 1, p.nx), **kw), u=torch.empty((B, T, p.nu), **kw),
+                   iter=torch.empty((B, T), dtype=torch.int32, device=self.dev),
+                   solved=torch.empty((B, T), dtype=torch.int32, device=self.dev), residuals=torch.empty((B, T, 4), **kw))
+        sol_x = torch.empty((B, N, p.nx), **kw) if self.want_solution else None
+        sol_u = torch.empty((B, N - 1, p.nu), **kw) if self.want_solution else None
+        b = abi.Batch()
+        b.B, b.x0, b.cold_start = B, self.x0.data_ptr(), int(self._first)
+        for n, a in state.items():
+            setattr(b.state, n, a.data_ptr())
+        b.sol_x = None if sol_x is None else sol_x.data_ptr()
+        b.sol_u = None if sol_u is None else sol_u.data_ptr()
+        b.models = self.models.data_ptr() if het else None
+        r = abi.Rollout()
+        r.T, r.reset_duals, r.carry_v = T, int(self.reset_duals), int("v" in self.fields)
+        r.Xref, r.xref_per_instance = X.data_ptr(), int(X.dim() == 3)
+        r.Uref, r.uref_per_instance = (None, 0) if U is None else (U.data_ptr(), int(U.dim() == 3))
+        r.w = None if W is None else W.data_ptr()
+        r.x_traj, r.u_traj, r.residuals_traj = res["x"].data_ptr(), res["u"].data_ptr(), res["residuals"].data_ptr()
+        r.iter_traj, r.solved_traj = res["iter"].data_ptr(), res["solved"].data_ptr()
+        check(s._lib.tinympc_b200_rollout(s._h, C.byref(b), C.byref(r), C.c_void_p(st.cuda_stream)))
+        self._roll_inputs = (X, U, W)  # read by the launch on `stream`
+        if T == 0:
+            res["x"] = self.x0.clone().reshape(B, 1, p.nx)
+            return res
+        self.state = state
+        self.out = dict(sol_x=sol_x, sol_u=sol_u, u0=res["u"][:, -1], iter=res["iter"][:, -1], solved=res["solved"][:, -1],
+                        residuals=res["residuals"][:, -1], **state)
+        self._first = False
+        with torch.cuda.stream(st):
+            self.x0.copy_(res["x"][:, -1])
+        return res

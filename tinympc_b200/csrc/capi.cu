@@ -17,6 +17,7 @@
 #include "host_precompute.h"
 #include "kparams_fill.h"
 #include "model_blob.h"
+#include "rollout.h"
 
 #define TM_DECL(nx, nu) extern "C" const tmpc::DimEntry *tm_dim_entry_##nx##_##nu();
 TM_DIMS(TM_DECL)
@@ -118,13 +119,13 @@ struct tinympc_b200_solver {
     DevBuf vscratch;
     DevBuf gps_ws;
     DevBuf shared_ref;  // host path: references shared by the whole batch
-    DevBuf d_adapt;     // adaptive rho: GpiAdapt arguments + the shared dKinf_drho + dPinf_drho (adapt.h)
-    // page-locked staging of d_adapt's contents, a ring so that the copy stays asynchronous: slot i is rewritten only once
-    // the copy three solves back (ev_adapt[i]) has read it
-    PinBuf adapt_pin[3];
-    cudaEvent_t ev_adapt[3] = {};
-    bool adapt_used[3] = {false, false, false};
-    int adapt_next = 0;
+    DevBuf d_args;      // adaptive rho: GpiAdapt arguments + the shared dKinf_drho + dPinf_drho (adapt.h); rollout: GpiRoll (rollout.h)
+    // page-locked staging of d_args's contents, a ring so that the copy stays asynchronous: slot i is rewritten only once
+    // the copy three solves back (ev_args[i]) has read it
+    PinBuf args_pin[3];
+    cudaEvent_t ev_args[3] = {};
+    bool args_used[3] = {false, false, false};
+    int args_next = 0;
     cudaEvent_t ev_last = nullptr;  // recorded after the last enqueue
     cudaStream_t last_stream = nullptr;
     bool have_last = false;
@@ -184,8 +185,19 @@ size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s
 // The plan of a solve of B instances (models: per-instance models; adapt: adaptive rho).  GPI = lane groups, state
 // on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane
 // mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature cannot be served.
-int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B, SolvePlan *p) {
+int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B, SolvePlan *p, bool rollout = false) {
     const tmpc::Features ft = features(s);
+    if (rollout) {  // closed-loop rollout: the on-chip kernel's rollout variant, with the on-chip plan a solve would use
+        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts are available in STRICT mode only");
+        if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts cover box constraints only (no cones or hyperplanes)");
+        if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
+            return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run on the on-chip (GPI) kernel family only");
+        p->gpi = s->dim->gpi_plan(s->pd.dtype, s->pd.N, s->max_smem_optin);
+        if (p->gpi.smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "rollout: the horizon does not fit the on-chip kernel");
+        p->family = TINYMPC_KERNEL_GPI;
+        p->per_cta = p->gpi.instances_per_cta;
+        return 0;
+    }
     if (adapt) {  // adaptive rho: the on-chip kernel's adaptive variant, whose tables take shared memory
         if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho is available in STRICT mode only");
         if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho covers box constraints only (no cones or hyperplanes)");
@@ -247,59 +259,85 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B,
     return 0;
 }
 
-// the adaptive kernel's arguments (GpiAdapt<T>, then the shared tables) into s->d_adapt, ordered on `stream`: an asynchronous
-// copy from a page-locked staging slot (the host returns without waiting for earlier work on the stream).  Per-instance
-// tables are device arrays already: the arguments point at them and nothing follows the header.
+// `bytes` of launch arguments of an on-chip kernel variant, written by fill(host staging), into s->d_args, ordered on `stream`:
+// an asynchronous copy from a page-locked staging slot (the host returns without waiting for earlier work on the stream).
+// `what` names the variant in error messages.
+template <typename F>
+int upload_args(tinympc_b200_solver *s, size_t bytes, cudaStream_t stream, const char *what, F &&fill) {
+    if (s->d_args.bytes < bytes) {
+        if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still read the old buffer
+        if (s->d_args.ensure(bytes)) return fail(TINYMPC_ERR_CUDA, std::string(what) + " argument allocation failed");
+    }
+    const int slot = s->args_next;
+    s->args_next = (slot + 1) % 3;
+    if (!s->ev_args[slot]) CUDA_TRY(cudaEventCreateWithFlags(&s->ev_args[slot], cudaEventDisableTiming));
+    if (s->args_used[slot]) CUDA_TRY(cudaEventSynchronize(s->ev_args[slot]));  // its previous copy has been read
+    if (s->args_pin[slot].ensure(bytes)) return fail(TINYMPC_ERR_CUDA, std::string(what) + " staging allocation failed");
+    char *h = (char *)s->args_pin[slot].p;
+    std::memset(h, 0, bytes);
+    fill(h);
+    CUDA_TRY(cudaMemcpyAsync(s->d_args.p, h, bytes, cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaEventRecord(s->ev_args[slot], stream));
+    s->args_used[slot] = true;
+    return 0;
+}
+
+// the adaptive kernel's arguments (GpiAdapt<T>, then the shared tables).  Per-instance tables are device arrays already: the
+// arguments point at them and nothing follows the header.
 template <typename T>
 int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, const void *models, cudaStream_t stream) {
     const size_t nk = (size_t)s->pd.nu * s->pd.nx, np = (size_t)s->pd.nx * s->pd.nx;
     const bool per = ar->tables_per_instance != 0;
     const size_t bytes = tmpc::GPI_ADAPT_HDR + (per ? 0 : (nk + np) * sizeof(T));
-    if (s->d_adapt.bytes < bytes) {
-        if (s->have_last) CUDA_TRY(cudaEventSynchronize(s->ev_last));  // a previous solve may still read the old buffer
-        if (s->d_adapt.ensure(bytes)) return fail(TINYMPC_ERR_CUDA, "adaptive-rho argument allocation failed");
-    }
-    const int slot = s->adapt_next;
-    s->adapt_next = (slot + 1) % 3;
-    if (!s->ev_adapt[slot]) CUDA_TRY(cudaEventCreateWithFlags(&s->ev_adapt[slot], cudaEventDisableTiming));
-    if (s->adapt_used[slot]) CUDA_TRY(cudaEventSynchronize(s->ev_adapt[slot]));  // its previous copy has been read
-    if (s->adapt_pin[slot].ensure(bytes)) return fail(TINYMPC_ERR_CUDA, "adaptive-rho staging allocation failed");
-    char *h = (char *)s->adapt_pin[slot].p;
-    std::memset(h, 0, bytes);
-    tmpc::GpiAdapt<T> a{};
-    a.models = (T *)models;
-    if (per) {  // [B][nu*nx], [B][nx*nx] device arrays, read by the GPI_ADAPT_TABLES kernel variant
-        a.dK = (const T *)ar->dKinf_drho;
-        a.dP = (const T *)ar->dPinf_drho;
-    } else {
-        T *tab = (T *)(h + tmpc::GPI_ADAPT_HDR);
-        std::memcpy(tab, ar->dKinf_drho, nk * sizeof(T));
-        std::memcpy(tab + nk, ar->dPinf_drho, np * sizeof(T));
-        a.dK = (const T *)((char *)s->d_adapt.p + tmpc::GPI_ADAPT_HDR);
-        a.dP = a.dK + nk;
-    }
-    a.rho_min = (T)ar->rho_min;
-    a.rho_max = (T)ar->rho_max;
-    a.clip = ar->enable_clipping != 0;
-    const long cols = (long)s->pd.nx * s->pd.N + (long)s->pd.nu * (s->pd.N - 1);
-    a.maskA = tmpc::gemv_block_mask((long)(s->pd.nx + s->pd.nu) * (s->pd.N - 1), cols, sizeof(T));
-    a.maskP = tmpc::gemv_block_mask(cols, cols, sizeof(T));
-    static_assert(sizeof(a) <= tmpc::GPI_ADAPT_HDR, "GpiAdapt must fit its header");
-    std::memcpy(h, &a, sizeof(a));
-    CUDA_TRY(cudaMemcpyAsync(s->d_adapt.p, h, bytes, cudaMemcpyHostToDevice, stream));
-    CUDA_TRY(cudaEventRecord(s->ev_adapt[slot], stream));
-    s->adapt_used[slot] = true;
-    return 0;
+    return upload_args(s, bytes, stream, "adaptive-rho", [&](char *h) {
+        tmpc::GpiAdapt<T> a{};
+        a.models = (T *)models;
+        if (per) {  // [B][nu*nx], [B][nx*nx] device arrays, read by the GPI_ADAPT_TABLES kernel variant
+            a.dK = (const T *)ar->dKinf_drho;
+            a.dP = (const T *)ar->dPinf_drho;
+        } else {
+            T *tab = (T *)(h + tmpc::GPI_ADAPT_HDR);
+            std::memcpy(tab, ar->dKinf_drho, nk * sizeof(T));
+            std::memcpy(tab + nk, ar->dPinf_drho, np * sizeof(T));
+            a.dK = (const T *)((char *)s->d_args.p + tmpc::GPI_ADAPT_HDR);
+            a.dP = a.dK + nk;
+        }
+        a.rho_min = (T)ar->rho_min;
+        a.rho_max = (T)ar->rho_max;
+        a.clip = ar->enable_clipping != 0;
+        const long cols = (long)s->pd.nx * s->pd.N + (long)s->pd.nu * (s->pd.N - 1);
+        a.maskA = tmpc::gemv_block_mask((long)(s->pd.nx + s->pd.nu) * (s->pd.N - 1), cols, sizeof(T));
+        a.maskP = tmpc::gemv_block_mask(cols, cols, sizeof(T));
+        static_assert(sizeof(a) <= tmpc::GPI_ADAPT_HDR, "GpiAdapt must fit its header");
+        std::memcpy(h, &a, sizeof(a));
+    });
+}
+
+// the rollout kernel's arguments (GpiRoll<T>)
+template <typename T>
+int upload_rollout(tinympc_b200_solver *s, const tinympc_rollout_t *ro, cudaStream_t stream) {
+    return upload_args(s, sizeof(tmpc::GpiRoll<T>), stream, "rollout", [&](char *h) {
+        tmpc::GpiRoll<T> r{};
+        r.steps = ro->T;
+        r.reset_duals = ro->reset_duals;
+        r.w = (const T *)ro->w;
+        r.x_traj = (T *)ro->x_traj;
+        r.u_traj = (T *)ro->u_traj;
+        r.res_traj = (T *)ro->residuals_traj;
+        r.iter_traj = ro->iter_traj;
+        r.solved_traj = ro->solved_traj;
+        std::memcpy(h, &r, sizeof(r));
+    });
 }
 
 // enqueue one batched solve on `stream` (device pointers, checked by check_solve); fills stats.  io->models: the model blobs
 // the kernel reads, the per-instance models or, with ar (adaptive rho, else null), the blobs it adapts in place
 int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stream, bool timed,
-            const tinympc_adaptive_rho_t *ar = nullptr) {
+            const tinympc_adaptive_rho_t *ar = nullptr, const tinympc_rollout_t *ro = nullptr) {
     SolvePlan plan;
-    if (ar || io->B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, ar != nullptr, io->B, &plan)) return rc;
-    if (io->B <= 0) return TINYMPC_OK;
+    if (ar || ro || io->B > 0)  // an adaptive solve or a rollout is checked whole even when the batch is empty
+        if (int rc = plan_solve(s, io->models != nullptr, ar != nullptr, io->B, &plan, ro != nullptr)) return rc;
+    if (io->B <= 0 || (ro && ro->T == 0)) return TINYMPC_OK;
     const int family = plan.family;
     // The launch scratch of a handle (work queue, workspaces, timing events) is single-buffered: a solve enqueued on a
     // different stream than the previous one first waits for it.
@@ -317,7 +355,12 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
                                                 : upload_adaptive<float>(s, ar, io->models, stream))
             return rc;
         d.adapt = ar->tables_per_instance ? 2 : 1;
-        d.adapt_args = s->d_adapt.p;
+        d.adapt_args = s->d_args.p;
+    }
+    if (ro) {
+        if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_rollout<double>(s, ro, stream) : upload_rollout<float>(s, ro, stream)) return rc;
+        d.rollout = 1;
+        d.roll_args = s->d_args.p;
     }
     if (timed) CUDA_TRY(cudaEventRecord(s->ev0, stream));
     d.family = family;
@@ -334,7 +377,9 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
         CUDA_TRY(cudaMemsetAsync(s->queue.p, 0, 256, stream));
         d.work_queue = s->queue.p;
         d.gpi = plan.gpi;
-        if (family == TINYMPC_KERNEL_GPI && (io->state.v || io->state.z)) {  // previous-iteration slacks are staged in pack layout, one 16-byte store per knot point
+        // previous-iteration slacks are staged in pack layout, one 16-byte store per knot point; a rollout carries them there from
+        // one step to the next
+        if (family == TINYMPC_KERNEL_GPI && (ro ? ro->carry_v != 0 : (io->state.v || io->state.z))) {
             if (s->vscratch.ensure((size_t)io->B * plan.gpi.vscratch_per_instance + 256)) return fail(TINYMPC_ERR_CUDA, "GPI v-scratch allocation failed");
             d.gpi_vscratch = s->vscratch.p;
         }
@@ -662,7 +707,7 @@ int tinympc_b200_destroy(tinympc_b200_solver_t *s) {
     if (!s) return TINYMPC_OK;
     cudaSetDevice(s->device);
     for (int i = 0; i < 3; ++i)
-        if (s->ev_adapt[i]) cudaEventDestroy(s->ev_adapt[i]);
+        if (s->ev_args[i]) cudaEventDestroy(s->ev_args[i]);
     for (int i = 0; i < tinympc_b200_solver::SLOTS; ++i) {
         if (s->ev_in[i]) cudaEventDestroy(s->ev_in[i]);
         if (s->ev_k[i]) cudaEventDestroy(s->ev_k[i]);
@@ -716,6 +761,28 @@ int tinympc_b200_solve_adaptive(tinympc_b200_solver_t *s, const tinympc_batch_t 
     tinympc_batch_t adapted = *io;
     adapted.models = ar->models;  // the blobs the kernel adapts in place
     return enqueue(s, &adapted, (cudaStream_t)cuda_stream, true, ar);
+}
+
+int tinympc_b200_rollout(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_rollout_t *ro, void *cuda_stream) {
+    if (!s || !io || !ro) return fail(TINYMPC_ERR_ARG, "null argument");
+    if (io->Xref || io->Uref || io->iter || io->solved || io->residuals || io->u0)
+        return fail(TINYMPC_ERR_ARG, "rollout: io->Xref, Uref, iter, solved, residuals and u0 must be NULL (the references and "
+                                     "per-step outputs are trajectories in tinympc_rollout_t)");
+    if (io->state.x || io->state.u) return fail(TINYMPC_ERR_ARG, "rollout: io->state.x and state.u must be NULL");
+    if (ro->T < 0 || !ro->Xref) return fail(TINYMPC_ERR_ARG, "rollout: T must be >= 0 and Xref is required");
+    if ((ro->reset_duals != 0 && ro->reset_duals != 1) || (ro->carry_v != 0 && ro->carry_v != 1))
+        return fail(TINYMPC_ERR_ARG, "rollout: reset_duals and carry_v must be 0 or 1");
+    if (ro->reserved != 0 || ro->reserved1[0] != 0 || ro->reserved1[1] != 0) return fail(TINYMPC_ERR_ARG, "rollout: reserved fields must be 0");
+    if (!ro->carry_v && (io->state.v || io->state.z))
+        return fail(TINYMPC_ERR_ARG, "rollout: io->state.v / state.z need carry_v = 1 (without it work->v / work->z read as zeros)");
+    CUDA_TRY(cudaSetDevice(s->device));
+    tinympc_batch_t b = *io;  // the first step's window is the trajectory's start: the kernel reads the trajectories in its place
+    b.Xref = ro->Xref;
+    b.xref_per_instance = ro->xref_per_instance;
+    b.Uref = ro->Uref;
+    b.uref_per_instance = ro->uref_per_instance;
+    if (int rc = check_solve(s, &b, nullptr)) return rc;
+    return enqueue(s, &b, (cudaStream_t)cuda_stream, true, nullptr, ro);
 }
 
 namespace {

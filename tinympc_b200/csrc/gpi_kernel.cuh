@@ -24,6 +24,7 @@
 #include "common.cuh"
 #include "lanegroup.cuh"
 #include "model_blob.h"
+#include "rollout.h"
 
 namespace tmpc {
 
@@ -73,6 +74,10 @@ constexpr int GPI_ADAPT = 64;
 // its own, so that the shared-table adaptive kernel keeps its machine code (a run-time choice between the staged and the
 // per-instance tables cost it 2-3 %, DESIGN.md §5.5).
 constexpr int GPI_ADAPT_TABLES = 128;
+// Closed-loop rollout (tinympc_b200_rollout): the kernel runs GpiRoll::steps warm-started MPC steps per instance and reads its
+// GpiRoll arguments (rollout.h: gpi_roll_args).  Encoded in the lane parameter for the same reason as GPI_ADAPT; never combined
+// with it.
+constexpr int GPI_ROLLOUT = 256;
 
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
@@ -80,13 +85,17 @@ template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = fal
 __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     gpi_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
     constexpr bool ADAPT = (LA & GPI_ADAPT) != 0;       // adaptive rho
-    constexpr bool PERTAB = LA >= GPI_ADAPT_TABLES;     // ... with per-instance tables
+    constexpr bool PERTAB = (LA & GPI_ADAPT_TABLES) != 0;  // ... with per-instance tables
+    constexpr bool ROLL = (LA & GPI_ROLLOUT) != 0;        // closed-loop rollout
     constexpr int L = LA % GPI_ADAPT;
-    static_assert(LA < 2 * GPI_ADAPT_TABLES && L > 0 && (ADAPT || !PERTAB),
-                  "lane count: 4, 8 or 16, plus GPI_ADAPT (and GPI_ADAPT_TABLES) for the adaptive variants");
+    static_assert(LA < 2 * GPI_ROLLOUT && L > 0 && (ADAPT || !PERTAB) && !(ADAPT && ROLL),
+                  "lane count: 4, 8 or 16, plus GPI_ADAPT (and GPI_ADAPT_TABLES) for the adaptive variants or GPI_ROLLOUT");
     static_assert(!ADAPT || (HET && !FAST && !MM), "adaptive rho runs on heterogeneous STRICT batches");
+    static_assert(!ROLL || !FAST, "rollouts run in STRICT mode");
     GpiAdapt<T> AP{};
     if constexpr (ADAPT) AP = *gpi_adapt_args<T>(P);
+    const GpiRoll<T> *RP = nullptr;
+    if constexpr (ROLL) RP = gpi_roll_args<T>(P);
     using Cfg = GpiCfg<NX, NU, L, (int)sizeof(T)>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, PVP = Cfg::PVP, NPV = Cfg::NPV;
     constexpr int NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -311,7 +320,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     T loX[RX], hiX[RX], loU[RU], hiU[RU];  // bounds of this lane's rows (reloaded per k only if time-varying)
     box_bounds<true>(P, l, 0, true, enx, enu, xok, uok, loX, hiX, loU, hiU);
     const T kInf = (T)INFINITY;
-    const bool keep_v = (P.s_v != nullptr) || (P.s_z != nullptr);
+    bool keep_v = (P.s_v != nullptr) || (P.s_z != nullptr);
+    // ROLL: the scratch carries work->v / work->z from one step to the next, so every forward pass stages them
+    if constexpr (ROLL) keep_v = keep_v || P.gpi_vscratch != nullptr;
     // where element (k, row i) of instance-slot s lives inside a pack region
     auto idx_x = [&](int s, int k, int i) { return (k * 32 + s * L + i / RX) * PVP + (i % RX); };
     auto idx_u = [&](int s, int k, int j) { return (k * 32 + s * L + j / RU) * PVP + RX + (j % RU); };
@@ -321,6 +332,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     bool busy = false;    // the slot holds an unfinished instance
     bool want = true;     // the slot should try to fetch an instance
     int it = 0, solved = 0;
+    int tstep = 0;  // ROLL: the step of the slot's episode
     // ADAPT: an adaptation of this slot's Kinf / Pinf waiting to be applied (at the next iteration start or at retire: the
     // retire-time replay of work->x / work->u must use the Kinf of the last forward pass); the two deltas of
     // update_matrices_with_derivatives (rho_benchmark.cpp:240, admm.cpp:421)
@@ -954,6 +966,22 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             else if (P.s_z && s_solved && !(s_it == 1 && !cold)) P.s_z[ou + e] = P.gpi_vscratch[((ib * N + k) * L + j / RU) * PVP + RX + (j % RU)];
             else if (P.s_z && cold && s_it == 0) P.s_z[ou + e] = T(0);
         }
+        if constexpr (ROLL) {
+            // the rules above with "the last step started cold" per slot (only the first step of an episode can), where an
+            // untouched work->v / work->z is the previous step's, which the scratch carries (the caller's, staged at the load,
+            // before the first step); each lane rewrites the elements it wrote above
+            const bool scold = cold && __shfl_sync(0xffffffffu, tstep, s * L) == 0;
+            for (int e = lane; e < N * NX; e += 32) {
+                const int k = e / NX, i = e - k * NX;
+                if (P.s_v && !(!s_solved && s_it > 0))
+                    P.s_v[ox + e] = (scold && s_it == 0) ? T(0) : P.gpi_vscratch[((ib * N + k) * L + i / RX) * PVP + (i % RX)];
+            }
+            for (int e = lane; e < (N - 1) * NU; e += 32) {
+                const int k = e / NU, j = e - k * NU;
+                if (P.s_z && !(!s_solved && s_it > 0))
+                    P.s_z[ou + e] = (scold && s_it == 0) ? T(0) : P.gpi_vscratch[((ib * N + k) * L + j / RU) * PVP + RX + (j % RU)];
+            }
+        }
         // work->u.col(0): one rollout step from d_0 (every lane computes, the lanes of slot s store)
         if constexpr (PS) {
             if (P.u0 || P.s_x || P.s_u) load_fwd_rows(rowsrc);
@@ -1029,6 +1057,130 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         __syncwarp();
     };
 
+    // ---- ROLL: the reference window of slot s's current step (knot points tstep ... tstep+N-1 of its trajectory, whose
+    // instances are steps+N-1 knots apart) and the terminal-cost constant it implies ----
+    auto roll_window = [&](int s) {
+        if (slot == s) {
+            const int64_t kx = (int64_t)RP->steps + N - 1;
+            xrefp = P.Xref + (P.xref_pi ? inst * kx * NX : 0) + (int64_t)tstep * NX + l * RX;
+            urefp = has_uref ? P.Uref + (P.uref_pi ? inst * (kx - 1) * NU : 0) + (int64_t)tstep * NU + l * RU : P.Xref;
+            const T *pinf = P.Pinf_g;
+            if constexpr (HET) pinf = P.models + inst * (int64_t)MB.model + MB.Pinf;
+            T xr[NX];
+            const T *xl = xrefp - l * RX + (int64_t)(N - 1) * NX;
+#pragma unroll
+            for (int m = 0; m < NX; ++m) xr[m] = __ldg(xl + m);
+#pragma unroll
+            for (int a = 0; a < RX; ++a) {
+                const int ii = xv[a] ? l * RX + a : 0;
+                const T pt = terminal_cost<FAST, NX>([&](int m) { return xr[m]; }, pinf, ii);
+                pterm[a] = xv[a] ? pt : T(0);
+            }
+        }
+        __syncwarp();
+    };
+    // ---- ROLL: the end of step t of slot s (instance ib), in place of the write-back: record the step's outputs, apply
+    // u0 = -(Kinf x0) - d_0 to the plant, x0 <- (A x0 + B u0) + f (+ w), with the arithmetic of tinympc_b200_advance.  Unless
+    // that was the episode's last step, set the slot up for step t+1 with its primal / dual packs and d left where they are:
+    // duals reset if asked, padding rows cleared (a fresh load leaves them zero), work->v / work->z staged for the next first
+    // iteration as the write-back and the next load would leave them, counters reset, window moved.  Returns true when the
+    // slot keeps its instance (warp-uniform).
+    auto roll_boundary = [&](int s, int64_t ib) -> bool {
+        const int steps = RP->steps;
+        const int s_t = __shfl_sync(0xffffffffu, tstep, s * L);
+        const int s_it = __shfl_sync(0xffffffffu, it, s * L);
+        const int s_solved = __shfl_sync(0xffffffffu, solved, s * L);
+        const bool last = s_t + 1 >= steps;
+        const int64_t bt = ib * steps + s_t;
+        if (slot == s && l == 0) {
+            if (RP->iter_traj) RP->iter_traj[bt] = it;
+            if (RP->solved_traj) RP->solved_traj[bt] = solved;
+            if (RP->res_traj) {
+                T *r = RP->res_traj + 4 * bt;
+                r[0] = res_px; r[1] = res_dx; r[2] = res_pu; r[3] = res_du;
+            }
+        }
+        if constexpr (PS) load_fwd_rows(rowsrc);
+        __syncwarp();
+        T xo0[RX], Xf0[NX], t10[RX + RU], d0[RU], u0v[RU], Uf0[NU], bu0[RX];
+#pragma unroll
+        for (int a = 0; a < RX; ++a) xo0[a] = x0o[a];
+        gather_x(xo0, Xf0);
+        load_d(0, d0);
+        dots<FAST>(mS1f, Xf0, t10);
+#pragma unroll
+        for (int b = 0; b < RU; ++b) {
+            u0v[b] = (-t10[RX + b]) - d0[b];
+            if (s_it == 0) u0v[b] = T(0);  // no iteration ran: work->u of a loop state without work->u
+        }
+        gather_u(u0v, Uf0);
+        dots<FAST>(mB, Uf0, bu0);
+        T *xt = RP->x_traj;
+        const T *w = RP->w;
+        if (slot == s) {
+            const int64_t ox = (ib * (steps + 1) + s_t) * NX;
+#pragma unroll
+            for (int a = 0; a < RX; ++a) {
+                T xn = (t10[a] + bu0[a]) + vf[a];
+                if (w && xv[a]) xn = xn + w[bt * NX + l * RX + a];
+                if (xt && xv[a]) xt[ox + l * RX + a] = x0o[a];
+                x0o[a] = xv[a] ? xn : T(0);
+                if (xt && xv[a] && last) xt[ox + NX + l * RX + a] = x0o[a];
+            }
+#pragma unroll
+            for (int b = 0; b < RU; ++b)
+                if (RP->u_traj && uv[b]) RP->u_traj[bt * NU + l * RU + b] = u0v[b];
+        }
+        __syncwarp();
+        if (last) return false;
+        const bool reset = RP->reset_duals != 0;
+        // work->v / work->z of the next first iteration: vnew / znew after an unconverged step that iterated (admm.cpp:445),
+        // zeros after a cold step that did not, else what the scratch holds (the previous iteration's slacks, staged by the
+        // last forward pass, or the caller's, when no iteration overwrote them)
+        const bool stage_v = P.gpi_vscratch && !s_solved && (s_it > 0 || (cold && s_t == 0));
+        if (slot == s) {
+            if (!EXACT || reset) {
+                for (int k = 0; k < N; ++k) {
+                    T pa[PVP], pb[PVP];
+                    load_pack(aPA, k, pa);
+                    load_pb(k, pb);
+#pragma unroll
+                    for (int e = 0; e < PVP; ++e) {
+                        bool real = false;  // a state row, or an input row of a knot point with inputs
+                        if (e < RX) real = xv[e];
+                        else if (e < RX + RU) real = uv[e - RX] && k < N - 1;
+                        if (!real) pa[e] = pb[e] = T(0);
+                        if (reset) pb[e] = T(0);
+                    }
+                    store_pack(aPA, k, pa);
+                    store_pb(k, pb);
+                }
+            }
+            if (stage_v) {
+                for (int k = 0; k < N; ++k) {
+                    T pa[PVP];
+                    load_pack(aPA, k, pa);
+                    T *dst = P.gpi_vscratch + ((ib * N + k) * L + l) * PVP;
+#pragma unroll
+                    for (int c = 0; c < NPV; ++c) {
+                        using V16 = typename Vec16<T>::type;
+                        V16 v16;
+                        T *e16 = reinterpret_cast<T *>(&v16);
+#pragma unroll
+                        for (int e = 0; e < W; ++e) e16[e] = pa[c * W + e];
+                        reinterpret_cast<V16 *>(dst)[c] = v16;
+                    }
+                }
+            }
+            tstep += 1;
+            it = 0;
+            solved = 0;
+            res_px = res_dx = res_pu = res_du = T(0);
+        }
+        roll_window(s);
+        return true;
+    };
+
     // ---- persistent loop: every slot runs its own instance; a slot that terminates (converged or max_iter) is
     // written back and refilled from the global queue immediately, so no lane group waits for the slowest
     // instance of its warp (termination is per instance, admm.cpp:310-328) ----
@@ -1040,6 +1192,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             const int s = (__ffs(m) - 1) / L;
             const int64_t ib_old = __shfl_sync(0xffffffffu, inst, s * L);
             const int was_busy = __shfl_sync(0xffffffffu, (int)busy, s * L);
+            if constexpr (ROLL) {
+                if (was_busy && roll_boundary(s, ib_old)) continue;  // the slot goes on with the next step of its episode
+            }
             // the queue ticket is requested before the write-back of the finished instance so that the atomic's
             // latency hides behind it.  (Never hold a ticket in advance: a ticket prefetched by every warp keeps instances
             // hostage until a slot frees up, which can cost a whole extra wave per launch.)
@@ -1049,6 +1204,10 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             nxt = __shfl_sync(0xffffffffu, nxt, 0);
             if ((int64_t)nxt < P.B) {
                 load_slot(s, (int64_t)nxt);
+                if constexpr (ROLL) {
+                    if (slot == s) tstep = 0;
+                    roll_window(s);
+                }
             } else if (slot == s) {
                 busy = false;
                 want = false;
@@ -1123,7 +1282,8 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         __syncwarp();
 
         T rpx = T(0), rdx = T(0), rpu = T(0), rdu = T(0);
-        const bool vin = busy && (!cold) && it == 0;  // work->v / work->z come from the caller on the first iteration
+        bool vin = busy && (!cold) && it == 0;  // work->v / work->z come from the caller on the first iteration
+        if constexpr (ROLL) vin = busy && (!cold || tstep > 0) && it == 0;  // ... or from the previous step after the first
         if (keep_v || __any_sync(0xffffffffu, vin)) forward(BoolTag<true>{}, vin, rpx, rdx, rpu, rdu);
         else forward(BoolTag<false>{}, false, rpx, rdx, rpu, rdu);
         __syncwarp();

@@ -107,15 +107,23 @@ int launch_gpi(LaunchDesc *d) {
     if (L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     const bool het = d->io.models != nullptr;  // heterogeneous batch: per-instance model blobs
     if (d->adapt && (FAST || !het || !d->adapt_args)) return TINYMPC_ERR_UNSUPPORTED;  // adaptive rho: heterogeneous STRICT batches
+    if (d->rollout && (FAST || d->adapt || !d->roll_args)) return TINYMPC_ERR_UNSUPPORTED;  // rollouts: STRICT, no adaptive rho
     KParams<T, NX, NU> P;
     fill_params<T, NX, NU>(P, *d);
     if (d->adapt) set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
+    if (d->rollout) set_gpi_roll_args<T>(P, d->roll_args);  // GpiRoll<T>, uploaded by the caller (capi.cu: upload_rollout)
     const T *gmat = (const T *)d->pd->blob;
-    // STRICT: adaptive rho has its own variant; fp32 with a shared model (the headline path) clamps with min / max when no bound
-    // is a signed zero
+    // STRICT: adaptive rho and the rollout have variants of their own; fp32 with a shared model (the headline path) clamps with
+    // min / max when no bound is a signed zero
 #define TM_GPI_CASE(LL)                                                                                                  \
     if (L == LL) {                                                                                                       \
         if constexpr (!FAST) {                                                                                           \
+            if (d->rollout) {                                                                                            \
+                if (het) return launch_gpi_L<T, NX, NU, LL + GPI_ROLLOUT, false, true>(d, P, gmat);                      \
+                if constexpr (sizeof(T) == 4)                                                                            \
+                    if (d->pd->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL + GPI_ROLLOUT, false, false, true>(d, P, gmat); \
+                return launch_gpi_L<T, NX, NU, LL + GPI_ROLLOUT, false, false>(d, P, gmat);                              \
+            }                                                                                                            \
             if (d->adapt == 2) /* per-instance tables */                                                                 \
                 return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT + GPI_ADAPT_TABLES, false, true>(d, P, gmat);              \
             if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                       \

@@ -62,6 +62,10 @@ struct LaunchDesc {
     // GpiAdapt<T> (adapt.h) followed by dKinf_drho and dPinf_drho
     int adapt;  // 0: no; 1: one shared table pair; 2: per-instance tables
     const void *adapt_args;
+    // closed-loop rollout (tinympc_b200_rollout): io.Xref / io.Uref are then the reference trajectories, roll_args = device copy
+    // of GpiRoll<T> (rollout.h)
+    int rollout;
+    const void *roll_args;
 
     cudaStream_t stream;
     int sm_count;
