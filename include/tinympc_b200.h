@@ -175,11 +175,29 @@ typedef struct tinympc_batch {
     /* Heterogeneous batch (optional, SURVEY §8f-2): one model + cache per instance instead of the handle's shared one.
      * [B][tinympc_b200_model_blob_elems(nx,nu)] elements of the problem dtype, each blob =
      *   Adyn | Bdyn | fdyn | Q | R | Kinf | Pinf | Quu_inv | AmBKt | APf | BPf | rho      (column-major pieces, as in
-     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Bounds, cones, hyperplanes and settings
-     * stay shared.  Served by the lane-group kernels: the on-chip (GPI) kernel when the family is AUTO or GPI, the problem
-     * has box constraints only and the horizon fits in shared memory; otherwise (explicit GPS, cones or hyperplanes, a
-     * horizon off chip) the streamed (GPS) kernel, one instance per lane group.  TPI returns TINYMPC_ERR_UNSUPPORTED. */
+     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Cones, hyperplanes and settings stay shared;
+     * box bounds are the handle's unless the batch brings its own (bounds_per_instance below).  Served by the lane-group
+     * kernels: the on-chip (GPI) kernel when the family is AUTO or GPI, the problem has box constraints only and the
+     * horizon fits in shared memory; otherwise (explicit GPS, cones or hyperplanes, a horizon off chip) the streamed (GPS)
+     * kernel, one instance per lane group.  TPI returns TINYMPC_ERR_UNSUPPORTED. */
     const void *models;
+    /* Per-instance box bounds (optional): instance b clamps with its own x_min, x_max, u_min, u_max, as a TinySolver whose
+     * tiny_set_bound_constraints was called with them would.  Arrays of the problem dtype, selected per call by
+     * bounds_per_instance:
+     *   0: the handle's bounds (the pointers are ignored; what every zero-initialised batch gets);
+     *   1: x_min / x_max [B][nx], u_min / u_max [B][nu]: one column per instance, the same at every knot point;
+     *   2: x_min / x_max [B][N][nx], u_min / u_max [B][N-1][nu]: the full nx x N / nu x (N-1) matrices per instance
+     *      (the layout of a per-instance Xref / Uref).
+     * With 1 or 2 they replace the handle's bounds on both sides, and the handle needs no bounds of its own.  A side the
+     * settings enable (en_state_bound, en_input_bound) needs both pointers of its pair (else TINYMPC_ERR_NO_BOUNDS); a pair
+     * for a disabled side is never read.  One pointer of a pair without the other, any other mode value or a non-zero
+     * reserved2 return TINYMPC_ERR_ARG.  DEVICE pointers for tinympc_b200_solve, HOST pointers (staged per chunk) for
+     * tinympc_b200_solve_host.  Routed like `models` (lane-group kernels only; explicit TPI returns
+     * TINYMPC_ERR_UNSUPPORTED) and STRICT only: FAST mode, adaptive rho and rollouts return TINYMPC_ERR_UNSUPPORTED. */
+    const void *x_min, *x_max; /* per-instance state bounds (see bounds_per_instance), or NULL */
+    const void *u_min, *u_max; /* per-instance input bounds, or NULL                         */
+    int32_t bounds_per_instance; /* 0: the handle's bounds; 1: one column per instance; 2: full horizon per instance */
+    int32_t reserved2;           /* must be 0 */
 } tinympc_batch_t;
 
 typedef struct tinympc_b200_solver tinympc_b200_solver_t;

@@ -69,6 +69,8 @@ class Batch(C.Structure):
         ("iter", vp), ("solved", vp), ("residuals", vp),
         ("u0", vp),
         ("models", vp),
+        ("x_min", vp), ("x_max", vp), ("u_min", vp), ("u_max", vp),
+        ("bounds_per_instance", C.c_int32), ("reserved2", C.c_int32),
     ]
 
 

@@ -11,11 +11,49 @@ from . import abi
 from .problem import MPCProblem
 
 
+BOUND_NAMES = ("x_min", "x_max", "u_min", "u_max")
+
+
+def bounds_layout(bounds: dict, B: int, N: int, nx: int, nu: int, dtype) -> int:
+    """Check per-instance box bounds (a dict with any of x_min, x_max, u_min, u_max; numpy arrays or torch tensors) against a
+    batch of B instances and return their layout (tinympc_batch_t.bounds_per_instance): 1 for [B, nx] / [B, nu] (one column
+    per instance), 2 for [B, N, nx] / [B, N-1, nu] (a horizon per instance).  A side may be absent when its bound is
+    disabled; min and max of a side come together."""
+    unknown = set(bounds) - set(BOUND_NAMES)
+    if unknown:
+        raise ValueError(f"bounds: unknown keys {sorted(unknown)}; expected any of {BOUND_NAMES}")
+    given = {k: v for k, v in bounds.items() if v is not None}
+    for lo, hi in (("x_min", "x_max"), ("u_min", "u_max")):
+        if (lo in given) != (hi in given):
+            raise ValueError(f"bounds: {lo} and {hi} are given together")
+    if not given:
+        raise ValueError("bounds: give x_min / x_max, u_min / u_max or both")
+    want = np.dtype(dtype)
+    layouts = set()
+    for k, a in given.items():
+        dt = a.dtype if hasattr(a, "dtype") else None
+        ok_dt = (str(dt).replace("torch.", "") == want.name) if dt is not None else False
+        if not ok_dt:
+            raise ValueError(f"bounds: {k} must have the problem dtype {want.name}, got {dt}")
+        w, kn = (nx, N) if k[0] == "x" else (nu, N - 1)
+        shape = tuple(a.shape)
+        if shape == (B, w):
+            layouts.add(1)
+        elif shape == (B, kn, w):
+            layouts.add(2)
+        else:
+            raise ValueError(f"bounds: {k} must be [{B}, {w}] (one column per instance) or [{B}, {kn}, {w}] (a horizon per "
+                             f"instance), got {list(shape)}")
+    if len(layouts) != 1:
+        raise ValueError("bounds: every array takes the same layout ([B, n] or [B, N, n])")
+    return layouts.pop()
+
+
 class HostBatch:
     """Owns the numpy buffers of one batched solve and the ctypes struct pointing at them."""
 
     def __init__(self, prob: MPCProblem, x0, Xref, Uref=None, state: dict | None = None, cold_start=True,
-                 want_state=(), want_residuals=True, models=None):
+                 want_state=(), want_residuals=True, models=None, bounds: dict | None = None):
         dt = prob.dtype
         nx, nu, N = prob.nx, prob.nu, prob.N
         self.prob = prob
@@ -45,6 +83,11 @@ class HostBatch:
                 self.state[name] = np.zeros(shape, dtype=dt)
         self.cold_start = bool(cold_start)
         self.models = None if models is None else np.ascontiguousarray(models, dtype=dt).reshape(B, -1)
+        # per-instance box bounds (see bounds_layout); bounds_per_instance 0 = the problem's
+        self.bounds_per_instance, self.bounds = 0, {}
+        if bounds is not None:
+            self.bounds_per_instance = bounds_layout(bounds, B, N, nx, nu, dt)
+            self.bounds = {k: np.ascontiguousarray(v) for k, v in bounds.items() if v is not None}
         self.sol_x = np.zeros((B, N, nx), dtype=dt)
         self.sol_u = np.zeros((B, N - 1, nu), dtype=dt)
         self.iter = np.zeros(B, dtype=np.int32)
@@ -68,6 +111,9 @@ class HostBatch:
         b.solved = self.solved.ctypes.data
         b.residuals = None if self.residuals is None else self.residuals.ctypes.data
         b.models = None if self.models is None else self.models.ctypes.data
+        b.bounds_per_instance = self.bounds_per_instance
+        for k, a in self.bounds.items():
+            setattr(b, k, a.ctypes.data)
         b._owner = self
         return b
 

@@ -159,8 +159,19 @@ tmpc::Features features(const tinympc_b200_solver *s) {
 // order decides which error a caller sees.
 int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
     const tinympc_settings_t &st = s->settings;
-    if ((st.en_state_bound && !s->pd.x_min) || (st.en_input_bound && !s->pd.u_min))
-        return fail(TINYMPC_ERR_NO_BOUNDS, "en_state_bound/en_input_bound set but bounds were never provided");
+    const int bpi = io->bounds_per_instance;
+    if (bpi < 0 || bpi > 2 || io->reserved2 != 0)
+        return fail(TINYMPC_ERR_ARG, "bounds_per_instance must be 0 (the handle's bounds), 1 (one column per instance) or 2 "
+                                     "(a horizon per instance), and reserved2 must be 0");
+    if (bpi == 0) {
+        if ((st.en_state_bound && !s->pd.x_min) || (st.en_input_bound && !s->pd.u_min))
+            return fail(TINYMPC_ERR_NO_BOUNDS, "en_state_bound/en_input_bound set but bounds were never provided");
+    } else {  // the batch's bounds replace the handle's
+        if (!io->x_min != !io->x_max || !io->u_min != !io->u_max)
+            return fail(TINYMPC_ERR_ARG, "per-instance bounds: x_min / x_max and u_min / u_max are given in pairs");
+        if ((st.en_state_bound && !io->x_min) || (st.en_input_bound && !io->u_min))
+            return fail(TINYMPC_ERR_NO_BOUNDS, "per-instance bounds: en_state_bound/en_input_bound set but the batch has no x_min/x_max or u_min/u_max");
+    }
     if (st.check_termination <= 0) return fail(TINYMPC_ERR_ARG, "check_termination must be >= 1");
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     if (ar && io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
@@ -182,11 +193,17 @@ struct SolvePlan {
 // shared memory the adaptive kernel adds per CTA for its tables
 size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->pd.nx, s->pd.nu, esize(s->pd.dtype)); }
 
-// The plan of a solve of B instances (models: per-instance models; adapt: adaptive rho).  GPI = lane groups, state
-// on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane
-// mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature cannot be served.
-int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B, SolvePlan *p, bool rollout = false) {
+// The plan of a solve of B instances (models: per-instance models; bounds: per-instance box bounds; adapt: adaptive rho).
+// GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed
+// (everything else the lane mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature
+// cannot be served.
+int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool adapt, int64_t B, SolvePlan *p, bool rollout = false) {
     const tmpc::Features ft = features(s);
+    if (bounds) {  // per-instance bounds have STRICT solve variants only
+        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's bounds (bounds_per_instance must be 0)");
+        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's bounds (bounds_per_instance must be 0)");
+        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance bounds are available in STRICT mode only");
+    }
     if (rollout) {  // closed-loop rollout: the on-chip kernel's rollout variant, with the on-chip plan a solve would use
         if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts are available in STRICT mode only");
         if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts cover box constraints only (no cones or hyperplanes)");
@@ -240,17 +257,18 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool adapt, int64_t B,
         p->family = (!gpi_ok || (ipc > 0 && few && !tpi_heavy && big_batch)) ? streamed : TINYMPC_KERNEL_GPI;
     }
     if (p->family == TINYMPC_KERNEL_GPI) p->per_cta = p->gpi.instances_per_cta;
-    // Per-instance models: the on-chip kernel, exactly as without models, when the family is AUTO or GPI and the problem has
-    // box constraints only and an on-chip plan (per_cta is left as the rules above set it: the host path rounds such chunks
-    // by the family a shared model would get).  Otherwise the streamed kernel's per-instance-model variant: explicit GPS,
-    // cones or hyperplanes, or a horizon that does not fit on chip.  One thread per instance has no such variant.
-    if (models) {
+    // Per-instance data (models, bounds or both): the on-chip kernel, exactly as without them, when the family is AUTO or GPI
+    // and the problem has box constraints only and an on-chip plan (per_cta is left as the rules above set it: the host path
+    // rounds such chunks by the family a shared model would get).  Otherwise the streamed kernel's one-instance-per-lane-group
+    // variant: explicit GPS, cones or hyperplanes, or a horizon that does not fit on chip.  One thread per instance has no
+    // such variant.
+    if (models || bounds) {
         if (s->family == TINYMPC_KERNEL_TPI)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models run on the lane-group kernel families (GPI, GPS), not on one thread per instance");
+            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models and bounds run on the lane-group kernel families (GPI, GPS), not on one thread per instance");
         if (s->family != TINYMPC_KERNEL_GPS && !ft.ext && gpi_ok) {
             p->family = TINYMPC_KERNEL_GPI;
         } else {
-            if (!gps_ok) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models: this problem needs the streamed lane-group kernel, which does not cover this shape");
+            if (!gps_ok) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models / bounds: this problem needs the streamed lane-group kernel, which does not cover this shape");
             p->family = TINYMPC_KERNEL_GPS;
             p->per_cta = s->dim->gps_het_slots(s->pd.dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, s->max_smem_optin);
         }
@@ -336,7 +354,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
             const tinympc_adaptive_rho_t *ar = nullptr, const tinympc_rollout_t *ro = nullptr) {
     SolvePlan plan;
     if (ar || ro || io->B > 0)  // an adaptive solve or a rollout is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, ar != nullptr, io->B, &plan, ro != nullptr)) return rc;
+        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, ar != nullptr, io->B, &plan, ro != nullptr)) return rc;
     if (io->B <= 0 || (ro && ro->T == 0)) return TINYMPC_OK;
     const int family = plan.family;
     // The launch scratch of a handle (work queue, workspaces, timing events) is single-buffered: a solve enqueued on a
@@ -350,6 +368,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     d.fast = s->mode == TINYMPC_MODE_FAST;
     d.sm_count = s->sm_count;
     d.max_smem_optin = s->max_smem_optin;
+    d.bounds = io->bounds_per_instance;
     if (ar) {
         if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, io->models, stream)
                                                 : upload_adaptive<float>(s, ar, io->models, stream))
@@ -872,7 +891,7 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     chunk = (chunk + 31) / 32 * 32;
     SolvePlan plan;  // of a chunk
     if (ar || B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, ar != nullptr, chunk, &plan)) return rc;
+        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, ar != nullptr, chunk, &plan)) return rc;
     if (B <= 0) return TINYMPC_OK;
     const size_t es = esize(s->pd.dtype);
     const size_t bx = es * s->pd.nx * s->pd.N, bu = es * s->pd.nu * (s->pd.N - 1);
@@ -904,6 +923,21 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     if (io->models) fields.push_back({io->models, nullptr, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, false, (void **)&dev.models});
     // adaptive rho: the model blobs are in/out; they travel in dev.models (io->models is NULL), where the kernel adapts them
     if (ar) fields.push_back({ar->models, ar->models, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, true, (void **)&dev.models});
+    if (io->bounds_per_instance) {  // sliced per chunk like the models; a disabled side is never read
+        const size_t kx = io->bounds_per_instance == 2 ? s->pd.N : 1, ku = io->bounds_per_instance == 2 ? s->pd.N - 1 : 1;
+        if (s->settings.en_state_bound) {
+            fields.push_back({io->x_min, nullptr, es * s->pd.nx * kx, true, false, (void **)&dev.x_min});
+            fields.push_back({io->x_max, nullptr, es * s->pd.nx * kx, true, false, (void **)&dev.x_max});
+        } else {
+            dev.x_min = dev.x_max = nullptr;
+        }
+        if (s->settings.en_input_bound) {
+            fields.push_back({io->u_min, nullptr, es * s->pd.nu * ku, true, false, (void **)&dev.u_min});
+            fields.push_back({io->u_max, nullptr, es * s->pd.nu * ku, true, false, (void **)&dev.u_max});
+        } else {
+            dev.u_min = dev.u_max = nullptr;
+        }
+    }
     if (ar && ar->tables_per_instance) {  // sliced per chunk like the models
         fields.push_back({ar->dKinf_drho, nullptr, es * s->pd.nu * s->pd.nx, true, false, (void **)&args.ar.dKinf_drho});
         fields.push_back({ar->dPinf_drho, nullptr, es * s->pd.nx * s->pd.nx, true, false, (void **)&args.ar.dPinf_drho});

@@ -78,6 +78,11 @@ constexpr int GPI_ADAPT_TABLES = 128;
 // GpiRoll arguments (rollout.h: gpi_roll_args).  Encoded in the lane parameter for the same reason as GPI_ADAPT; never combined
 // with it.
 constexpr int GPI_ROLLOUT = 256;
+// Per-instance box bounds (tinympc_batch_t.bounds_per_instance): P.x_min ... u_max point at the batch's [B][nx] / [B][nu] columns
+// (P.bounds_tv == 0) or [B][N][nx] / [B][N-1][nu] horizons (P.bounds_tv == 1), and every slot loads its instance's column 0 when it
+// is refilled.  Encoded in the lane parameter for the same reason as GPI_ADAPT; STRICT only, never with MM, GPI_ADAPT or
+// GPI_ROLLOUT (the host cannot tell whether a per-instance bound is a signed zero, so the clamp stays compare-select).
+constexpr int GPI_BOUNDS = 512;
 
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
@@ -87,11 +92,13 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     constexpr bool ADAPT = (LA & GPI_ADAPT) != 0;       // adaptive rho
     constexpr bool PERTAB = (LA & GPI_ADAPT_TABLES) != 0;  // ... with per-instance tables
     constexpr bool ROLL = (LA & GPI_ROLLOUT) != 0;        // closed-loop rollout
+    constexpr bool BND = (LA & GPI_BOUNDS) != 0;          // per-instance box bounds
     constexpr int L = LA % GPI_ADAPT;
-    static_assert(LA < 2 * GPI_ROLLOUT && L > 0 && (ADAPT || !PERTAB) && !(ADAPT && ROLL),
-                  "lane count: 4, 8 or 16, plus GPI_ADAPT (and GPI_ADAPT_TABLES) for the adaptive variants or GPI_ROLLOUT");
+    static_assert(LA < 2 * GPI_BOUNDS && L > 0 && (ADAPT || !PERTAB) && !(ADAPT && ROLL),
+                  "lane count: 4, 8 or 16, plus GPI_ADAPT (and GPI_ADAPT_TABLES) for the adaptive variants, GPI_ROLLOUT or GPI_BOUNDS");
     static_assert(!ADAPT || (HET && !FAST && !MM), "adaptive rho runs on heterogeneous STRICT batches");
     static_assert(!ROLL || !FAST, "rollouts run in STRICT mode");
+    static_assert(!BND || (!FAST && !MM && !ADAPT && !ROLL), "per-instance bounds run in STRICT mode, alone");
     GpiAdapt<T> AP{};
     if constexpr (ADAPT) AP = *gpi_adapt_args<T>(P);
     const GpiRoll<T> *RP = nullptr;
@@ -405,7 +412,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 na[e] = pa[e];
                 nb[e] = pb[e];
             }
-            if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            if constexpr (!BND) {  // per-instance horizons are loaded at the top of the step (bounds_at below)
+                if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            }
             if constexpr (FAST) {
     #pragma unroll
                 for (int a = 0; a < RX; ++a) {  // vnew = clamp(x + g), g += x - vnew
@@ -523,8 +532,17 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 }
             }
         };
+        // BND, layout 2: column k of the slot's instance (laid out like Xref / Uref; a slot without an instance reads instance
+        // 0), issued at the top of step k so that its latency hides behind the step's mat-vec and gathers
+        auto bounds_at = [&](int k, const bool HASU) {
+            if constexpr (BND) {
+                const int64_t bi = inst < 0 ? 0 : inst;
+                if (tvb) box_bounds_at<false>(P, bi * N * NX, bi * (N - 1) * NU, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            }
+        };
         for (int k = 0; k < N - 1; ++k) {
             T u[RU], Uf[NU], t1[RX + RU], bu[RX], vprev[PVP], pbk[PVP], dk[RU];
+            bounds_at(k, true);
             load_vprev(k, vprev);
             load_pb(k, pbk);
             load_d(k, dk);
@@ -547,6 +565,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             T udummy[RU], vprev[PVP], pbk[PVP];
 #pragma unroll
             for (int b = 0; b < RU; ++b) udummy[b] = T(0);
+            bounds_at(N - 1, false);
             load_vprev(N - 1, vprev);
             load_pb(N - 1, pbk);
             column(N - 1, false, udummy, vprev, pbk);
@@ -691,6 +710,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             offu = ib * (int64_t)(N - 1) * NU;
             xrefp = P.Xref + (P.xref_pi ? offx : 0) + l * RX;
             urefp = has_uref ? P.Uref + (P.uref_pi ? offu : 0) + l * RU : P.Xref;
+            // per-instance bounds: column 0 of this instance (one column per instance, or its horizon)
+            if constexpr (BND)
+                box_bounds_at<true>(P, tvb ? offx : ib * NX, tvb ? offu : ib * NU, l, 0, true, enx, enu, xok, uok, loX, hiX, loU, hiU);
             // heterogeneous batch: this instance has its own model / cache blob (same layout as the shared one, rho appended)
             const T *pinf = P.Pinf_g;
             if constexpr (HET) {

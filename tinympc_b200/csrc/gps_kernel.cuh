@@ -199,13 +199,21 @@ __device__ __forceinline__ void stg_piece(T *p, const T (&v)[R], unsigned pr) {
 // staged copy.  It runs one instance per lane group: the NI = 2 variant shares the matrix registers between the two
 // instances of a group, and two sets of rows do not fit.
 constexpr int GPS_HET = 8;
+// Per-instance box bounds (tinympc_batch_t.bounds_per_instance): GPS_BOUNDS added to the family mask.  P.x_min ... u_max point at
+// the batch's [B][nx] / [B][nu] columns (P.bounds_tv == 0) or [B][N][nx] / [B][N-1][nu] horizons (P.bounds_tv == 1); a slot loads
+// its instance's column 0 when it is loaded.  One instance per lane group, as GPS_HET: the bound registers are per lane, and
+// two instances with bounds of their own do not fit the NI = 2 budget.
+constexpr int GPS_BOUNDS = 16;
+constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS;  // the family-mask bits that are not constraint families
 
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     gps_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
-    constexpr bool HET = (FAMH & GPS_HET) != 0;  // per-instance models
-    constexpr int FAM = FAMH & ~GPS_HET;         // constraint families compiled in
+    constexpr bool HET = (FAMH & GPS_HET) != 0;     // per-instance models
+    constexpr bool BND = (FAMH & GPS_BOUNDS) != 0;  // per-instance box bounds
+    constexpr int FAM = FAMH & ~GPS_VARIANTS;       // constraint families compiled in
     static_assert(!HET || NI == 1, "per-instance models run one instance per lane group");
+    static_assert(!BND || (NI == 1 && !FAST), "per-instance bounds run one instance per lane group, in STRICT mode");
     using Cfg = GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAM>;
     using REC = GpsRec<NX, NU, Cfg::SPW, (int)sizeof(T), FAM>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -622,7 +630,12 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                     for (int b = 0; b < RU; ++b) u[j][b] = (-t1[j][RX + b]) - dk[j][b];  // u_k = -(Kinf x_k) - d_k
                 gather_u(u, Uf);
             }
-            if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            if constexpr (BND) {  // per-instance horizons are laid out like Xref / Uref; a slot without an instance reads instance 0
+                const int64_t bi = inst[0] < 0 ? 0 : inst[0];
+                if (tvb) box_bounds_at<false>(P, bi * N * NX, bi * (N - 1) * NU, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            } else {
+                if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            }
             // ---- box constraints: state column k and input column k ----
             T q[NI][RX], r[NI][RU];
 #pragma unroll
@@ -888,6 +901,9 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                 rho_h = rho_l;
                 mrow = mbl;
             }
+            // per-instance bounds: column 0 of this instance (one column per instance, or its horizon)
+            if constexpr (BND)
+                box_bounds_at<true>(P, tvb ? ox : ib * NX, tvb ? ou : ib * NU, l, 0, true, enx, enu, xok, uok, loX, hiX, loU, hiU);
             const T *xl = xrefb + (int64_t)(N - 1) * NX;
             T x0v[RX], ptv[RX];
 #pragma unroll
@@ -1145,10 +1161,10 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     return p;
 }
 
-// FAMH: family mask, plus GPS_HET for per-instance models
+// FAMH: family mask, plus GPS_HET for per-instance models and GPS_BOUNDS for per-instance bounds
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
-    const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH & ~GPS_HET>(*d);
+    const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH & ~GPS_VARIANTS>(*d);
     if (plan.L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     d->out_ws_need = plan.ws_bytes;
     if (!d->gps_ws || d->gps_ws_bytes < plan.ws_bytes) return TM_ERR_WORKSPACE;
@@ -1172,6 +1188,24 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     } else {
         constexpr int NI = gps_pick_NI<T, NX, NU, L>();
         const int fam = gps_family_mask(d->ft.soc_x || d->ft.soc_u, d->ft.lin_x || d->ft.lin_u || d->ft.tvl_x || d->ft.tvl_u);
+        if (d->bounds) {  // per-instance bounds (STRICT): one instance per lane group, with or without per-instance models
+            if constexpr (FAST) {
+                return TINYMPC_ERR_UNSUPPORTED;
+            } else {
+                const bool het = d->io.models != nullptr;
+#define TM_GPS_BND_CASE(FF)                                                                       \
+    if (fam == FF) {                                                                              \
+        if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_BOUNDS | GPS_HET, false>(d, P0); \
+        return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_BOUNDS, false>(d, P0);                    \
+    }
+                TM_GPS_BND_CASE(0)
+                TM_GPS_BND_CASE(1)
+                TM_GPS_BND_CASE(6)
+                TM_GPS_BND_CASE(7)
+#undef TM_GPS_BND_CASE
+                return TINYMPC_ERR_UNSUPPORTED;
+            }
+        }
         if (d->io.models) {  // per-instance models: one instance per lane group, the same family variants
 #define TM_GPS_HET_CASE(FF) \
     if (fam == FF) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_HET, FAST>(d, P0);
@@ -1193,8 +1227,8 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     }
 }
 
-// instances one CTA of the per-instance-model variant holds when the batch fills every SM (the host path rounds its chunks to
-// whole waves of these); 0 = shape not available
+// instances one CTA of the one-instance-per-lane-group variants (per-instance models, per-instance bounds, or both) holds when the
+// batch fills every SM (the host path rounds its chunks to whole waves of these); 0 = shape not available
 template <typename T, int NX, int NU>
 int gps_het_slots(int fam, int max_smem_optin) {
     constexpr int L = gps_pick_L<T, NX, NU>();

@@ -47,7 +47,7 @@ int launch_tpi(LaunchDesc *d) {
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->io.models) return TINYMPC_ERR_UNSUPPORTED;  // per-instance models: the lane-group kernels only
+    if (d->io.models || d->bounds) return TINYMPC_ERR_UNSUPPORTED;  // per-instance models and bounds: the lane-group kernels only
     if (d->ft.ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
     return d->fast ? launch_tpi<T, true, false>(d) : launch_tpi<T, false, false>(d);
 }
@@ -108,13 +108,14 @@ int launch_gpi(LaunchDesc *d) {
     const bool het = d->io.models != nullptr;  // heterogeneous batch: per-instance model blobs
     if (d->adapt && (FAST || !het || !d->adapt_args)) return TINYMPC_ERR_UNSUPPORTED;  // adaptive rho: heterogeneous STRICT batches
     if (d->rollout && (FAST || d->adapt || !d->roll_args)) return TINYMPC_ERR_UNSUPPORTED;  // rollouts: STRICT, no adaptive rho
+    if (d->bounds && (FAST || d->adapt || d->rollout)) return TINYMPC_ERR_UNSUPPORTED;  // per-instance bounds: STRICT solves
     KParams<T, NX, NU> P;
     fill_params<T, NX, NU>(P, *d);
     if (d->adapt) set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
     if (d->rollout) set_gpi_roll_args<T>(P, d->roll_args);  // GpiRoll<T>, uploaded by the caller (capi.cu: upload_rollout)
     const T *gmat = (const T *)d->pd->blob;
-    // STRICT: adaptive rho and the rollout have variants of their own; fp32 with a shared model (the headline path) clamps with
-    // min / max when no bound is a signed zero
+    // STRICT: adaptive rho, the rollout and per-instance bounds have variants of their own; fp32 with a shared model (the
+    // headline path) clamps with min / max when no bound of the problem is a signed zero
 #define TM_GPI_CASE(LL)                                                                                                  \
     if (L == LL) {                                                                                                       \
         if constexpr (!FAST) {                                                                                           \
@@ -127,6 +128,9 @@ int launch_gpi(LaunchDesc *d) {
             if (d->adapt == 2) /* per-instance tables */                                                                 \
                 return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT + GPI_ADAPT_TABLES, false, true>(d, P, gmat);              \
             if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                       \
+            if (d->bounds) /* before MM: the host cannot scan per-instance bounds for signed zeros */                   \
+                return het ? launch_gpi_L<T, NX, NU, LL + GPI_BOUNDS, false, true>(d, P, gmat)                           \
+                           : launch_gpi_L<T, NX, NU, LL + GPI_BOUNDS, false, false>(d, P, gmat);                         \
             if constexpr (sizeof(T) == 4)                                                                                \
                 if (!het && d->pd->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, false, false, true>(d, P, gmat); \
         }                                                                                                                \

@@ -92,6 +92,10 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
     P.uref_pi = io.uref_per_instance;
     P.x0 = (const T *)io.x0; P.Xref = (const T *)io.Xref; P.Uref = (const T *)io.Uref;
     P.x_min = (const T *)pd.x_min; P.x_max = (const T *)pd.x_max; P.u_min = (const T *)pd.u_min; P.u_max = (const T *)pd.u_max;
+    if (d.bounds) {  // per-instance bounds replace the problem's; the kernels derive an instance's offset from NX, NU, N and bounds_tv
+        P.x_min = (const T *)io.x_min; P.x_max = (const T *)io.x_max; P.u_min = (const T *)io.u_min; P.u_max = (const T *)io.u_max;
+        P.bounds_tv = d.bounds == 2;
+    }
     P.Alin_x = (const T *)pd.Alin_x; P.blin_x = (const T *)pd.blin_x; P.Alin_u = (const T *)pd.Alin_u; P.blin_u = (const T *)pd.blin_u;
     P.tv_Alin_x = (const T *)pd.tv_Alin_x; P.tv_blin_x = (const T *)pd.tv_blin_x;
     P.tv_Alin_u = (const T *)pd.tv_Alin_u; P.tv_blin_u = (const T *)pd.tv_blin_u;

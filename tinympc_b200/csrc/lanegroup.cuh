@@ -183,6 +183,27 @@ __device__ __forceinline__ void box_bounds(const KParams<T, NX, NU> &P, int l, i
         }
     }
 }
+// the same for per-instance bounds (tinympc_batch_t.bounds_per_instance): column k of the instance whose columns start at
+// element ox of the state bounds and ou of the input bounds (k = 0 for INIT)
+template <bool INIT, typename T, int NX, int NU, int RX, int RU, typename XV, typename UV>
+__device__ __forceinline__ void box_bounds_at(const KParams<T, NX, NU> &P, int64_t ox, int64_t ou, int l, int k, const bool HASU,
+                                              const bool enx, const bool enu, XV xv, UV uv, T (&loX)[RX], T (&hiX)[RX], T (&loU)[RU],
+                                              T (&hiU)[RU]) {
+    const T kInf = (T)INFINITY;
+    const int64_t bx = ox + (int64_t)k * NX + l * RX, bu = ou + (int64_t)k * NU + l * RU;
+#pragma unroll
+    for (int a = 0; a < RX; ++a) {
+        loX[a] = (enx && xv(a)) ? __ldg(P.x_min + bx + a) : (INIT ? -kInf : loX[a]);
+        hiX[a] = (enx && xv(a)) ? __ldg(P.x_max + bx + a) : (INIT ? kInf : hiX[a]);
+    }
+    if (INIT || HASU) {
+#pragma unroll
+        for (int b = 0; b < RU; ++b) {
+            loU[b] = (enu && uv(b)) ? __ldg(P.u_min + bu + b) : (INIT ? -kInf : loU[b]);
+            hiU[b] = (enu && uv(b)) ? __ldg(P.u_max + bu + b) : (INIT ? kInf : hiU[b]);
+        }
+    }
+}
 
 template <typename T, int L>
 __device__ __forceinline__ T group_max(T v) {

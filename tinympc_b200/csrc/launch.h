@@ -66,6 +66,9 @@ struct LaunchDesc {
     // of GpiRoll<T> (rollout.h)
     int rollout;
     const void *roll_args;
+    // per-instance box bounds (io.bounds_per_instance): 0 = the problem's; 1 = io.x_min ... u_max hold one column per instance;
+    // 2 = they hold a horizon per instance.  The lane-group kernels' GPI_BOUNDS / GPS_BOUNDS variants read them.
+    int bounds;
 
     cudaStream_t stream;
     int sm_count;

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import abi
 from ._lib import check, load
-from .batch import HostBatch
+from .batch import BOUND_NAMES, HostBatch, bounds_layout
 from .problem import MPCProblem, copy_settings, default_settings, dtype_code
 from .workloads import ModelSpec
 
@@ -219,15 +219,19 @@ class BatchedTinySolver:
 
     # ---- host buffers (numpy): the call a reference user would make; H2D/D2H inside ------------------
     def solve(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), models=None,
-              adaptive_rho: AdaptiveRho | None = None) -> dict:
+              adaptive_rho: AdaptiveRho | None = None, bounds: dict | None = None) -> dict:
         """With adaptive_rho: every instance adapts its own rho / Kinf / Pinf, starting from its blob in `models` (default:
-        the problem's own cache, pack_models); the result's "models" holds the adapted blobs, the start of the next solve."""
+        the problem's own cache, pack_models); the result's "models" holds the adapted blobs, the start of the next solve.
+        bounds: per-instance box bounds in place of the problem's, a dict with any of x_min, x_max, u_min, u_max of the
+        problem dtype: [B, nx] / [B, nu] (one column per instance) or [B, N, nx] / [B, N-1, nu] (a horizon per instance);
+        a side may be absent when its bound is disabled (tinympc_batch_t.bounds_per_instance)."""
         if adaptive_rho is None:
-            hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, models=models)
+            hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, models=models,
+                           bounds=bounds)
             cb = hb.to_c()
             check(self._lib.tinympc_b200_solve_host(self._h, C.byref(cb)))
             return hb.result()
-        hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state)
+        hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, bounds=bounds)
         m = pack_models(self.problem, hb.B) if models is None else np.array(models, dtype=self.problem.dtype).reshape(hb.B, -1)
         cb, ar = hb.to_c(), adaptive_rho.to_c(self.problem, m.ctypes.data, hb.B)
         check(self._lib.tinympc_b200_solve_adaptive_host(self._h, C.byref(cb), C.byref(ar)))
@@ -293,8 +297,9 @@ class BatchedTinySolver:
 
     # ---- device buffers (torch tensors on cuda:<device>) ---------------------------------------------
     def make_device_batch(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), want_residuals=True,
-                          want_u0=False, want_solution=True, models=None):
-        """Allocate/adopt torch CUDA tensors and build the device-pointer tinympc_batch_t."""
+                          want_u0=False, want_solution=True, models=None, bounds: dict | None = None):
+        """Allocate/adopt torch CUDA tensors and build the device-pointer tinympc_batch_t.  bounds: per-instance box bounds as
+        in solve(); torch CUDA tensors of the problem dtype are used in place, numpy arrays are uploaded."""
         import torch
 
         p = self.problem
@@ -343,6 +348,12 @@ class BatchedTinySolver:
         models_t = None if models is None else t(models)
         tens["models"] = models_t
         b.models = None if models_t is None else models_t.data_ptr()
+        if bounds is not None:
+            b.bounds_per_instance = bounds_layout(bounds, B, p.N, p.nx, p.nu, p.dtype)
+            bt = {k: t(v) for k, v in bounds.items() if v is not None}
+            for k in BOUND_NAMES:
+                setattr(b, k, bt[k].data_ptr() if k in bt else None)
+            tens["bounds"] = bt
         b.iter, b.solved = out["iter"].data_ptr(), out["solved"].data_ptr()
         b.residuals = None if out["residuals"] is None else out["residuals"].data_ptr()
         res = dict(out)
