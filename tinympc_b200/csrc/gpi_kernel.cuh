@@ -143,11 +143,15 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // `src` = a cache blob in the layout above (the staged shared-memory copy, or one instance's blob in global memory).
     // Backward-sweep rows (AmBKt, B^T, Kinf^T, Quu_inv, APf, BPf and the cost weights Qd, Rd) and forward-sweep rows (A, Kinf,
     // B, f) load separately: fp64 re-reads the rows of a sweep when it starts (PS), everything else loads both once.
-    auto load_bwd_rows = [&](const T *src) {
-        auto rd = [src](int e) {
+    // blob_rd(src) reads element e of `src`; ADAPT with ld.global.cg (the blobs are rewritten during the launch)
+    auto blob_rd = [](const T *src) {
+        return [src](int e) {
             if constexpr (ADAPT) return __ldcg(src + e);
             else return src[e];
         };
+    };
+    auto load_bwd_rows = [&](const T *src) {
+        const auto rd = blob_rd(src);
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
@@ -166,10 +170,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         }
     };
     auto load_fwd_rows = [&](const T *src) {
-        auto rd = [src](int e) {
-            if constexpr (ADAPT) return __ldcg(src + e);
-            else return src[e];
-        };
+        const auto rd = blob_rd(src);
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
@@ -186,10 +187,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // both sets at once (everything but fp64), row by row with the backward and forward matrices interleaved: the load
     // order the kernel was tuned with (load_bwd_rows + load_fwd_rows compiles to a different schedule)
     auto load_rows = [&](const T *src) {
-        auto rd = [src](int e) {
-            if constexpr (ADAPT) return __ldcg(src + e);
-            else return src[e];
-        };
+        const auto rd = blob_rd(src);
 #pragma unroll
         for (int a = 0; a < RX; ++a) {
             const int ii = xv[a] ? l * RX + a : 0;
@@ -333,6 +331,9 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     // where element (k, row i) of instance-slot s lives inside a pack region
     auto idx_x = [&](int s, int k, int i) { return (k * 32 + s * L + i / RX) * PVP + (i % RX); };
     auto idx_u = [&](int s, int k, int j) { return (k * 32 + s * L + j / RU) * PVP + RX + (j % RU); };
+    // ... and element (k, row i) of instance ib inside the v-scratch (P.gpi_vscratch: [instance][k][lane][PVP], the pack layout)
+    auto vsc_x = [&](const int64_t ib, int k, int i) { return ((ib * N + k) * L + i / RX) * PVP + (i % RX); };
+    auto vsc_u = [&](const int64_t ib, int k, int j) { return ((ib * N + k) * L + j / RU) * PVP + RX + (j % RU); };
 
     // ---- per-slot bookkeeping (identical in the L lanes of a slot) ----
     int64_t inst = -1;    // instance held by this lane's slot
@@ -974,7 +975,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             // if that was the first iteration of a warm start), else = vnew (admm.cpp:445); untouched when no iteration
             // ran on a warm start
             if (P.s_v && !s_solved && s_it > 0) P.s_v[ox + e] = v;
-            else if (P.s_v && s_solved && !(s_it == 1 && !cold)) P.s_v[ox + e] = P.gpi_vscratch[((ib * N + k) * L + i / RX) * PVP + (i % RX)];
+            else if (P.s_v && s_solved && !(s_it == 1 && !cold)) P.s_v[ox + e] = P.gpi_vscratch[vsc_x(ib, k, i)];
             else if (P.s_v && cold && s_it == 0) P.s_v[ox + e] = T(0);
         }
         for (int e = lane; e < (N - 1) * NU; e += 32) {
@@ -985,7 +986,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             if (P.s_znew) P.s_znew[ou + e] = z;
             if (P.s_y) P.s_y[ou + e] = gPB[w];
             if (P.s_z && !s_solved && s_it > 0) P.s_z[ou + e] = z;
-            else if (P.s_z && s_solved && !(s_it == 1 && !cold)) P.s_z[ou + e] = P.gpi_vscratch[((ib * N + k) * L + j / RU) * PVP + RX + (j % RU)];
+            else if (P.s_z && s_solved && !(s_it == 1 && !cold)) P.s_z[ou + e] = P.gpi_vscratch[vsc_u(ib, k, j)];
             else if (P.s_z && cold && s_it == 0) P.s_z[ou + e] = T(0);
         }
         if constexpr (ROLL) {
@@ -996,12 +997,12 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             for (int e = lane; e < N * NX; e += 32) {
                 const int k = e / NX, i = e - k * NX;
                 if (P.s_v && !(!s_solved && s_it > 0))
-                    P.s_v[ox + e] = (scold && s_it == 0) ? T(0) : P.gpi_vscratch[((ib * N + k) * L + i / RX) * PVP + (i % RX)];
+                    P.s_v[ox + e] = (scold && s_it == 0) ? T(0) : P.gpi_vscratch[vsc_x(ib, k, i)];
             }
             for (int e = lane; e < (N - 1) * NU; e += 32) {
                 const int k = e / NU, j = e - k * NU;
                 if (P.s_z && !(!s_solved && s_it > 0))
-                    P.s_z[ou + e] = (scold && s_it == 0) ? T(0) : P.gpi_vscratch[((ib * N + k) * L + j / RU) * PVP + RX + (j % RU)];
+                    P.s_z[ou + e] = (scold && s_it == 0) ? T(0) : P.gpi_vscratch[vsc_u(ib, k, j)];
             }
         }
         // work->u.col(0): one rollout step from d_0 (every lane computes, the lanes of slot s store)
