@@ -175,8 +175,9 @@ typedef struct tinympc_batch {
     /* Heterogeneous batch (optional, SURVEY §8f-2): one model + cache per instance instead of the handle's shared one.
      * [B][tinympc_b200_model_blob_elems(nx,nu)] elements of the problem dtype, each blob =
      *   Adyn | Bdyn | fdyn | Q | R | Kinf | Pinf | Quu_inv | AmBKt | APf | BPf | rho      (column-major pieces, as in
-     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Cones, hyperplanes and settings stay shared;
-     * box bounds are the handle's unless the batch brings its own (bounds_per_instance below).  Served by the lane-group
+     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Hyperplanes, the cone structure and settings
+     * stay shared; box bounds and cone coefficients are the handle's unless the batch brings its own (bounds_per_instance,
+     * cones_per_instance below).  Served by the lane-group
      * kernels: the on-chip (GPI) kernel when the family is AUTO or GPI, the problem has box constraints only and the
      * horizon fits in shared memory; otherwise (explicit GPS, cones or hyperplanes, a horizon off chip) the streamed (GPS)
      * kernel, one instance per lane group.  TPI returns TINYMPC_ERR_UNSUPPORTED. */
@@ -198,6 +199,20 @@ typedef struct tinympc_batch {
     const void *u_min, *u_max; /* per-instance input bounds, or NULL                         */
     int32_t bounds_per_instance; /* 0: the handle's bounds; 1: one column per instance; 2: full horizon per instance */
     int32_t reserved2;           /* must be 0 */
+    /* Per-instance cone coefficients (optional): instance b projects its cones with its own mu, as a TinySolver whose
+     * tiny_set_cone_constraints got these cx / cu would.  The cone structure (Acx, qcx, Acu, qcu) stays the handle's.
+     * Arrays of the problem dtype, named positionally as in tinympc_problem_t: cone_x_mu goes with Acx / qcx (the state
+     * cones), cone_u_mu with Acu / qcu (the input cones).  With cones_per_instance = 1 a side whose cone loop runs
+     * (en_state_soc / en_input_soc set and the handle has cones on that side) needs its pointer (else TINYMPC_ERR_ARG); a
+     * side whose loop does not run is never read, and when neither runs the solve is the one without per-instance cones.
+     * Any other mode value or a non-zero reserved3 return TINYMPC_ERR_ARG.  DEVICE pointers for tinympc_b200_solve, HOST
+     * pointers (staged per chunk) for tinympc_b200_solve_host.  Served by the streamed (GPS) kernel, the one that runs
+     * cones, with two instances per lane group where the shared solve has two; combines with models and bounds.  STRICT
+     * only: FAST mode, explicit TPI, adaptive rho and rollouts return TINYMPC_ERR_UNSUPPORTED. */
+    const void *cone_x_mu;      /* [B][num_state_cones]: state-cone mu per instance (replaces problem->cx), or NULL */
+    const void *cone_u_mu;      /* [B][num_input_cones]: input-cone mu per instance (replaces problem->cu), or NULL */
+    int32_t cones_per_instance; /* 0: the handle's cx / cu (every zero-initialised batch); 1: the arrays above */
+    int32_t reserved3;          /* must be 0 */
 } tinympc_batch_t;
 
 typedef struct tinympc_b200_solver tinympc_b200_solver_t;

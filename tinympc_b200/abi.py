@@ -71,6 +71,8 @@ class Batch(C.Structure):
         ("models", vp),
         ("x_min", vp), ("x_max", vp), ("u_min", vp), ("u_max", vp),
         ("bounds_per_instance", C.c_int32), ("reserved2", C.c_int32),
+        ("cone_x_mu", vp), ("cone_u_mu", vp),
+        ("cones_per_instance", C.c_int32), ("reserved3", C.c_int32),
     ]
 
 

@@ -49,11 +49,35 @@ def bounds_layout(bounds: dict, B: int, N: int, nx: int, nu: int, dtype) -> int:
     return layouts.pop()
 
 
+CONE_NAMES = ("x_mu", "u_mu")
+
+
+def cones_check(cones: dict, B: int, ncx: int, ncu: int, dtype) -> None:
+    """Check per-instance cone coefficients (a dict with x_mu [B, ncx] for the state cones and / or u_mu [B, ncu] for the
+    input cones; numpy arrays or torch tensors of the problem dtype) against a batch of B instances of a problem with ncx
+    state and ncu input cones (tinympc_batch_t.cone_x_mu / cone_u_mu).  A side may be absent when its cone loop does not run."""
+    unknown = set(cones) - set(CONE_NAMES)
+    if unknown:
+        raise ValueError(f"cones: unknown keys {sorted(unknown)}; expected any of {CONE_NAMES}")
+    given = {k: v for k, v in cones.items() if v is not None}
+    if not given:
+        raise ValueError("cones: give x_mu, u_mu or both")
+    want = np.dtype(dtype)
+    for k, a in given.items():
+        dt = a.dtype if hasattr(a, "dtype") else None
+        if dt is None or str(dt).replace("torch.", "") != want.name:
+            raise ValueError(f"cones: {k} must have the problem dtype {want.name}, got {dt}")
+        nc = ncx if k == "x_mu" else ncu
+        if tuple(a.shape) != (B, nc):
+            raise ValueError(f"cones: {k} must be [{B}, {nc}] (one mu per instance and {'state' if k == 'x_mu' else 'input'} cone), "
+                             f"got {list(a.shape)}")
+
+
 class HostBatch:
     """Owns the numpy buffers of one batched solve and the ctypes struct pointing at them."""
 
     def __init__(self, prob: MPCProblem, x0, Xref, Uref=None, state: dict | None = None, cold_start=True,
-                 want_state=(), want_residuals=True, models=None, bounds: dict | None = None):
+                 want_state=(), want_residuals=True, models=None, bounds: dict | None = None, cones: dict | None = None):
         dt = prob.dtype
         nx, nu, N = prob.nx, prob.nu, prob.N
         self.prob = prob
@@ -88,6 +112,11 @@ class HostBatch:
         if bounds is not None:
             self.bounds_per_instance = bounds_layout(bounds, B, N, nx, nu, dt)
             self.bounds = {k: np.ascontiguousarray(v) for k, v in bounds.items() if v is not None}
+        # per-instance cone coefficients (see cones_check); cones_per_instance 0 = the problem's cx / cu
+        self.cones = None
+        if cones is not None:
+            cones_check(cones, B, len(prob.Acx), len(prob.Acu), dt)
+            self.cones = {k: np.ascontiguousarray(v) for k, v in cones.items() if v is not None}
         self.sol_x = np.zeros((B, N, nx), dtype=dt)
         self.sol_u = np.zeros((B, N - 1, nu), dtype=dt)
         self.iter = np.zeros(B, dtype=np.int32)
@@ -114,6 +143,10 @@ class HostBatch:
         b.bounds_per_instance = self.bounds_per_instance
         for k, a in self.bounds.items():
             setattr(b, k, a.ctypes.data)
+        if self.cones is not None:
+            b.cones_per_instance = 1
+            for k, a in self.cones.items():
+                setattr(b, "cone_" + k, a.ctypes.data)
         b._owner = self
         return b
 

@@ -15,7 +15,7 @@ import ctypes as C
 
 from . import abi
 from ._lib import check
-from .batch import bounds_layout
+from .batch import bounds_layout, cones_check
 from .solver import AdaptiveRho, BatchedTinySolver, pack_models
 
 # box-constrained warm start: slacks + duals (+ the previous-iteration slacks v, z, which only feed the dual residual of
@@ -28,14 +28,16 @@ WARM_FIELDS_FAST = ("vnew", "znew", "g", "y")
 
 class DeviceMPCLoop:
     def __init__(self, solver: BatchedTinySolver, x0, reset_duals: bool = False, extra_state=(), exact_first_residual: bool = True,
-                 adaptive_rho: AdaptiveRho | None = None, models=None, bounds: dict | None = None):
+                 adaptive_rho: AdaptiveRho | None = None, models=None, bounds: dict | None = None, cones: dict | None = None):
         """models ([B, blob], tinympc_batch_t.models, e.g. from setup_models): a heterogeneous fleet, one model, cache and rho
         per plant.  Every step solves with them and advances plant b with its own A, B, f (tinympc_b200_advance_models).
         adaptive_rho: every plant adapts its own rho / Kinf / Pinf, kept on the device across steps in self.models
         (starting from `models` or the problem's own cache), as one TinySolver per robot would; with `models`, give it
         per-instance tables (solver.setup_sensitivity_device), which stay on the GPU with the models.
         bounds: per-instance box bounds of every plant (a dict as in BatchedTinySolver.solve), kept on the device across steps
-        in self.bounds; step(..., bounds=...) replaces them for one step (a moving corridor)."""
+        in self.bounds; step(..., bounds=...) replaces them for one step (a moving corridor).
+        cones: per-instance cone coefficients of every plant (a dict as in BatchedTinySolver.solve), kept on the device across
+        steps in self.cones; step(..., cones=...) replaces them for one step."""
         import torch
 
         self.solver = solver
@@ -57,6 +59,7 @@ class DeviceMPCLoop:
             self.adaptive_rho = AdaptiveRho(cm(adaptive_rho.dKinf_drho), cm(adaptive_rho.dPinf_drho), adaptive_rho.rho_min,
                                             adaptive_rho.rho_max, adaptive_rho.enable_clipping)
         self.bounds = None if bounds is None else self._device_bounds(bounds)
+        self.cones = None if cones is None else self._device_cones(cones)
         self.models = None
         if adaptive_rho is not None or models is not None:
             m = pack_models(p, self.B) if models is None else models
@@ -69,10 +72,17 @@ class DeviceMPCLoop:
         bounds_layout(bounds, self.B, p.N, p.nx, p.nu, p.dtype)
         return {k: torch.as_tensor(v, device=self.dev).contiguous() for k, v in bounds.items() if v is not None}
 
-    def step(self, Xref, Uref=None, stream=None, bounds=None):
+    def _device_cones(self, cones):
+        import torch
+
+        p = self.solver.problem
+        cones_check(cones, self.B, len(p.Acx), len(p.Acu), p.dtype)
+        return {k: torch.as_tensor(v, device=self.dev).contiguous() for k, v in cones.items() if v is not None}
+
+    def step(self, Xref, Uref=None, stream=None, bounds=None, cones=None):
         """One MPC step for every instance: solve (warm-started), then advance the plants.  Returns the output dict
         (device tensors: sol_x, sol_u, iter, solved, residuals and the state fields).  bounds: per-instance box bounds for this
-        step only, in place of the loop's."""
+        step only, in place of the loop's; cones: per-instance cone coefficients for this step only, likewise."""
         import torch
 
         s = self.solver
@@ -82,7 +92,7 @@ class DeviceMPCLoop:
         het = self.models is not None and self.adaptive_rho is None
         batch, out = s.make_device_batch(self.x0, Xref, Uref, state=self.state, cold_start=self._first, want_state=self.fields,
                                          want_u0=True, want_solution=self.want_solution, models=self.models if het else None,
-                                         bounds=self.bounds if bounds is None else bounds)
+                                         bounds=self.bounds if bounds is None else bounds, cones=self.cones if cones is None else cones)
         if self.adaptive_rho is None:
             s.solve_device(batch, stream)
         else:
@@ -112,6 +122,8 @@ class DeviceMPCLoop:
             raise ValueError("rollout: adaptive rho is not available in a rollout; use step()")
         if self.bounds is not None:
             raise ValueError("rollout: per-instance bounds are not available in a rollout; use step()")
+        if self.cones is not None:
+            raise ValueError("rollout: per-instance cones are not available in a rollout; use step()")
         if len(self.fields) != len(WARM_FIELDS if "v" in self.fields else WARM_FIELDS_FAST):
             raise ValueError("rollout: covers box constraints only (no extra_state); use step()")
         T = int(T)

@@ -172,6 +172,15 @@ int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const t
         if ((st.en_state_bound && !io->x_min) || (st.en_input_bound && !io->u_min))
             return fail(TINYMPC_ERR_NO_BOUNDS, "per-instance bounds: en_state_bound/en_input_bound set but the batch has no x_min/x_max or u_min/u_max");
     }
+    if ((io->cones_per_instance != 0 && io->cones_per_instance != 1) || io->reserved3 != 0)
+        return fail(TINYMPC_ERR_ARG, "cones_per_instance must be 0 (the handle's cone coefficients) or 1 (cone_x_mu / cone_u_mu per "
+                                     "instance), and reserved3 must be 0");
+    if (io->cones_per_instance) {  // a side whose cone loop runs needs its coefficients; the other side's pointer is never read
+        const tmpc::Features ft = features(s);
+        if ((ft.soc_x && !io->cone_x_mu) || (ft.soc_u && !io->cone_u_mu))
+            return fail(TINYMPC_ERR_ARG, "per-instance cones: en_state_soc / en_input_soc set on a side with cones but the batch has no "
+                                         "cone_x_mu / cone_u_mu for it");
+    }
     if (st.check_termination <= 0) return fail(TINYMPC_ERR_ARG, "check_termination must be >= 1");
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     if (ar && io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
@@ -193,12 +202,22 @@ struct SolvePlan {
 // shared memory the adaptive kernel adds per CTA for its tables
 size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->pd.nx, s->pd.nu, esize(s->pd.dtype)); }
 
-// The plan of a solve of B instances (models: per-instance models; bounds: per-instance box bounds; adapt: adaptive rho).
+// The plan of a solve of B instances (models: per-instance models; bounds: per-instance box bounds; cones: per-instance cone
+// coefficients, cones_per_instance set; adapt: adaptive rho).
 // GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed
 // (everything else the lane mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature
 // cannot be served.
-int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool adapt, int64_t B, SolvePlan *p, bool rollout = false) {
+int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cones, bool adapt, int64_t B, SolvePlan *p,
+               bool rollout = false) {
     const tmpc::Features ft = features(s);
+    if (cones) {  // per-instance cone coefficients have STRICT variants of the streamed kernel only
+        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's cone coefficients (cones_per_instance must be 0)");
+        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's cone coefficients (cones_per_instance must be 0)");
+        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones are available in STRICT mode only");
+        if (s->family == TINYMPC_KERNEL_TPI)
+            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones run on the streamed lane-group kernel (GPS), not on one thread per instance");
+    }
+    const bool cones_run = cones && (ft.soc_x || ft.soc_u);  // else the coefficients are never read: the plan without them
     if (bounds) {  // per-instance bounds have STRICT solve variants only
         if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's bounds (bounds_per_instance must be 0)");
         if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's bounds (bounds_per_instance must be 0)");
@@ -270,9 +289,14 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool adap
         } else {
             if (!gps_ok) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models / bounds: this problem needs the streamed lane-group kernel, which does not cover this shape");
             p->family = TINYMPC_KERNEL_GPS;
-            p->per_cta = s->dim->gps_het_slots(s->pd.dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, s->max_smem_optin);
+            p->per_cta = s->dim->gps_het_slots(s->pd.dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, cones_run,
+                                               s->max_smem_optin);
         }
     }
+    // A cone loop routes the solve to the streamed kernel when it covers the shape; its GPS_CONES variants keep the plan the
+    // rules above chose (alone: the shared solve's, whose chunks are not rounded; with models or bounds: gps_het_slots)
+    if (cones_run && p->family != TINYMPC_KERNEL_GPS)
+        return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones: this problem needs the streamed lane-group kernel, which does not cover this shape");
     if (p->family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
     return 0;
 }
@@ -354,7 +378,9 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
             const tinympc_adaptive_rho_t *ar = nullptr, const tinympc_rollout_t *ro = nullptr) {
     SolvePlan plan;
     if (ar || ro || io->B > 0)  // an adaptive solve or a rollout is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, ar != nullptr, io->B, &plan, ro != nullptr)) return rc;
+        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0, ar != nullptr, io->B,
+                                &plan, ro != nullptr))
+            return rc;
     if (io->B <= 0 || (ro && ro->T == 0)) return TINYMPC_OK;
     const int family = plan.family;
     // The launch scratch of a handle (work queue, workspaces, timing events) is single-buffered: a solve enqueued on a
@@ -369,6 +395,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     d.sm_count = s->sm_count;
     d.max_smem_optin = s->max_smem_optin;
     d.bounds = io->bounds_per_instance;
+    d.cones = io->cones_per_instance && (d.ft.soc_x || d.ft.soc_u);
     if (ar) {
         if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, io->models, stream)
                                                 : upload_adaptive<float>(s, ar, io->models, stream))
@@ -891,7 +918,8 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     chunk = (chunk + 31) / 32 * 32;
     SolvePlan plan;  // of a chunk
     if (ar || B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, ar != nullptr, chunk, &plan)) return rc;
+        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0, ar != nullptr, chunk, &plan))
+            return rc;
     if (B <= 0) return TINYMPC_OK;
     const size_t es = esize(s->pd.dtype);
     const size_t bx = es * s->pd.nx * s->pd.N, bu = es * s->pd.nu * (s->pd.N - 1);
@@ -937,6 +965,13 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
         } else {
             dev.u_min = dev.u_max = nullptr;
         }
+    }
+    if (io->cones_per_instance) {  // sliced per chunk like the bounds; a side whose cone loop does not run is never read
+        const tmpc::Features ft = features(s);
+        if (ft.soc_x) fields.push_back({io->cone_x_mu, nullptr, es * s->pd.ncx, true, false, (void **)&dev.cone_x_mu});
+        else dev.cone_x_mu = nullptr;
+        if (ft.soc_u) fields.push_back({io->cone_u_mu, nullptr, es * s->pd.ncu, true, false, (void **)&dev.cone_u_mu});
+        else dev.cone_u_mu = nullptr;
     }
     if (ar && ar->tables_per_instance) {  // sliced per chunk like the models
         fields.push_back({ar->dKinf_drho, nullptr, es * s->pd.nu * s->pd.nx, true, false, (void **)&args.ar.dKinf_drho});

@@ -212,7 +212,8 @@ struct KParams {
     T *gpi_vscratch;  // GPI: [B][N][L][PVP] copy of the previous primal pack (work->v / work->z) while v,z are persisted
     T *gps_ws;        // GPS: [resident warps][N][gps.rec] streamed state records
     GpsLayout gps;
-    // TPI workspace (structure-of-arrays, 16-byte vectors, [k][vec][Bpad])
+    // TPI workspace (structure-of-arrays, 16-byte vectors, [k][vec][Bpad]).  The streamed kernel's GPS_CONES variants find the
+    // per-instance cone coefficients in w_vc (state cones) and w_zc (input cones).
     void *w_v[2], *w_z[2], *w_g, *w_y, *w_d;
     void *w_vc, *w_zc, *w_gc, *w_yc, *w_vl, *w_zl, *w_gl, *w_yl, *w_vlt, *w_zlt, *w_glt, *w_ylt;
 };

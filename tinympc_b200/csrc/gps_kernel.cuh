@@ -62,6 +62,7 @@ struct GpsCfg : LaneGeom<NX, NU, L, ES> {
     static constexpr int SWEEP_REGS = (FWD_ROWS > BWD_ROWS ? FWD_ROWS : BWD_ROWS) * (ES / 4);
     static constexpr bool ok = (NX % RX == 0) && (NU % RU == 0) && SWEEP_REGS <= 112;
     static constexpr int PARK_BYTES = 32 * NI * 2 * RX * ES;  // per-lane x0 rows and terminal-cost rows (kept out of registers)
+    static constexpr int MU_BYTES = SPW * 2 * MAX_CONES * ES;  // GPS_CONES: the warp's cone-coefficient table [slot][side][cone]
 };
 
 // Record layout: one record per (warp, knot point), every field [slot of the warp][row] padded to 16 bytes.  Region A is
@@ -204,16 +205,25 @@ constexpr int GPS_HET = 8;
 // its instance's column 0 when it is loaded.  One instance per lane group, as GPS_HET: the bound registers are per lane, and
 // two instances with bounds of their own do not fit the NI = 2 budget.
 constexpr int GPS_BOUNDS = 16;
-constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS;  // the family-mask bits that are not constraint families
+// Per-instance cone coefficients (tinympc_batch_t.cones_per_instance): GPS_CONES added to a family mask with cones (1, 7).
+// P.w_vc / P.w_zc (thread-per-instance workspace pointers, which this kernel never reads otherwise) point at the batch's
+// [B][ncx] / [B][ncu] coefficients.  Each warp keeps a table [slot][side][MAX_CONES] in shared memory, after the rings of all
+// warps, which a slot's lanes fill when the slot is loaded.  In cones_xu lane l of a group always projects work item l, one
+// (instance, side) pair, so a lane reads the coefficients of one slot and one side only: they stay out of registers, and
+// the kernel keeps the NI of the shared solve (two instances per lane group where the shared model runs two).
+constexpr int GPS_CONES = 32;
+constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS | GPS_CONES;  // the family-mask bits that are not constraint families
 
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     gps_solve_kernel(const __grid_constant__ KParams<T, NX, NU> P, const T *__restrict__ gmat, unsigned long long *queue) {
     constexpr bool HET = (FAMH & GPS_HET) != 0;     // per-instance models
     constexpr bool BND = (FAMH & GPS_BOUNDS) != 0;  // per-instance box bounds
+    constexpr bool CN = (FAMH & GPS_CONES) != 0;    // per-instance cone coefficients
     constexpr int FAM = FAMH & ~GPS_VARIANTS;       // constraint families compiled in
     static_assert(!HET || NI == 1, "per-instance models run one instance per lane group");
     static_assert(!BND || (NI == 1 && !FAST), "per-instance bounds run one instance per lane group, in STRICT mode");
+    static_assert(!CN || ((FAM & 1) != 0 && !FAST), "per-instance cone coefficients need the cone family, in STRICT mode");
     using Cfg = GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAM>;
     using REC = GpsRec<NX, NU, Cfg::SPW, (int)sizeof(T), FAM>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -299,6 +309,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     const unsigned aPark = aGU + (unsigned)Cfg::GBU * ES + (unsigned)lane * (NI * 2 * RX) * ES;  // [j][x0 rows | pterm rows]
     const unsigned aRing = aGU + (unsigned)Cfg::GBU * ES + (unsigned)Cfg::PARK_BYTES;
     const unsigned aBar = aRing + (unsigned)RING::RING;  // NBAR mbarriers of this warp
+    // GPS_CONES: this warp's cone-coefficient table, behind the areas of all warps
+    const unsigned aMu = CN ? aZero + (unsigned)RING::ZERO_BYTES + (unsigned)nwarps * wbytes + (unsigned)warp * (unsigned)Cfg::MU_BYTES : 0u;
     // this lane's rows inside a state-shaped / input-shaped field of a record image (first instance of the group)
     const unsigned lxo = (unsigned)(grp * NX + l * RX) * ES, luo = (unsigned)(grp * NU + l * RU) * ES;
     // the CTA's zero image: what padding lanes read instead of a record image, so that their arithmetic stays finite and
@@ -421,6 +433,20 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
         sts_piece<T, RX, SX>(aPark + (unsigned)((2 * j) * RX) * ES, z);
         sts_piece<T, RX, SX>(aPark + (unsigned)((2 * j + 1) * RX) * ES, z);
     }
+    // GPS_CONES: the lanes of slot sidx's group copy instance ib's coefficients into the slot's rows of the table (unused
+    // cones: zeros).  P.ncx / P.ncu are 0 for a side whose cone loop does not run, whose pointer is then never read.
+    auto load_mu = [&](int sidx, int64_t ib) {
+        const T *const mux = (const T *)P.w_vc, *const muu = (const T *)P.w_zc;
+        for (int e = l; e < 2 * MAX_CONES; e += L) {
+            const int side = e / MAX_CONES, c = e - side * MAX_CONES, nc = side ? P.ncu : P.ncx;
+            const T mu = c < nc ? __ldg((side ? muu : mux) + ib * nc + c) : T(0);
+            sts(aMu + (unsigned)(sidx * 2 * MAX_CONES + e) * ES, mu);
+        }
+    };
+    if constexpr (CN) {  // a slot that never gets an instance projects with instance 0's coefficients
+#pragma unroll
+        for (int j = 0; j < NI; ++j) load_mu(j * IPW + grp, 0);
+    }
     // x0 rows / terminal-cost rows of instance j of this lane's group: parked in shared memory, fetched where used
     auto load_x0 = [&](int j, T (&v)[RX]) { lds_piece<T, RX, SX>(aPark + (unsigned)((2 * j) * RX) * ES, v); };
     auto load_pterm = [&](int j, T (&v)[RX]) { lds_piece<T, RX, SX>(aPark + (unsigned)((2 * j + 1) * RX) * ES, v); };
@@ -456,7 +482,9 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                 const int j_ = (item >> 1) < NI ? (item >> 1) : NI - 1;
                 const bool ok = item < 2 * NI && (side ? c < ncu : c < ncx);
                 const int st0 = ok ? (side ? P.cone_u_start[c] : P.cone_x_start[c]) : 0;
-                const T mu = side ? P.cone_u_mu[c] : P.cone_x_mu[c];
+                T mu;
+                if constexpr (CN) mu = lds(aMu + (unsigned)(((j_ * IPW + grp) * 2 + side) * MAX_CONES + c) * ES, T());  // the slot's own
+                else mu = side ? P.cone_u_mu[c] : P.cone_x_mu[c];
                 const unsigned base = (side ? guf(j_) : gxf(j_)) + (unsigned)st0 * ES;
                 T s0 = lds(base, T()), s1 = lds(base + ES, T()), s2 = lds(base + 2 * ES, T());
                 project_soc3_sel(s0, s1, s2, mu);
@@ -904,6 +932,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
             // per-instance bounds: column 0 of this instance (one column per instance, or its horizon)
             if constexpr (BND)
                 box_bounds_at<true>(P, tvb ? ox : ib * NX, tvb ? ou : ib * NU, l, 0, true, enx, enu, xok, uok, loX, hiX, loU, hiU);
+            if constexpr (CN) load_mu(sidx, ib);  // per-instance cone coefficients of this instance
             const T *xl = xrefb + (int64_t)(N - 1) * NX;
             T x0v[RX], ptv[RX];
 #pragma unroll
@@ -1118,26 +1147,29 @@ struct GpsPlan {
     GpsLayout ly;
 };
 
-// shared memory per CTA: the staged blob and the zero image, then one ring per warp
-template <typename T, int NX, int NU, int L, int NI, int FAM>
+// shared memory per CTA: the staged blob and the zero image, then one ring per warp (FAMH: family mask and variant bits;
+// GPS_CONES adds a cone-coefficient table per warp)
+template <typename T, int NX, int NU, int L, int NI, int FAMH>
 inline size_t gps_smem(int warps) {
-    using RINGH = GpsRing<NX, NU, L, (int)sizeof(T), NI, FAM>;
-    return cache_reserve_bytes(NX, NU, sizeof(T)) + RINGH::ZERO_BYTES + RINGH::WARP_BYTES * (size_t)warps;
+    using RINGH = GpsRing<NX, NU, L, (int)sizeof(T), NI, FAMH & ~GPS_VARIANTS>;
+    const size_t mu = (FAMH & GPS_CONES) ? (size_t)GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAMH & ~GPS_VARIANTS>::MU_BYTES : 0;
+    return cache_reserve_bytes(NX, NU, sizeof(T)) + RINGH::ZERO_BYTES + (RINGH::WARP_BYTES + mu) * (size_t)warps;
 }
 
 // most warps per CTA: shared memory, registers (gps_max_warps) and TINYMPC_GPS_WARPS; 0 = not even one warp fits
-template <typename T, int NX, int NU, int L, int NI, int FAM>
+template <typename T, int NX, int NU, int L, int NI, int FAMH>
 inline int gps_warps_max(int max_smem_optin) {
-    const size_t max_smem = (size_t)(max_smem_optin - 64), fixed = gps_smem<T, NX, NU, L, NI, FAM>(0);
-    const size_t per_warp = gps_smem<T, NX, NU, L, NI, FAM>(1) - fixed;
+    const size_t max_smem = (size_t)(max_smem_optin - 64), fixed = gps_smem<T, NX, NU, L, NI, FAMH>(0);
+    const size_t per_warp = gps_smem<T, NX, NU, L, NI, FAMH>(1) - fixed;
     if (fixed + per_warp > max_smem) return 0;
     const int maxw = (int)std::min<size_t>(gps_max_warps(NI), (max_smem - fixed) / per_warp);
     const char *e = std::getenv("TINYMPC_GPS_WARPS");  // a cap for tests that need many waves
     return std::max(1, std::min(maxw, std::max(1, e ? std::atoi(e) : gps_max_warps(NI))));
 }
 
-template <typename T, int NX, int NU, int L, int NI, int FAM>
+template <typename T, int NX, int NU, int L, int NI, int FAMH>
 inline GpsPlan gps_plan_L(const LaunchDesc &d) {
+    constexpr int FAM = FAMH & ~GPS_VARIANTS;
     using Cfg = GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAM>;
     using REC = GpsRec<NX, NU, Cfg::SPW, (int)sizeof(T), FAM>;
     GpsPlan p;
@@ -1145,7 +1177,7 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     const tinympc_state_t &s = d.io.state;
     // region B: previous box slacks (work->v / work->z) and family slacks, only when the caller wants them back
     p.ly.has_b = (s.v || s.z || s.vcnew || s.zcnew || s.vlnew || s.zlnew || s.vlnew_tv || s.zlnew_tv) ? 1 : 0;
-    const int maxw = gps_warps_max<T, NX, NU, L, NI, FAM>(d.max_smem_optin);
+    const int maxw = gps_warps_max<T, NX, NU, L, NI, FAMH>(d.max_smem_optin);
     if (maxw == 0) return p;
     // balance the waves: with `waves` passes over the resident slots, use just enough warps per SM to hold B / waves
     const int64_t groups = (d.io.B + SPW - 1) / SPW;  // warps' worth of instances
@@ -1156,15 +1188,16 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     p.NI = NI;
     p.warps = warps;
     p.ctas = (int)std::max<int64_t>(1, std::min<int64_t>(d.sm_count, (groups + warps - 1) / warps));
-    p.smem = gps_smem<T, NX, NU, L, NI, FAM>(warps);
+    p.smem = gps_smem<T, NX, NU, L, NI, FAMH>(warps);
     p.ws_bytes = (size_t)p.ctas * warps * d.pd->N * (REC::recA + (p.ly.has_b ? REC::recB : 0)) * sizeof(T);
     return p;
 }
 
-// FAMH: family mask, plus GPS_HET for per-instance models and GPS_BOUNDS for per-instance bounds
+// FAMH: family mask, plus GPS_HET for per-instance models, GPS_BOUNDS for per-instance bounds and GPS_CONES for per-instance
+// cone coefficients
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
-    const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH & ~GPS_VARIANTS>(*d);
+    const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH>(*d);
     if (plan.L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
     d->out_ws_need = plan.ws_bytes;
     if (!d->gps_ws || d->gps_ws_bytes < plan.ws_bytes) return TM_ERR_WORKSPACE;
@@ -1188,6 +1221,27 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     } else {
         constexpr int NI = gps_pick_NI<T, NX, NU, L>();
         const int fam = gps_family_mask(d->ft.soc_x || d->ft.soc_u, d->ft.lin_x || d->ft.lin_u || d->ft.tvl_x || d->ft.tvl_u);
+        if (d->cones) {  // per-instance cone coefficients (STRICT; a cone loop runs, so the mask is 1 or 7): the shared solve's NI
+                         // on their own, one instance per lane group with per-instance models or bounds
+            if constexpr (FAST) {
+                return TINYMPC_ERR_UNSUPPORTED;
+            } else {
+                const bool het = d->io.models != nullptr;
+#define TM_GPS_CN_CASE(FF)                                                                                             \
+    if (fam == FF) {                                                                                                   \
+        if (d->bounds) {                                                                                               \
+            if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_CONES | GPS_BOUNDS | GPS_HET, false>(d, P0);      \
+            return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_CONES | GPS_BOUNDS, false>(d, P0);                         \
+        }                                                                                                              \
+        if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_CONES | GPS_HET, false>(d, P0);                       \
+        return launch_gps_cfg<T, NX, NU, L, NI, FF | GPS_CONES, false>(d, P0);                                         \
+    }
+                TM_GPS_CN_CASE(1)
+                TM_GPS_CN_CASE(7)
+#undef TM_GPS_CN_CASE
+                return TINYMPC_ERR_UNSUPPORTED;
+            }
+        }
         if (d->bounds) {  // per-instance bounds (STRICT): one instance per lane group, with or without per-instance models
             if constexpr (FAST) {
                 return TINYMPC_ERR_UNSUPPORTED;
@@ -1227,16 +1281,19 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     }
 }
 
-// instances one CTA of the one-instance-per-lane-group variants (per-instance models, per-instance bounds, or both) holds when the
-// batch fills every SM (the host path rounds its chunks to whole waves of these); 0 = shape not available
+// instances one CTA of the one-instance-per-lane-group variants (per-instance models, per-instance bounds, or both; cones: with
+// per-instance cone coefficients too) holds when the batch fills every SM (the host path rounds its chunks to whole waves of
+// these); 0 = shape not available
 template <typename T, int NX, int NU>
-int gps_het_slots(int fam, int max_smem_optin) {
+int gps_het_slots(int fam, bool cones, int max_smem_optin) {
     constexpr int L = gps_pick_L<T, NX, NU>();
     if constexpr (L == 0) {
         return 0;
     } else {
         int warps;
-        if (fam == 0) warps = gps_warps_max<T, NX, NU, L, 1, 0>(max_smem_optin);
+        if (cones) warps = fam == 1 ? gps_warps_max<T, NX, NU, L, 1, 1 | GPS_CONES>(max_smem_optin)
+                                    : gps_warps_max<T, NX, NU, L, 1, 7 | GPS_CONES>(max_smem_optin);
+        else if (fam == 0) warps = gps_warps_max<T, NX, NU, L, 1, 0>(max_smem_optin);
         else if (fam == 1) warps = gps_warps_max<T, NX, NU, L, 1, 1>(max_smem_optin);
         else if (fam == 6) warps = gps_warps_max<T, NX, NU, L, 1, 6>(max_smem_optin);
         else warps = gps_warps_max<T, NX, NU, L, 1, 7>(max_smem_optin);

@@ -24,7 +24,7 @@ extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d);
 extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin);
 extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d);
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype);
-extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, int max_smem_optin);
+extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, bool cones, int max_smem_optin);
 
 #if TM_PART == 0
 // =========================================================================================================
@@ -47,7 +47,7 @@ int launch_tpi(LaunchDesc *d) {
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->io.models || d->bounds) return TINYMPC_ERR_UNSUPPORTED;  // per-instance models and bounds: the lane-group kernels only
+    if (d->io.models || d->bounds || d->cones) return TINYMPC_ERR_UNSUPPORTED;  // per-instance data: the lane-group kernels only
     if (d->ft.ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
     return d->fast ? launch_tpi<T, true, false>(d) : launch_tpi<T, false, false>(d);
 }
@@ -195,10 +195,10 @@ extern "C" int TM_SYM(tm_gps_lanes_)(int dtype) {
     if (dtype == TINYMPC_F64) return tmpc::gps_pick_L<double, TM_NX, TM_NU>();
     return 0;
 }
-extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, int max_smem_optin) {
+extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, bool cones, int max_smem_optin) {
     const int fam = tmpc::gps_family_mask(soc, lin);
-    if (dtype == TINYMPC_F32) return tmpc::gps_het_slots<float, TM_NX, TM_NU>(fam, max_smem_optin);
-    if (dtype == TINYMPC_F64) return tmpc::gps_het_slots<double, TM_NX, TM_NU>(fam, max_smem_optin);
+    if (dtype == TINYMPC_F32) return tmpc::gps_het_slots<float, TM_NX, TM_NU>(fam, cones && soc, max_smem_optin);
+    if (dtype == TINYMPC_F64) return tmpc::gps_het_slots<double, TM_NX, TM_NU>(fam, cones && soc, max_smem_optin);
     return 0;
 }
 #endif

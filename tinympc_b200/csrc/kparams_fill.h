@@ -116,6 +116,10 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
         tpi_workspace(NX, NU, pd.N, pd.dtype, d.Bpad, ft, (char *)d.tpi_ws, w);
         std::memcpy((char *)&P + offsetof(KP, w_v), w, sizeof(w));
     }
+    if (d.cones) {  // per-instance cone coefficients ride in two workspace pointers the streamed kernel never reads (gps_kernel.cuh: GPS_CONES)
+        P.w_vc = const_cast<void *>(d.io.cone_x_mu);
+        P.w_zc = const_cast<void *>(d.io.cone_u_mu);
+    }
 }
 
 }  // namespace tmpc

@@ -69,6 +69,9 @@ struct LaunchDesc {
     // per-instance box bounds (io.bounds_per_instance): 0 = the problem's; 1 = io.x_min ... u_max hold one column per instance;
     // 2 = they hold a horizon per instance.  The lane-group kernels' GPI_BOUNDS / GPS_BOUNDS variants read them.
     int bounds;
+    // per-instance cone coefficients (io.cones_per_instance) with a cone loop that runs: io.cone_x_mu / cone_u_mu hold [B][ncx] /
+    // [B][ncu].  The streamed kernel's GPS_CONES variants read them.
+    int cones;
 
     cudaStream_t stream;
     int sm_count;
@@ -113,8 +116,8 @@ struct DimEntry {
     // streamed lane-group kernel (gps_kernel.cuh): lanes per instance; 0 = shape not available
     int (*gps_lanes)(int dtype);
     // its per-instance-model variant (io.models): instances per CTA when the batch fills every SM, for the shape and the
-    // constraint families (cones, hyperplanes); 0 = not available
-    int (*gps_het_slots)(int dtype, bool soc, bool lin, int max_smem_optin);
+    // constraint families (cones, hyperplanes), with or without per-instance cone coefficients; 0 = not available
+    int (*gps_het_slots)(int dtype, bool soc, bool lin, bool cones, int max_smem_optin);
 };
 
 }  // namespace tmpc

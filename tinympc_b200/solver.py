@@ -19,7 +19,7 @@ import numpy as np
 
 from . import abi
 from ._lib import check, load
-from .batch import BOUND_NAMES, HostBatch, bounds_layout
+from .batch import BOUND_NAMES, CONE_NAMES, HostBatch, bounds_layout, cones_check
 from .problem import MPCProblem, copy_settings, default_settings, dtype_code
 from .workloads import ModelSpec
 
@@ -219,19 +219,23 @@ class BatchedTinySolver:
 
     # ---- host buffers (numpy): the call a reference user would make; H2D/D2H inside ------------------
     def solve(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), models=None,
-              adaptive_rho: AdaptiveRho | None = None, bounds: dict | None = None) -> dict:
+              adaptive_rho: AdaptiveRho | None = None, bounds: dict | None = None, cones: dict | None = None) -> dict:
         """With adaptive_rho: every instance adapts its own rho / Kinf / Pinf, starting from its blob in `models` (default:
         the problem's own cache, pack_models); the result's "models" holds the adapted blobs, the start of the next solve.
         bounds: per-instance box bounds in place of the problem's, a dict with any of x_min, x_max, u_min, u_max of the
         problem dtype: [B, nx] / [B, nu] (one column per instance) or [B, N, nx] / [B, N-1, nu] (a horizon per instance);
-        a side may be absent when its bound is disabled (tinympc_batch_t.bounds_per_instance)."""
+        a side may be absent when its bound is disabled (tinympc_batch_t.bounds_per_instance).
+        cones: per-instance cone coefficients in place of the problem's cx / cu, a dict with x_mu [B, num state cones] and / or
+        u_mu [B, num input cones] of the problem dtype; a side may be absent when its cone loop does not run
+        (tinympc_batch_t.cones_per_instance)."""
         if adaptive_rho is None:
             hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, models=models,
-                           bounds=bounds)
+                           bounds=bounds, cones=cones)
             cb = hb.to_c()
             check(self._lib.tinympc_b200_solve_host(self._h, C.byref(cb)))
             return hb.result()
-        hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, bounds=bounds)
+        hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, bounds=bounds,
+                       cones=cones)
         m = pack_models(self.problem, hb.B) if models is None else np.array(models, dtype=self.problem.dtype).reshape(hb.B, -1)
         cb, ar = hb.to_c(), adaptive_rho.to_c(self.problem, m.ctypes.data, hb.B)
         check(self._lib.tinympc_b200_solve_adaptive_host(self._h, C.byref(cb), C.byref(ar)))
@@ -297,9 +301,10 @@ class BatchedTinySolver:
 
     # ---- device buffers (torch tensors on cuda:<device>) ---------------------------------------------
     def make_device_batch(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), want_residuals=True,
-                          want_u0=False, want_solution=True, models=None, bounds: dict | None = None):
-        """Allocate/adopt torch CUDA tensors and build the device-pointer tinympc_batch_t.  bounds: per-instance box bounds as
-        in solve(); torch CUDA tensors of the problem dtype are used in place, numpy arrays are uploaded."""
+                          want_u0=False, want_solution=True, models=None, bounds: dict | None = None, cones: dict | None = None):
+        """Allocate/adopt torch CUDA tensors and build the device-pointer tinympc_batch_t.  bounds: per-instance box bounds,
+        cones: per-instance cone coefficients, both as in solve(); torch CUDA tensors of the problem dtype are used in place,
+        numpy arrays are uploaded."""
         import torch
 
         p = self.problem
@@ -354,6 +359,13 @@ class BatchedTinySolver:
             for k in BOUND_NAMES:
                 setattr(b, k, bt[k].data_ptr() if k in bt else None)
             tens["bounds"] = bt
+        if cones is not None:
+            cones_check(cones, B, len(p.Acx), len(p.Acu), p.dtype)
+            ct = {k: t(v) for k, v in cones.items() if v is not None}
+            b.cones_per_instance = 1
+            for k in CONE_NAMES:
+                setattr(b, "cone_" + k, ct[k].data_ptr() if k in ct else None)
+            tens["cones"] = ct
         b.iter, b.solved = out["iter"].data_ptr(), out["solved"].data_ptr()
         b.residuals = None if out["residuals"] is None else out["residuals"].data_ptr()
         res = dict(out)

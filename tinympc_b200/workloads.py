@@ -91,6 +91,20 @@ def rocket_fleet(B, N=100, seed=0, mass_spread=0.2) -> dict:
                 Rdiag=tile(spec.Rdiag), rho=np.full(B, spec.rho), m=m, spec=spec)
 
 
+def cone_fleet(spec: ModelSpec, B, seed=0, scale=(0.6, 1.0), dtype=np.float64) -> dict:
+    """Per-robot cone coefficients for a fleet of B robots of `spec` (e.g. rocket(), or rocket_fleet's spec): robot b's mu
+    of every state and input cone is the spec's cx / cu times its own factor drawn from U(scale), e.g. a tighter glide
+    slope and thrust-vector cone per rocket, or a friction coefficient per legged robot.  -> dict(x_mu [B, ncx],
+    u_mu [B, ncu]) of `dtype`, the `cones=` argument of BatchedTinySolver.solve / make_device_batch / DeviceMPCLoop."""
+    rng = np.random.default_rng(seed)
+    cx = np.asarray(spec.constraints.get("cx", []), dtype=np.float64)
+    cu = np.asarray(spec.constraints.get("cu", []), dtype=np.float64)
+    lo, hi = scale
+    x_mu = cx[None, :] * rng.uniform(lo, hi, size=(B, cx.size))
+    u_mu = cu[None, :] * rng.uniform(lo, hi, size=(B, cu.size))
+    return dict(x_mu=x_mu.astype(dtype), u_mu=u_mu.astype(dtype))
+
+
 def random_lti(nx, nu, N, seed=0) -> ModelSpec:
     """SURVEY §8d C5 generator: A = I + 0.05 G rescaled to spectral radius 1, B ~ N(0, 0.1^2)."""
     rng = np.random.default_rng(1000003 * seed + 7919 * nx + 104729 * nu)
