@@ -175,9 +175,9 @@ typedef struct tinympc_batch {
     /* Heterogeneous batch (optional, SURVEY §8f-2): one model + cache per instance instead of the handle's shared one.
      * [B][tinympc_b200_model_blob_elems(nx,nu)] elements of the problem dtype, each blob =
      *   Adyn | Bdyn | fdyn | Q | R | Kinf | Pinf | Quu_inv | AmBKt | APf | BPf | rho      (column-major pieces, as in
-     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Hyperplanes, the cone structure and settings
-     * stay shared; box bounds and cone coefficients are the handle's unless the batch brings its own (bounds_per_instance,
-     * cones_per_instance below).  Served by the lane-group
+     * tinympc_problem_t); build it with tinympc_b200_precompute_cache_batch.  Time-varying hyperplanes, the cone structure
+     * and settings stay shared; box bounds, cone coefficients and static hyperplanes are the handle's unless the batch brings
+     * its own (bounds_per_instance, cones_per_instance, planes_per_instance below).  Served by the lane-group
      * kernels: the on-chip (GPI) kernel when the family is AUTO or GPI, the problem has box constraints only and the
      * horizon fits in shared memory; otherwise (explicit GPS, cones or hyperplanes, a horizon off chip) the streamed (GPS)
      * kernel, one instance per lane group.  TPI returns TINYMPC_ERR_UNSUPPORTED. */
@@ -213,6 +213,24 @@ typedef struct tinympc_batch {
     const void *cone_u_mu;      /* [B][num_input_cones]: input-cone mu per instance (replaces problem->cu), or NULL */
     int32_t cones_per_instance; /* 0: the handle's cx / cu (every zero-initialised batch); 1: the arrays above */
     int32_t reserved3;          /* must be 0 */
+    /* Per-instance static hyperplanes (optional): instance b projects its static linear constraints with its own Alin_x,
+     * blin_x, Alin_u, blin_u, as a TinySolver whose tiny_set_linear_constraints got them would.  The hyperplane structure
+     * (num_state_linear, num_input_linear, en_state_linear, en_input_linear), the time-varying hyperplanes, the cones, the
+     * bounds and the model stay the handle's.  Arrays of the problem dtype, each instance's matrix column-major as in
+     * tinympc_problem_t.  A row a = 0, b = 0 never projects, so an instance with fewer planes pads its rows with zeros.  With
+     * planes_per_instance = 1 a side whose static hyperplane loop runs (en_state_linear / en_input_linear set and the handle
+     * has rows on that side) needs both pointers of its pair (else TINYMPC_ERR_ARG); a side whose loop does not run is never
+     * read, and when neither runs the solve is the one without per-instance planes.  Any other mode value or a non-zero
+     * reserved4 return TINYMPC_ERR_ARG.  DEVICE pointers for tinympc_b200_solve, HOST pointers (staged per chunk) for
+     * tinympc_b200_solve_host.  Served by the streamed (GPS) kernel, the one that runs hyperplanes, with two instances per
+     * lane group where the shared solve has two; combines with models only.  STRICT only: FAST mode, explicit TPI, adaptive
+     * rho, rollouts and per-instance bounds or cones in the same batch return TINYMPC_ERR_UNSUPPORTED. */
+    const void *Alin_x;   /* [B][nx][num_state_linear]: instance b's Alin_x, column-major like tinympc_problem_t.Alin_x */
+    const void *blin_x;   /* [B][num_state_linear] */
+    const void *Alin_u;   /* [B][nu][num_input_linear] */
+    const void *blin_u;   /* [B][num_input_linear] */
+    int32_t planes_per_instance; /* 0: the handle's hyperplanes; 1: the arrays above */
+    int32_t reserved4;           /* must be 0 */
 } tinympc_batch_t;
 
 typedef struct tinympc_b200_solver tinympc_b200_solver_t;

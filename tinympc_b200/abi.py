@@ -73,6 +73,8 @@ class Batch(C.Structure):
         ("bounds_per_instance", C.c_int32), ("reserved2", C.c_int32),
         ("cone_x_mu", vp), ("cone_u_mu", vp),
         ("cones_per_instance", C.c_int32), ("reserved3", C.c_int32),
+        ("Alin_x", vp), ("blin_x", vp), ("Alin_u", vp), ("blin_u", vp),
+        ("planes_per_instance", C.c_int32), ("reserved4", C.c_int32),
     ]
 
 

@@ -73,11 +73,51 @@ def cones_check(cones: dict, B: int, ncx: int, ncu: int, dtype) -> None:
                              f"got {list(a.shape)}")
 
 
+PLANE_NAMES = ("Alin_x", "blin_x", "Alin_u", "blin_u")
+
+
+def planes_check(planes: dict, B: int, nlx: int, nlu: int, nx: int, nu: int, dtype) -> None:
+    """Check per-instance static hyperplanes (a dict with Alin_x [B, nlx, nx] and blin_x [B, nlx] for the state side and / or
+    Alin_u [B, nlu, nu] and blin_u [B, nlu] for the input side, rows as a TinySolver's tiny_set_linear_constraints takes them;
+    numpy arrays or torch tensors of the problem dtype) against a batch of B instances of a problem with nlx state and nlu
+    input hyperplanes (tinympc_batch_t.Alin_x ... blin_u).  A side may be absent when its static hyperplane loop does not run."""
+    unknown = set(planes) - set(PLANE_NAMES)
+    if unknown:
+        raise ValueError(f"planes: unknown keys {sorted(unknown)}; expected any of {PLANE_NAMES}")
+    given = {k: v for k, v in planes.items() if v is not None}
+    if not given:
+        raise ValueError("planes: give Alin_x / blin_x, Alin_u / blin_u or both pairs")
+    for a, b in (("Alin_x", "blin_x"), ("Alin_u", "blin_u")):
+        if (a in given) != (b in given):
+            raise ValueError(f"planes: {a} and {b} are given in pairs")
+    want = np.dtype(dtype)
+    shapes = dict(Alin_x=(B, nlx, nx), blin_x=(B, nlx), Alin_u=(B, nlu, nu), blin_u=(B, nlu))
+    for k, a in given.items():
+        dt = a.dtype if hasattr(a, "dtype") else None
+        if dt is None or str(dt).replace("torch.", "") != want.name:
+            raise ValueError(f"planes: {k} must have the problem dtype {want.name}, got {dt}")
+        if tuple(a.shape) != shapes[k]:
+            raise ValueError(f"planes: {k} must be {list(shapes[k])} (one set of the problem's hyperplane rows per instance), "
+                             f"got {list(a.shape)}")
+
+
+def planes_abi(planes: dict) -> dict:
+    """the given arrays of a checked planes dict with each instance's matrix in the ABI's column-major order ([B, n, nx] ->
+    a [B, nx, n] view; numpy arrays or torch tensors, made contiguous by the caller)"""
+    return {k: (v.swapaxes(1, 2) if k.startswith("Alin") else v) for k, v in planes.items() if v is not None}
+
+
+def num_planes(prob: MPCProblem) -> tuple:
+    """(state, input) static hyperplane rows of a problem"""
+    return (0 if prob.Alin_x is None else prob.Alin_x.shape[0], 0 if prob.Alin_u is None else prob.Alin_u.shape[0])
+
+
 class HostBatch:
     """Owns the numpy buffers of one batched solve and the ctypes struct pointing at them."""
 
     def __init__(self, prob: MPCProblem, x0, Xref, Uref=None, state: dict | None = None, cold_start=True,
-                 want_state=(), want_residuals=True, models=None, bounds: dict | None = None, cones: dict | None = None):
+                 want_state=(), want_residuals=True, models=None, bounds: dict | None = None, cones: dict | None = None,
+                 planes: dict | None = None):
         dt = prob.dtype
         nx, nu, N = prob.nx, prob.nu, prob.N
         self.prob = prob
@@ -117,6 +157,11 @@ class HostBatch:
         if cones is not None:
             cones_check(cones, B, len(prob.Acx), len(prob.Acu), dt)
             self.cones = {k: np.ascontiguousarray(v) for k, v in cones.items() if v is not None}
+        # per-instance static hyperplanes (see planes_check), each matrix column-major; planes_per_instance 0 = the problem's
+        self.planes = None
+        if planes is not None:
+            planes_check(planes, B, *num_planes(prob), nx, nu, dt)
+            self.planes = {k: np.ascontiguousarray(v) for k, v in planes_abi(planes).items()}
         self.sol_x = np.zeros((B, N, nx), dtype=dt)
         self.sol_u = np.zeros((B, N - 1, nu), dtype=dt)
         self.iter = np.zeros(B, dtype=np.int32)
@@ -147,6 +192,10 @@ class HostBatch:
             b.cones_per_instance = 1
             for k, a in self.cones.items():
                 setattr(b, "cone_" + k, a.ctypes.data)
+        if self.planes is not None:
+            b.planes_per_instance = 1
+            for k, a in self.planes.items():
+                setattr(b, k, a.ctypes.data)
         b._owner = self
         return b
 

@@ -15,7 +15,7 @@ import ctypes as C
 
 from . import abi
 from ._lib import check
-from .batch import bounds_layout, cones_check
+from .batch import bounds_layout, cones_check, num_planes, planes_abi, planes_check
 from .solver import AdaptiveRho, BatchedTinySolver, pack_models
 
 # box-constrained warm start: slacks + duals (+ the previous-iteration slacks v, z, which only feed the dual residual of
@@ -28,7 +28,8 @@ WARM_FIELDS_FAST = ("vnew", "znew", "g", "y")
 
 class DeviceMPCLoop:
     def __init__(self, solver: BatchedTinySolver, x0, reset_duals: bool = False, extra_state=(), exact_first_residual: bool = True,
-                 adaptive_rho: AdaptiveRho | None = None, models=None, bounds: dict | None = None, cones: dict | None = None):
+                 adaptive_rho: AdaptiveRho | None = None, models=None, bounds: dict | None = None, cones: dict | None = None,
+                 planes: dict | None = None):
         """models ([B, blob], tinympc_batch_t.models, e.g. from setup_models): a heterogeneous fleet, one model, cache and rho
         per plant.  Every step solves with them and advances plant b with its own A, B, f (tinympc_b200_advance_models).
         adaptive_rho: every plant adapts its own rho / Kinf / Pinf, kept on the device across steps in self.models
@@ -37,7 +38,10 @@ class DeviceMPCLoop:
         bounds: per-instance box bounds of every plant (a dict as in BatchedTinySolver.solve), kept on the device across steps
         in self.bounds; step(..., bounds=...) replaces them for one step (a moving corridor).
         cones: per-instance cone coefficients of every plant (a dict as in BatchedTinySolver.solve), kept on the device across
-        steps in self.cones; step(..., cones=...) replaces them for one step."""
+        steps in self.cones; step(..., cones=...) replaces them for one step.
+        planes: per-instance static hyperplanes of every plant (a dict as in BatchedTinySolver.solve), converted to the ABI's
+        column-major layout once and kept on the device across steps in self.planes; step(..., planes=...) replaces them for one
+        step (a moving obstacle's fresh half-space)."""
         import torch
 
         self.solver = solver
@@ -60,6 +64,7 @@ class DeviceMPCLoop:
                                             adaptive_rho.rho_max, adaptive_rho.enable_clipping)
         self.bounds = None if bounds is None else self._device_bounds(bounds)
         self.cones = None if cones is None else self._device_cones(cones)
+        self.planes = None if planes is None else self._device_planes(planes)
         self.models = None
         if adaptive_rho is not None or models is not None:
             m = pack_models(p, self.B) if models is None else models
@@ -79,10 +84,24 @@ class DeviceMPCLoop:
         cones_check(cones, self.B, len(p.Acx), len(p.Acu), p.dtype)
         return {k: torch.as_tensor(v, device=self.dev).contiguous() for k, v in cones.items() if v is not None}
 
-    def step(self, Xref, Uref=None, stream=None, bounds=None, cones=None):
+    def _device_planes(self, planes):
+        import torch
+
+        p = self.solver.problem
+        planes_check(planes, self.B, *num_planes(p), p.nx, p.nu, p.dtype)
+        # each matrix is kept column-major ([B, nx, n] contiguous) and handed on as its [B, n, nx] view, which
+        # make_device_batch uses in place
+        out = {}
+        for k, v in planes_abi(planes).items():
+            a = torch.as_tensor(v, device=self.dev).contiguous()
+            out[k] = a.swapaxes(1, 2) if k.startswith("Alin") else a
+        return out
+
+    def step(self, Xref, Uref=None, stream=None, bounds=None, cones=None, planes=None):
         """One MPC step for every instance: solve (warm-started), then advance the plants.  Returns the output dict
         (device tensors: sol_x, sol_u, iter, solved, residuals and the state fields).  bounds: per-instance box bounds for this
-        step only, in place of the loop's; cones: per-instance cone coefficients for this step only, likewise."""
+        step only, in place of the loop's; cones: per-instance cone coefficients for this step only, likewise; planes:
+        per-instance static hyperplanes for this step only, likewise."""
         import torch
 
         s = self.solver
@@ -92,7 +111,8 @@ class DeviceMPCLoop:
         het = self.models is not None and self.adaptive_rho is None
         batch, out = s.make_device_batch(self.x0, Xref, Uref, state=self.state, cold_start=self._first, want_state=self.fields,
                                          want_u0=True, want_solution=self.want_solution, models=self.models if het else None,
-                                         bounds=self.bounds if bounds is None else bounds, cones=self.cones if cones is None else cones)
+                                         bounds=self.bounds if bounds is None else bounds, cones=self.cones if cones is None else cones,
+                                         planes=self.planes if planes is None else planes)
         if self.adaptive_rho is None:
             s.solve_device(batch, stream)
         else:
@@ -124,6 +144,8 @@ class DeviceMPCLoop:
             raise ValueError("rollout: per-instance bounds are not available in a rollout; use step()")
         if self.cones is not None:
             raise ValueError("rollout: per-instance cones are not available in a rollout; use step()")
+        if self.planes is not None:
+            raise ValueError("rollout: per-instance hyperplanes are not available in a rollout; use step()")
         if len(self.fields) != len(WARM_FIELDS if "v" in self.fields else WARM_FIELDS_FAST):
             raise ValueError("rollout: covers box constraints only (no extra_state); use step()")
         T = int(T)

@@ -155,6 +155,12 @@ tmpc::Features features(const tinympc_b200_solver *s) {
     return f;
 }
 
+// the static hyperplane loops that run and read their coefficients (enabled, with rows): bit 0 state side, bit 1 input side
+int plane_sides(const tinympc_b200_solver *s) {
+    const tmpc::Features ft = features(s);
+    return (ft.lin_x && s->pd.nlx > 0 ? 1 : 0) | (ft.lin_u && s->pd.nlu > 0 ? 2 : 0);
+}
+
 // The checks of a solve before it is planned: the handle's state, then the arguments (ar: adaptive rho, or null).  Their
 // order decides which error a caller sees.
 int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
@@ -181,6 +187,15 @@ int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const t
             return fail(TINYMPC_ERR_ARG, "per-instance cones: en_state_soc / en_input_soc set on a side with cones but the batch has no "
                                          "cone_x_mu / cone_u_mu for it");
     }
+    if ((io->planes_per_instance != 0 && io->planes_per_instance != 1) || io->reserved4 != 0)
+        return fail(TINYMPC_ERR_ARG, "planes_per_instance must be 0 (the handle's hyperplanes) or 1 (Alin_x / blin_x / Alin_u / blin_u per "
+                                     "instance), and reserved4 must be 0");
+    if (io->planes_per_instance) {  // a side whose static hyperplane loop runs needs its pair; the other side's is never read
+        const int sides = plane_sides(s);
+        if (((sides & 1) && (!io->Alin_x || !io->blin_x)) || ((sides & 2) && (!io->Alin_u || !io->blin_u)))
+            return fail(TINYMPC_ERR_ARG, "per-instance hyperplanes: en_state_linear / en_input_linear set on a side with rows but the "
+                                         "batch has no Alin_x / blin_x or Alin_u / blin_u for it");
+    }
     if (st.check_termination <= 0) return fail(TINYMPC_ERR_ARG, "check_termination must be >= 1");
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
     if (ar && io->models) return fail(TINYMPC_ERR_ARG, "adaptive rho: the model blobs go in tinympc_adaptive_rho_t.models (in/out); io->models must be NULL");
@@ -203,13 +218,23 @@ struct SolvePlan {
 size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->pd.nx, s->pd.nu, esize(s->pd.dtype)); }
 
 // The plan of a solve of B instances (models: per-instance models; bounds: per-instance box bounds; cones: per-instance cone
-// coefficients, cones_per_instance set; adapt: adaptive rho).
+// coefficients, cones_per_instance set; planes: per-instance static hyperplanes, planes_per_instance set; adapt: adaptive rho).
 // GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed
 // (everything else the lane mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature
 // cannot be served.
-int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cones, bool adapt, int64_t B, SolvePlan *p,
+int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cones, bool planes, bool adapt, int64_t B, SolvePlan *p,
                bool rollout = false) {
     const tmpc::Features ft = features(s);
+    if (planes) {  // per-instance static hyperplanes have STRICT variants of the streamed kernel only, alone or with models
+        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's hyperplanes (planes_per_instance must be 0)");
+        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's hyperplanes (planes_per_instance must be 0)");
+        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes are available in STRICT mode only");
+        if (s->family == TINYMPC_KERNEL_TPI)
+            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes run on the streamed lane-group kernel (GPS), not on one thread per instance");
+        if (bounds || cones)
+            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes do not combine with per-instance bounds or cones in one batch");
+    }
+    const bool planes_run = planes && plane_sides(s) != 0;  // else the coefficients are never read: the plan without them
     if (cones) {  // per-instance cone coefficients have STRICT variants of the streamed kernel only
         if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's cone coefficients (cones_per_instance must be 0)");
         if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's cone coefficients (cones_per_instance must be 0)");
@@ -297,6 +322,9 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cone
     // rules above chose (alone: the shared solve's, whose chunks are not rounded; with models or bounds: gps_het_slots)
     if (cones_run && p->family != TINYMPC_KERNEL_GPS)
         return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones: this problem needs the streamed lane-group kernel, which does not cover this shape");
+    // likewise a static hyperplane loop: its GPS_PLANES variants keep the shared solve's plan, or gps_het_slots with models
+    if (planes_run && p->family != TINYMPC_KERNEL_GPS)
+        return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes: this problem needs the streamed lane-group kernel, which does not cover this shape");
     if (p->family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
     return 0;
 }
@@ -378,8 +406,8 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
             const tinympc_adaptive_rho_t *ar = nullptr, const tinympc_rollout_t *ro = nullptr) {
     SolvePlan plan;
     if (ar || ro || io->B > 0)  // an adaptive solve or a rollout is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0, ar != nullptr, io->B,
-                                &plan, ro != nullptr))
+        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0,
+                                io->planes_per_instance != 0, ar != nullptr, io->B, &plan, ro != nullptr))
             return rc;
     if (io->B <= 0 || (ro && ro->T == 0)) return TINYMPC_OK;
     const int family = plan.family;
@@ -396,6 +424,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     d.max_smem_optin = s->max_smem_optin;
     d.bounds = io->bounds_per_instance;
     d.cones = io->cones_per_instance && (d.ft.soc_x || d.ft.soc_u);
+    d.planes = io->planes_per_instance && plane_sides(s) != 0;
     if (ar) {
         if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, io->models, stream)
                                                 : upload_adaptive<float>(s, ar, io->models, stream))
@@ -918,7 +947,8 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     chunk = (chunk + 31) / 32 * 32;
     SolvePlan plan;  // of a chunk
     if (ar || B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0, ar != nullptr, chunk, &plan))
+        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0,
+                                io->planes_per_instance != 0, ar != nullptr, chunk, &plan))
             return rc;
     if (B <= 0) return TINYMPC_OK;
     const size_t es = esize(s->pd.dtype);
@@ -972,6 +1002,22 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
         else dev.cone_x_mu = nullptr;
         if (ft.soc_u) fields.push_back({io->cone_u_mu, nullptr, es * s->pd.ncu, true, false, (void **)&dev.cone_u_mu});
         else dev.cone_u_mu = nullptr;
+    }
+    if (io->planes_per_instance) {  // sliced per chunk like the cones; a side whose static hyperplane loop does not run is never read
+        const int sides = plane_sides(s);
+        const size_t nlx = s->pd.nlx, nlu = s->pd.nlu;
+        if (sides & 1) {
+            fields.push_back({io->Alin_x, nullptr, es * s->pd.nx * nlx, true, false, (void **)&dev.Alin_x});
+            fields.push_back({io->blin_x, nullptr, es * nlx, true, false, (void **)&dev.blin_x});
+        } else {
+            dev.Alin_x = dev.blin_x = nullptr;
+        }
+        if (sides & 2) {
+            fields.push_back({io->Alin_u, nullptr, es * s->pd.nu * nlu, true, false, (void **)&dev.Alin_u});
+            fields.push_back({io->blin_u, nullptr, es * nlu, true, false, (void **)&dev.blin_u});
+        } else {
+            dev.Alin_u = dev.blin_u = nullptr;
+        }
     }
     if (ar && ar->tables_per_instance) {  // sliced per chunk like the models
         fields.push_back({ar->dKinf_drho, nullptr, es * s->pd.nu * s->pd.nx, true, false, (void **)&args.ar.dKinf_drho});

@@ -212,7 +212,13 @@ constexpr int GPS_BOUNDS = 16;
 // (instance, side) pair, so a lane reads the coefficients of one slot and one side only: they stay out of registers, and
 // the kernel keeps the NI of the shared solve (two instances per lane group where the shared model runs two).
 constexpr int GPS_CONES = 32;
-constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS | GPS_CONES;  // the family-mask bits that are not constraint families
+// Per-instance static hyperplanes (tinympc_batch_t.planes_per_instance): GPS_PLANES added to a family mask with static
+// hyperplanes (6, 7), alone or with GPS_HET.  P.Alin_x / blin_x / Alin_u / blin_u point at the batch's [B][nx][nlx] / [B][nlx] /
+// [B][nu][nlu] / [B][nlu] arrays, and planes_x / planes_u add the slot's instance offset.  project_rows reads the coefficients
+// from memory row by row and never holds them in registers, so the per-slot cost is a pointer and the kernel keeps the NI of
+// the shared solve.
+constexpr int GPS_PLANES = 64;
+constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS | GPS_CONES | GPS_PLANES;  // the family-mask bits that are not constraint families
 
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
@@ -220,10 +226,13 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     constexpr bool HET = (FAMH & GPS_HET) != 0;     // per-instance models
     constexpr bool BND = (FAMH & GPS_BOUNDS) != 0;  // per-instance box bounds
     constexpr bool CN = (FAMH & GPS_CONES) != 0;    // per-instance cone coefficients
+    constexpr bool PL = (FAMH & GPS_PLANES) != 0;   // per-instance static hyperplanes
     constexpr int FAM = FAMH & ~GPS_VARIANTS;       // constraint families compiled in
     static_assert(!HET || NI == 1, "per-instance models run one instance per lane group");
     static_assert(!BND || (NI == 1 && !FAST), "per-instance bounds run one instance per lane group, in STRICT mode");
     static_assert(!CN || ((FAM & 1) != 0 && !FAST), "per-instance cone coefficients need the cone family, in STRICT mode");
+    static_assert(!PL || ((FAM & 2) != 0 && !FAST && !BND && !CN),
+                  "per-instance hyperplanes need the static hyperplane family, in STRICT mode, without per-instance bounds or cones");
     using Cfg = GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAM>;
     using REC = GpsRec<NX, NU, Cfg::SPW, (int)sizeof(T), FAM>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -503,25 +512,37 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
         }
     };
     // hyperplanes (admm.cpp:138-211): the rows are applied one after the other to the whole column, so every lane of
-    // the group carries the full vector through the sequence (same arithmetic on every lane) and keeps its own rows
-    auto planes_x = [&](T (&own)[NI][RX], const T *A, int ld, int row0, int n, const T *bvec) {
+    // the group carries the full vector through the sequence (same arithmetic on every lane) and keeps its own rows.
+    // pi = IntTag<1>: per-instance planes (GPS_PLANES static family), instance j's n rows start n * NX (n * NU) coefficients
+    // and n offsets further per instance; a slot that never got an instance reads instance 0's, as xref_of does.
+    auto planes_x = [&](auto pi, T (&own)[NI][RX], const T *A, int ld, int row0, int n, const T *bvec) {
         T full[NI][NX];
         gather_x(own, full);
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
-            project_rows<FAST, T, NX>(full[j], A, ld, row0, n, bvec);
+            if constexpr (decltype(pi)::value != 0) {
+                const int64_t ib = inst[j] < 0 ? 0 : inst[j];
+                project_rows<FAST, T, NX>(full[j], A + ib * n * NX, ld, row0, n, bvec + ib * n);
+            } else {
+                project_rows<FAST, T, NX>(full[j], A, ld, row0, n, bvec);
+            }
             T o[RX];
             extract_own<T, NX, RX, L>(full[j], l, o);
 #pragma unroll
             for (int a = 0; a < RX; ++a) own[j][a] = xvl ? o[a] : own[j][a];
         }
     };
-    auto planes_u = [&](T (&own)[NI][RU], const T *A, int ld, int row0, int n, const T *bvec) {
+    auto planes_u = [&](auto pi, T (&own)[NI][RU], const T *A, int ld, int row0, int n, const T *bvec) {
         T full[NI][NU];
         gather_u(own, full);
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
-            project_rows<FAST, T, NU>(full[j], A, ld, row0, n, bvec);
+            if constexpr (decltype(pi)::value != 0) {
+                const int64_t ib = inst[j] < 0 ? 0 : inst[j];
+                project_rows<FAST, T, NU>(full[j], A + ib * n * NU, ld, row0, n, bvec + ib * n);
+            } else {
+                project_rows<FAST, T, NU>(full[j], A, ld, row0, n, bvec);
+            }
             T o[RU];
             extract_own<T, NU, RU, L>(full[j], l, o);
 #pragma unroll
@@ -556,6 +577,7 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
                              const T (&u)[NI][RU], T (&q)[NI][RX], T (&r)[NI][RU]) {
         constexpr int F = decltype(ftag)::value;
         constexpr int FSEL_ = F;
+        constexpr IntTag<(PL && F == 1) ? 1 : 0> pi{};  // per-instance static hyperplanes
         if (fx[F]) {
             T gf[NI][RX], sf[NI][RX];
 #pragma unroll
@@ -564,8 +586,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
                 for (int a = 0; a < RX; ++a) sf[j][a] = xo[j][a] + gf[j][a];
             }
-            if (F == 1) planes_x(sf, P.Alin_x, P.nlx, 0, P.nlx, P.blin_x);
-            else planes_x(sf, P.tv_Alin_x, P.ntvx * N, P.ntvx * k, P.ntvx, P.tv_blin_x + (int64_t)k * P.ntvx);
+            if (F == 1) planes_x(pi, sf, P.Alin_x, P.nlx, 0, P.nlx, P.blin_x);
+            else planes_x(pi, sf, P.tv_Alin_x, P.ntvx * N, P.ntvx * k, P.ntvx, P.tv_blin_x + (int64_t)k * P.ntvx);
 #pragma unroll
             for (int j = 0; j < NI; ++j) {
                 T gfn[RX];
@@ -586,8 +608,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
 #pragma unroll
                 for (int b = 0; b < RU; ++b) sf[j][b] = u[j][b] + yf[j][b];
             }
-            if (F == 1) planes_u(sf, P.Alin_u, P.nlu, 0, P.nlu, P.blin_u);
-            else planes_u(sf, P.tv_Alin_u, P.ntvu * (N - 1), P.ntvu * k, P.ntvu, P.tv_blin_u + (int64_t)k * P.ntvu);
+            if (F == 1) planes_u(pi, sf, P.Alin_u, P.nlu, 0, P.nlu, P.blin_u);
+            else planes_u(pi, sf, P.tv_Alin_u, P.ntvu * (N - 1), P.ntvu * k, P.ntvu, P.tv_blin_u + (int64_t)k * P.ntvu);
 #pragma unroll
             for (int j = 0; j < NI; ++j) {
                 T yfn[RU];
@@ -1193,8 +1215,8 @@ inline GpsPlan gps_plan_L(const LaunchDesc &d) {
     return p;
 }
 
-// FAMH: family mask, plus GPS_HET for per-instance models, GPS_BOUNDS for per-instance bounds and GPS_CONES for per-instance
-// cone coefficients
+// FAMH: family mask, plus GPS_HET for per-instance models, GPS_BOUNDS for per-instance bounds, GPS_CONES for per-instance
+// cone coefficients and GPS_PLANES for per-instance static hyperplanes
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     const GpsPlan plan = gps_plan_L<T, NX, NU, L, NI, FAMH>(*d);
@@ -1221,6 +1243,24 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     } else {
         constexpr int NI = gps_pick_NI<T, NX, NU, L>();
         const int fam = gps_family_mask(d->ft.soc_x || d->ft.soc_u, d->ft.lin_x || d->ft.lin_u || d->ft.tvl_x || d->ft.tvl_u);
+        if (d->planes) {  // per-instance static hyperplanes (STRICT; a static hyperplane loop runs, so the mask is 6 or 7; no
+                          // per-instance bounds or cones): the shared solve's NI alone, one instance per lane group with models
+            if constexpr (FAST) {
+                return TINYMPC_ERR_UNSUPPORTED;
+            } else {
+                if (d->bounds || d->cones) return TINYMPC_ERR_UNSUPPORTED;
+                const bool het = d->io.models != nullptr;
+#define TM_GPS_PL_CASE(FF)                                                                        \
+    if (fam == FF) {                                                                              \
+        if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_PLANES | GPS_HET, false>(d, P0); \
+        return launch_gps_cfg<T, NX, NU, L, NI, FF | GPS_PLANES, false>(d, P0);                   \
+    }
+                TM_GPS_PL_CASE(6)
+                TM_GPS_PL_CASE(7)
+#undef TM_GPS_PL_CASE
+                return TINYMPC_ERR_UNSUPPORTED;
+            }
+        }
         if (d->cones) {  // per-instance cone coefficients (STRICT; a cone loop runs, so the mask is 1 or 7): the shared solve's NI
                          // on their own, one instance per lane group with per-instance models or bounds
             if constexpr (FAST) {

@@ -47,7 +47,7 @@ int launch_tpi(LaunchDesc *d) {
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->io.models || d->bounds || d->cones) return TINYMPC_ERR_UNSUPPORTED;  // per-instance data: the lane-group kernels only
+    if (d->io.models || d->bounds || d->cones || d->planes) return TINYMPC_ERR_UNSUPPORTED;  // per-instance data: the lane-group kernels only
     if (d->ft.ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
     return d->fast ? launch_tpi<T, true, false>(d) : launch_tpi<T, false, false>(d);
 }

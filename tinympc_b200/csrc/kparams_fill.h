@@ -120,6 +120,9 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
         P.w_vc = const_cast<void *>(d.io.cone_x_mu);
         P.w_zc = const_cast<void *>(d.io.cone_u_mu);
     }
+    if (d.planes) {  // per-instance static hyperplanes replace the problem's; the kernel adds the slot's instance offset
+        P.Alin_x = (const T *)io.Alin_x; P.blin_x = (const T *)io.blin_x; P.Alin_u = (const T *)io.Alin_u; P.blin_u = (const T *)io.blin_u;
+    }
 }
 
 }  // namespace tmpc

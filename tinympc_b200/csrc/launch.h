@@ -72,6 +72,9 @@ struct LaunchDesc {
     // per-instance cone coefficients (io.cones_per_instance) with a cone loop that runs: io.cone_x_mu / cone_u_mu hold [B][ncx] /
     // [B][ncu].  The streamed kernel's GPS_CONES variants read them.
     int cones;
+    // per-instance static hyperplanes (io.planes_per_instance) with a static hyperplane loop that runs: io.Alin_x / blin_x /
+    // Alin_u / blin_u hold [B][nx][nlx] / [B][nlx] / [B][nu][nlu] / [B][nlu].  The streamed kernel's GPS_PLANES variants read them.
+    int planes;
 
     cudaStream_t stream;
     int sm_count;

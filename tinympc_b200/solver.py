@@ -19,7 +19,7 @@ import numpy as np
 
 from . import abi
 from ._lib import check, load
-from .batch import BOUND_NAMES, CONE_NAMES, HostBatch, bounds_layout, cones_check
+from .batch import BOUND_NAMES, CONE_NAMES, PLANE_NAMES, HostBatch, bounds_layout, cones_check, num_planes, planes_abi, planes_check
 from .problem import MPCProblem, copy_settings, default_settings, dtype_code
 from .workloads import ModelSpec
 
@@ -219,7 +219,8 @@ class BatchedTinySolver:
 
     # ---- host buffers (numpy): the call a reference user would make; H2D/D2H inside ------------------
     def solve(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), models=None,
-              adaptive_rho: AdaptiveRho | None = None, bounds: dict | None = None, cones: dict | None = None) -> dict:
+              adaptive_rho: AdaptiveRho | None = None, bounds: dict | None = None, cones: dict | None = None,
+              planes: dict | None = None) -> dict:
         """With adaptive_rho: every instance adapts its own rho / Kinf / Pinf, starting from its blob in `models` (default:
         the problem's own cache, pack_models); the result's "models" holds the adapted blobs, the start of the next solve.
         bounds: per-instance box bounds in place of the problem's, a dict with any of x_min, x_max, u_min, u_max of the
@@ -227,15 +228,19 @@ class BatchedTinySolver:
         a side may be absent when its bound is disabled (tinympc_batch_t.bounds_per_instance).
         cones: per-instance cone coefficients in place of the problem's cx / cu, a dict with x_mu [B, num state cones] and / or
         u_mu [B, num input cones] of the problem dtype; a side may be absent when its cone loop does not run
-        (tinympc_batch_t.cones_per_instance)."""
+        (tinympc_batch_t.cones_per_instance).
+        planes: per-instance static hyperplanes in place of the problem's, a dict with Alin_x [B, nlx, nx] / blin_x [B, nlx]
+        and / or Alin_u [B, nlu, nu] / blin_u [B, nlu] of the problem dtype (rows as tiny_set_linear_constraints takes them;
+        nlx, nlu: the problem's row counts); a side may be absent when its static hyperplane loop does not run
+        (tinympc_batch_t.planes_per_instance)."""
         if adaptive_rho is None:
             hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, models=models,
-                           bounds=bounds, cones=cones)
+                           bounds=bounds, cones=cones, planes=planes)
             cb = hb.to_c()
             check(self._lib.tinympc_b200_solve_host(self._h, C.byref(cb)))
             return hb.result()
         hb = HostBatch(self.problem, x0, Xref, Uref, state=state, cold_start=cold_start, want_state=want_state, bounds=bounds,
-                       cones=cones)
+                       cones=cones, planes=planes)
         m = pack_models(self.problem, hb.B) if models is None else np.array(models, dtype=self.problem.dtype).reshape(hb.B, -1)
         cb, ar = hb.to_c(), adaptive_rho.to_c(self.problem, m.ctypes.data, hb.B)
         check(self._lib.tinympc_b200_solve_adaptive_host(self._h, C.byref(cb), C.byref(ar)))
@@ -301,10 +306,12 @@ class BatchedTinySolver:
 
     # ---- device buffers (torch tensors on cuda:<device>) ---------------------------------------------
     def make_device_batch(self, x0, Xref, Uref=None, state=None, cold_start=True, want_state=(), want_residuals=True,
-                          want_u0=False, want_solution=True, models=None, bounds: dict | None = None, cones: dict | None = None):
+                          want_u0=False, want_solution=True, models=None, bounds: dict | None = None, cones: dict | None = None,
+                          planes: dict | None = None):
         """Allocate/adopt torch CUDA tensors and build the device-pointer tinympc_batch_t.  bounds: per-instance box bounds,
-        cones: per-instance cone coefficients, both as in solve(); torch CUDA tensors of the problem dtype are used in place,
-        numpy arrays are uploaded."""
+        cones: per-instance cone coefficients, planes: per-instance static hyperplanes, all as in solve(); torch CUDA tensors
+        of the problem dtype are used in place (a plane matrix that is the [B, n, nx] view of a contiguous [B, nx, n] tensor
+        too), numpy arrays are uploaded."""
         import torch
 
         p = self.problem
@@ -366,6 +373,13 @@ class BatchedTinySolver:
             for k in CONE_NAMES:
                 setattr(b, "cone_" + k, ct[k].data_ptr() if k in ct else None)
             tens["cones"] = ct
+        if planes is not None:
+            planes_check(planes, B, *num_planes(p), p.nx, p.nu, p.dtype)
+            pt = {k: t(v) for k, v in planes_abi(planes).items()}
+            b.planes_per_instance = 1
+            for k in PLANE_NAMES:
+                setattr(b, k, pt[k].data_ptr() if k in pt else None)
+            tens["planes"] = pt
         b.iter, b.solved = out["iter"].data_ptr(), out["solved"].data_ptr()
         b.residuals = None if out["residuals"] is None else out["residuals"].data_ptr()
         res = dict(out)

@@ -105,6 +105,26 @@ def cone_fleet(spec: ModelSpec, B, seed=0, scale=(0.6, 1.0), dtype=np.float64) -
     return dict(x_mu=x_mu.astype(dtype), u_mu=u_mu.astype(dtype))
 
 
+def plane_fleet(spec: ModelSpec, B, seed=0, tilt=0.25, shift=(-0.3, 0.1), dtype=np.float64) -> dict:
+    """Per-robot static hyperplanes for a fleet of B robots of `spec` (a spec with Alin_x / blin_x and / or Alin_u / blin_u
+    constraints): robot b's row i is the spec's row i with every non-zero coefficient scaled by its own factor from
+    U(1 - tilt, 1 + tilt) and its offset moved by U(shift), e.g. a separating half-space per robot from the obstacle that
+    robot sees.  The default shift tightens most rows, so most robots meet an active row.  -> dict(Alin_x [B, nlx, nx],
+    blin_x [B, nlx], Alin_u [B, nlu, nu], blin_u [B, nlu]) of `dtype` (the sides the spec has), the `planes=` argument of
+    BatchedTinySolver.solve / make_device_batch / DeviceMPCLoop."""
+    rng = np.random.default_rng(seed)
+    out = {}
+    for side in ("x", "u"):
+        A = spec.constraints.get("Alin_" + side)
+        if A is None:
+            continue
+        A = np.asarray(A, dtype=np.float64)
+        b = np.asarray(spec.constraints["blin_" + side], dtype=np.float64).reshape(-1)
+        out["Alin_" + side] = (A[None] * rng.uniform(1.0 - tilt, 1.0 + tilt, size=(B,) + A.shape)).astype(dtype)
+        out["blin_" + side] = (b[None] + rng.uniform(*shift, size=(B, b.size))).astype(dtype)
+    return out
+
+
 def random_lti(nx, nu, N, seed=0) -> ModelSpec:
     """SURVEY §8d C5 generator: A = I + 0.05 G rescaled to spectral radius 1, B ~ N(0, 0.1^2)."""
     rng = np.random.default_rng(1000003 * seed + 7919 * nx + 104729 * nu)
