@@ -3,6 +3,7 @@
 // settings->adaptive_rho one tinympc_b200_solve_adaptive_host() call.
 #include "tinympc_shim.hpp"
 
+#include <algorithm>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -74,7 +75,9 @@ uint64_t fingerprint(const TinySolver *s, bool adaptive) {
     const TinyWorkspace *w = s->work;
     const TinyCache *c = s->cache;
     uint64_t h = 1469598103934665603ULL;
-    int dims[4] = {w->nx, w->nu, w->N, (int)adaptive};
+    // the counts key the handle too: a program may lower one directly and keep its matrices (the reference loops to the counts)
+    int dims[10] = {w->nx, w->nu, w->N, (int)adaptive, w->numStateCones, w->numInputCones, w->numStateLinear, w->numInputLinear,
+                    w->numtvStateLinear, w->numtvInputLinear};
     h = fnv(h, dims, sizeof(dims));
     if (!adaptive) h = fnv(h, &c->rho, sizeof(c->rho));
     h = fnv_m(h, w->Adyn); h = fnv_m(h, w->Bdyn); h = fnv_m(h, w->fdyn); h = fnv_m(h, w->Q); h = fnv_m(h, w->R);
@@ -95,6 +98,35 @@ const void *ptr(const M &m) {
     return m.size() ? static_cast<const void *>(m.data()) : nullptr;
 }
 
+// A count the program raised above the rows of its arrays, on a family a solve would run: the reference would read past
+// them, so the solve is refused instead.  (With the family switched off the reference never reads them.)
+int check_counts(const TinySolver *s) {
+    const TinyWorkspace *w = s->work;
+    const TinySettings *t = s->settings;
+    const long N = w->N;
+    const char *bad = nullptr;
+    if (t->en_state_soc && (w->numStateCones > w->Acx.size() || w->numStateCones > w->qcx.size() || w->numStateCones > w->cx.size()))
+        bad = "numStateCones";
+    else if (t->en_input_soc && (w->numInputCones > w->Acu.size() || w->numInputCones > w->qcu.size() || w->numInputCones > w->cu.size()))
+        bad = "numInputCones";
+    else if (t->en_state_linear && (w->numStateLinear > w->Alin_x.rows() || w->numStateLinear > w->blin_x.size()))
+        bad = "numStateLinear";
+    else if (t->en_input_linear && (w->numInputLinear > w->Alin_u.rows() || w->numInputLinear > w->blin_u.size()))
+        bad = "numInputLinear";
+    else if (t->en_tv_state_linear && (w->numtvStateLinear * N > w->tv_Alin_x.rows() || w->numtvStateLinear > w->tv_blin_x.rows()))
+        bad = "numtvStateLinear";
+    else if (t->en_tv_input_linear &&
+             (w->numtvInputLinear * (N - 1) > w->tv_Alin_u.rows() || w->numtvInputLinear > w->tv_blin_u.rows()))
+        bad = "numtvInputLinear";
+    if (!bad) return 0;
+    std::cout << "tinympc_b200 shim: work->" << bad << " exceeds the constraint arrays it counts" << std::endl;
+    return 1;
+}
+
+// the first `rows` rows of m (at most all of them) as their own column-major matrix: what the reference reads of a
+// constraint matrix whose count was lowered below its row count
+tinyMatrix top_rows(const tinyMatrix &m, long rows) { return m.topRows(std::min<long>(rows, m.rows())); }
+
 int ensure_handle(TinySolver *s, Impl &im) {
     const uint64_t fp = fingerprint(s, s->settings && s->settings->adaptive_rho);
     if (im.h && fp == im.fingerprint) return 0;
@@ -102,6 +134,16 @@ int ensure_handle(TinySolver *s, Impl &im) {
     im.h = nullptr;
     const TinyWorkspace *w = s->work;
     const TinyCache *c = s->cache;
+    const long N = w->N;
+    // counts above their arrays only reach here on a family that is off (check_counts), where they are never read
+    const int ncx = std::min<long>(w->numStateCones, std::min<long>(w->Acx.size(), std::min<long>(w->qcx.size(), w->cx.size())));
+    const int ncu = std::min<long>(w->numInputCones, std::min<long>(w->Acu.size(), std::min<long>(w->qcu.size(), w->cu.size())));
+    const tinyMatrix Ax = top_rows(w->Alin_x, w->numStateLinear), bx = top_rows(w->blin_x, Ax.rows());
+    const tinyMatrix Au = top_rows(w->Alin_u, w->numInputLinear), bu = top_rows(w->blin_u, Au.rows());
+    const int ntx = std::min<long>(w->numtvStateLinear, std::min<long>(w->tv_Alin_x.rows() / N, w->tv_blin_x.rows()));
+    const int ntu = std::min<long>(w->numtvInputLinear, std::min<long>(w->tv_Alin_u.rows() / (N - 1), w->tv_blin_u.rows()));
+    const tinyMatrix tAx = top_rows(w->tv_Alin_x, ntx * N), tbx = top_rows(w->tv_blin_x, ntx);
+    const tinyMatrix tAu = top_rows(w->tv_Alin_u, ntu * (N - 1)), tbu = top_rows(w->tv_blin_u, ntu);
     tinympc_problem_t p;
     std::memset(&p, 0, sizeof(p));
     p.nx = w->nx; p.nu = w->nu; p.N = w->N; p.dtype = TINYMPC_F64; p.rho = c->rho;
@@ -112,13 +154,13 @@ int ensure_handle(TinySolver *s, Impl &im) {
     const bool ub = w->u_min.rows() == w->nu && w->u_min.cols() == w->N - 1 && w->u_max.rows() == w->nu && w->u_max.cols() == w->N - 1;
     if (xb) { p.x_min = ptr(w->x_min); p.x_max = ptr(w->x_max); }
     if (ub) { p.u_min = ptr(w->u_min); p.u_max = ptr(w->u_max); }
-    p.num_state_cones = w->numStateCones; p.num_input_cones = w->numInputCones;
+    p.num_state_cones = ncx; p.num_input_cones = ncu;
     p.Acx = w->Acx.data(); p.qcx = w->qcx.data(); p.cx = ptr(w->cx);
     p.Acu = w->Acu.data(); p.qcu = w->qcu.data(); p.cu = ptr(w->cu);
-    p.num_state_linear = w->numStateLinear; p.num_input_linear = w->numInputLinear;
-    p.Alin_x = ptr(w->Alin_x); p.blin_x = ptr(w->blin_x); p.Alin_u = ptr(w->Alin_u); p.blin_u = ptr(w->blin_u);
-    p.num_tv_state_linear = w->numtvStateLinear; p.num_tv_input_linear = w->numtvInputLinear;
-    p.tv_Alin_x = ptr(w->tv_Alin_x); p.tv_blin_x = ptr(w->tv_blin_x); p.tv_Alin_u = ptr(w->tv_Alin_u); p.tv_blin_u = ptr(w->tv_blin_u);
+    p.num_state_linear = (int)Ax.rows(); p.num_input_linear = (int)Au.rows();
+    p.Alin_x = ptr(Ax); p.blin_x = ptr(bx); p.Alin_u = ptr(Au); p.blin_u = ptr(bu);
+    p.num_tv_state_linear = ntx; p.num_tv_input_linear = ntu;
+    p.tv_Alin_x = ptr(tAx); p.tv_blin_x = ptr(tbx); p.tv_Alin_u = ptr(tAu); p.tv_blin_u = ptr(tbu);
     int rc = tinympc_b200_create(&p, 0, &im.h);
     if (rc) {
         std::cout << "tinympc_b200 shim: " << tinympc_b200_last_error() << std::endl;
@@ -128,14 +170,19 @@ int ensure_handle(TinySolver *s, Impl &im) {
     return 0;
 }
 
-void push_settings(const TinySolver *s, Impl &im) {
+// a rejected update (check_termination <= 0) is an error of the solve: the handle would otherwise keep the previous settings
+int push_settings(const TinySolver *s, Impl &im) {
     const TinySettings *t = s->settings;
     tinympc_settings_t st;
     st.abs_pri_tol = t->abs_pri_tol; st.abs_dua_tol = t->abs_dua_tol; st.max_iter = t->max_iter;
     st.check_termination = t->check_termination; st.en_state_bound = t->en_state_bound; st.en_input_bound = t->en_input_bound;
     st.en_state_soc = t->en_state_soc; st.en_input_soc = t->en_input_soc; st.en_state_linear = t->en_state_linear;
     st.en_input_linear = t->en_input_linear; st.en_tv_state_linear = t->en_tv_state_linear; st.en_tv_input_linear = t->en_tv_input_linear;
-    tinympc_b200_update_settings(im.h, &st);
+    if (tinympc_b200_update_settings(im.h, &st)) {
+        std::cout << "tinympc_b200 shim: " << tinympc_b200_last_error() << std::endl;
+        return 1;
+    }
+    return 0;
 }
 
 template <class M>
@@ -395,8 +442,7 @@ int solve(TinySolver *s) {
         }
     }
     Impl &im = impl_of(s);
-    if (ensure_handle(s, im)) return 1;
-    push_settings(s, im);
+    if (check_counts(s) || ensure_handle(s, im) || push_settings(s, im)) return 1;  // nothing in the tree has changed yet
     const long nx = w->nx, nu = w->nu, N = w->N;
     tinympc_batch_t io;
     std::memset(&io, 0, sizeof(io));
@@ -462,8 +508,10 @@ int solve(TinySolver *s) {
     s->solution->solved = solved;
     w->iter = iter;
     w->status = solved ? 1 : 11;
-    w->primal_residual_state = res[0]; w->dual_residual_state = res[1];
-    w->primal_residual_input = res[2]; w->dual_residual_input = res[3];
+    if (iter >= s->settings->check_termination) {  // the reference writes the residuals only when a termination check runs
+        w->primal_residual_state = res[0]; w->dual_residual_state = res[1];
+        w->primal_residual_input = res[2]; w->dual_residual_input = res[3];
+    }
     if (solved) std::cout << "Solver converged in " << iter << " iterations" << std::endl;  // admm.cpp:439
     return solved ? 0 : 1;
 }
@@ -521,8 +569,7 @@ int tiny_destroy(TinySolver *s) {
 int tiny_solve_batch(TinySolver *s, const tinyMatrix &x0, const tinyMatrix &Xref, tinyMatrix &u0, VectorXi &iter, VectorXi &solved) {
     TinyWorkspace *w = s->work;
     Impl &im = impl_of(s);
-    if (ensure_handle(s, im)) return 1;
-    push_settings(s, im);
+    if (check_counts(s) || ensure_handle(s, im) || push_settings(s, im)) return 1;
     const long nx = w->nx, nu = w->nu, N = w->N, B = x0.cols();
     if (x0.rows() != nx || Xref.rows() != nx * N || Xref.cols() != B) return 1;
     std::vector<tinytype> sx((size_t)B * nx * N), su((size_t)B * nu * (N - 1)), ur((size_t)B * nu * (N - 1));

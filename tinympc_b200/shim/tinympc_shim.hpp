@@ -10,6 +10,11 @@
 // the "double rho" in the cache, tiny_set_bound_constraints returning 0 on a dimension mismatch, and the
 // "Solver converged in N iterations" line on stdout (admm.cpp:439).
 //
+// Every field of the tree a solve writes matches the reference bit for bit on the same cache
+// (tests/test_gpu_shim_parity.py), except work->{q, r, p, d}: per-iteration scratch the shim never writes.  Where the
+// reference is undefined (check_termination <= 0, a constraint count above its arrays) tiny_solve prints why and returns 1
+// with the tree unchanged (INTEGRATION.md §2).
+//
 // Needs an Eigen 3.4 include path supplied by the user (the reference vendors one under include/Eigen).
 // The reference's batched use is NOT expressible through this interface (it is single-instance by design);
 // batched callers use the C ABI directly or tiny_solve_batch() below.
