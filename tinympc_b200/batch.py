@@ -5,111 +5,98 @@ nx x N matrix (types.hpp:94-95) repeated B times.
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
+from typing import Callable
+
 import numpy as np
 
 from . import abi
 from .problem import MPCProblem
 
 
-BOUND_NAMES = ("x_min", "x_max", "u_min", "u_max")
+@dataclass(frozen=True)
+class Kind:
+    """One kind of per-instance data of a batch (tinympc_batch_t): the ABI mode field, the user's keys with the ABI field of
+    each, the keys that come in pairs, the accepted shapes of every key (shapes(dims, B) -> {key: {shape: mode}}, dims as
+    problem_dims gives them) and the
+    conversion of an array from the user's layout to the ABI's (an involution, a view)."""
+    mode_field: str
+    fields: dict
+    pairs: tuple
+    shapes: Callable
+    to_abi: Callable = lambda key, a: a
 
 
-def bounds_layout(bounds: dict, B: int, N: int, nx: int, nu: int, dtype) -> int:
-    """Check per-instance box bounds (a dict with any of x_min, x_max, u_min, u_max; numpy arrays or torch tensors) against a
-    batch of B instances and return their layout (tinympc_batch_t.bounds_per_instance): 1 for [B, nx] / [B, nu] (one column
-    per instance), 2 for [B, N, nx] / [B, N-1, nu] (a horizon per instance).  A side may be absent when its bound is
-    disabled; min and max of a side come together."""
-    unknown = set(bounds) - set(BOUND_NAMES)
+def _box_shapes(d, B):
+    return {k: {(B, w): 1, (B, n, w): 2} for k, w, n in (("x_min", d["nx"], d["N"]), ("x_max", d["nx"], d["N"]),
+                                                         ("u_min", d["nu"], d["N"] - 1), ("u_max", d["nu"], d["N"] - 1))}
+
+
+def _plane_shapes(d, B):
+    return {"Alin_x": {(B, d["nlx"], d["nx"]): 1}, "blin_x": {(B, d["nlx"]): 1}, "Alin_u": {(B, d["nlu"], d["nu"]): 1},
+            "blin_u": {(B, d["nlu"]): 1}}
+
+
+# bounds: [B, nx] / [B, nu] (one column per instance, mode 1) or [B, N, nx] / [B, N-1, nu] (a horizon per instance, mode 2);
+# cones: x_mu [B, state cones], u_mu [B, input cones]; planes: rows as tiny_set_linear_constraints takes them, Alin_x
+# [B, nlx, nx] / blin_x [B, nlx] and Alin_u [B, nlu, nu] / blin_u [B, nlu], each matrix column-major in the ABI
+KINDS = {
+    "bounds": Kind("bounds_per_instance", {k: k for k in ("x_min", "x_max", "u_min", "u_max")}, (("x_min", "x_max"), ("u_min", "u_max")),
+                   _box_shapes),
+    "cones": Kind("cones_per_instance", {"x_mu": "cone_x_mu", "u_mu": "cone_u_mu"}, (),
+                  lambda d, B: {"x_mu": {(B, d["ncx"]): 1}, "u_mu": {(B, d["ncu"]): 1}}),
+    "planes": Kind("planes_per_instance", {k: k for k in ("Alin_x", "blin_x", "Alin_u", "blin_u")},
+                   (("Alin_x", "blin_x"), ("Alin_u", "blin_u")), _plane_shapes,
+                   lambda key, a: a.swapaxes(1, 2) if key.startswith("Alin") else a),
+}
+
+
+def problem_dims(prob: MPCProblem) -> dict:
+    """the sizes the per-instance shapes depend on: horizon, state and input, cones and static hyperplane rows per side"""
+    nlx, nlu = (0 if a is None else a.shape[0] for a in (prob.Alin_x, prob.Alin_u))
+    return dict(N=prob.N, nx=prob.nx, nu=prob.nu, ncx=len(prob.Acx), ncu=len(prob.Acu), nlx=nlx, nlu=nlu)
+
+
+def per_instance(kind: str, arrays: dict, B: int, dims: dict, dtype) -> tuple:
+    """Check one kind's per-instance arrays (a dict keyed as users write them; numpy arrays or torch tensors of the problem
+    dtype) against a batch of B instances of a problem of these dims (problem_dims) -> (the ABI mode, {ABI field: the array
+    in ABI layout}).  A side may be absent when its loop does not run; the keys of a pair come together."""
+    spec = KINDS[kind]
+    unknown = set(arrays) - set(spec.fields)
     if unknown:
-        raise ValueError(f"bounds: unknown keys {sorted(unknown)}; expected any of {BOUND_NAMES}")
-    given = {k: v for k, v in bounds.items() if v is not None}
-    for lo, hi in (("x_min", "x_max"), ("u_min", "u_max")):
-        if (lo in given) != (hi in given):
-            raise ValueError(f"bounds: {lo} and {hi} are given together")
+        raise ValueError(f"{kind}: unknown keys {sorted(unknown)}; expected any of {tuple(spec.fields)}")
+    given = {k: v for k, v in arrays.items() if v is not None}
     if not given:
-        raise ValueError("bounds: give x_min / x_max, u_min / u_max or both")
-    want = np.dtype(dtype)
-    layouts = set()
+        raise ValueError(f"{kind}: give any of {tuple(spec.fields)}")
+    for a, b in spec.pairs:
+        if (a in given) != (b in given):
+            raise ValueError(f"{kind}: {a} and {b} are given in pairs")
+    want, shapes, modes = np.dtype(dtype), spec.shapes(dims, B), set()
     for k, a in given.items():
-        dt = a.dtype if hasattr(a, "dtype") else None
-        ok_dt = (str(dt).replace("torch.", "") == want.name) if dt is not None else False
-        if not ok_dt:
-            raise ValueError(f"bounds: {k} must have the problem dtype {want.name}, got {dt}")
-        w, kn = (nx, N) if k[0] == "x" else (nu, N - 1)
-        shape = tuple(a.shape)
-        if shape == (B, w):
-            layouts.add(1)
-        elif shape == (B, kn, w):
-            layouts.add(2)
-        else:
-            raise ValueError(f"bounds: {k} must be [{B}, {w}] (one column per instance) or [{B}, {kn}, {w}] (a horizon per "
-                             f"instance), got {list(shape)}")
-    if len(layouts) != 1:
-        raise ValueError("bounds: every array takes the same layout ([B, n] or [B, N, n])")
-    return layouts.pop()
-
-
-CONE_NAMES = ("x_mu", "u_mu")
-
-
-def cones_check(cones: dict, B: int, ncx: int, ncu: int, dtype) -> None:
-    """Check per-instance cone coefficients (a dict with x_mu [B, ncx] for the state cones and / or u_mu [B, ncu] for the
-    input cones; numpy arrays or torch tensors of the problem dtype) against a batch of B instances of a problem with ncx
-    state and ncu input cones (tinympc_batch_t.cone_x_mu / cone_u_mu).  A side may be absent when its cone loop does not run."""
-    unknown = set(cones) - set(CONE_NAMES)
-    if unknown:
-        raise ValueError(f"cones: unknown keys {sorted(unknown)}; expected any of {CONE_NAMES}")
-    given = {k: v for k, v in cones.items() if v is not None}
-    if not given:
-        raise ValueError("cones: give x_mu, u_mu or both")
-    want = np.dtype(dtype)
-    for k, a in given.items():
-        dt = a.dtype if hasattr(a, "dtype") else None
+        dt = getattr(a, "dtype", None)
         if dt is None or str(dt).replace("torch.", "") != want.name:
-            raise ValueError(f"cones: {k} must have the problem dtype {want.name}, got {dt}")
-        nc = ncx if k == "x_mu" else ncu
-        if tuple(a.shape) != (B, nc):
-            raise ValueError(f"cones: {k} must be [{B}, {nc}] (one mu per instance and {'state' if k == 'x_mu' else 'input'} cone), "
-                             f"got {list(a.shape)}")
+            raise ValueError(f"{kind}: {k} must have the problem dtype {want.name}, got {dt}")
+        if tuple(a.shape) not in shapes[k]:
+            raise ValueError(f"{kind}: {k} must be {' or '.join(str(list(sh)) for sh in shapes[k])}, got {list(a.shape)}")
+        modes.add(shapes[k][tuple(a.shape)])
+    if len(modes) != 1:
+        raise ValueError(f"{kind}: every array takes the same layout, got {sorted(given)} in modes {sorted(modes)}")
+    return modes.pop(), {spec.fields[k]: spec.to_abi(k, a) for k, a in given.items()}
 
 
-PLANE_NAMES = ("Alin_x", "blin_x", "Alin_u", "blin_u")
+# the key lists and the plane check and conversion under the names other modules and the tests import, all views of KINDS
+BOUND_NAMES = tuple(KINDS["bounds"].fields)
+PLANE_NAMES = tuple(KINDS["planes"].fields)
 
 
 def planes_check(planes: dict, B: int, nlx: int, nlu: int, nx: int, nu: int, dtype) -> None:
-    """Check per-instance static hyperplanes (a dict with Alin_x [B, nlx, nx] and blin_x [B, nlx] for the state side and / or
-    Alin_u [B, nlu, nu] and blin_u [B, nlu] for the input side, rows as a TinySolver's tiny_set_linear_constraints takes them;
-    numpy arrays or torch tensors of the problem dtype) against a batch of B instances of a problem with nlx state and nlu
-    input hyperplanes (tinympc_batch_t.Alin_x ... blin_u).  A side may be absent when its static hyperplane loop does not run."""
-    unknown = set(planes) - set(PLANE_NAMES)
-    if unknown:
-        raise ValueError(f"planes: unknown keys {sorted(unknown)}; expected any of {PLANE_NAMES}")
-    given = {k: v for k, v in planes.items() if v is not None}
-    if not given:
-        raise ValueError("planes: give Alin_x / blin_x, Alin_u / blin_u or both pairs")
-    for a, b in (("Alin_x", "blin_x"), ("Alin_u", "blin_u")):
-        if (a in given) != (b in given):
-            raise ValueError(f"planes: {a} and {b} are given in pairs")
-    want = np.dtype(dtype)
-    shapes = dict(Alin_x=(B, nlx, nx), blin_x=(B, nlx), Alin_u=(B, nlu, nu), blin_u=(B, nlu))
-    for k, a in given.items():
-        dt = a.dtype if hasattr(a, "dtype") else None
-        if dt is None or str(dt).replace("torch.", "") != want.name:
-            raise ValueError(f"planes: {k} must have the problem dtype {want.name}, got {dt}")
-        if tuple(a.shape) != shapes[k]:
-            raise ValueError(f"planes: {k} must be {list(shapes[k])} (one set of the problem's hyperplane rows per instance), "
-                             f"got {list(a.shape)}")
+    """per_instance's checks of per-instance static hyperplanes, for a problem with nlx / nlu rows"""
+    per_instance("planes", planes, B, dict(nx=nx, nu=nu, nlx=nlx, nlu=nlu), dtype)
 
 
 def planes_abi(planes: dict) -> dict:
-    """the given arrays of a checked planes dict with each instance's matrix in the ABI's column-major order ([B, n, nx] ->
-    a [B, nx, n] view; numpy arrays or torch tensors, made contiguous by the caller)"""
-    return {k: (v.swapaxes(1, 2) if k.startswith("Alin") else v) for k, v in planes.items() if v is not None}
-
-
-def num_planes(prob: MPCProblem) -> tuple:
-    """(state, input) static hyperplane rows of a problem"""
-    return (0 if prob.Alin_x is None else prob.Alin_x.shape[0], 0 if prob.Alin_u is None else prob.Alin_u.shape[0])
+    """the given arrays of a checked planes dict in the ABI's layout (each matrix a column-major view)"""
+    return {k: KINDS["planes"].to_abi(k, v) for k, v in planes.items() if v is not None}
 
 
 class HostBatch:
@@ -147,21 +134,12 @@ class HostBatch:
                 self.state[name] = np.zeros(shape, dtype=dt)
         self.cold_start = bool(cold_start)
         self.models = None if models is None else np.ascontiguousarray(models, dtype=dt).reshape(B, -1)
-        # per-instance box bounds (see bounds_layout); bounds_per_instance 0 = the problem's
-        self.bounds_per_instance, self.bounds = 0, {}
-        if bounds is not None:
-            self.bounds_per_instance = bounds_layout(bounds, B, N, nx, nu, dt)
-            self.bounds = {k: np.ascontiguousarray(v) for k, v in bounds.items() if v is not None}
-        # per-instance cone coefficients (see cones_check); cones_per_instance 0 = the problem's cx / cu
-        self.cones = None
-        if cones is not None:
-            cones_check(cones, B, len(prob.Acx), len(prob.Acu), dt)
-            self.cones = {k: np.ascontiguousarray(v) for k, v in cones.items() if v is not None}
-        # per-instance static hyperplanes (see planes_check), each matrix column-major; planes_per_instance 0 = the problem's
-        self.planes = None
-        if planes is not None:
-            planes_check(planes, B, *num_planes(prob), nx, nu, dt)
-            self.planes = {k: np.ascontiguousarray(v) for k, v in planes_abi(planes).items()}
+        # per-instance data (see KINDS): self.bounds / cones / planes = {ABI field: host array in ABI layout}; mode 0 = the problem's
+        self.modes = {}
+        for kind, arrays in dict(bounds=bounds, cones=cones, planes=planes).items():
+            mode, abi_arrays = (0, {}) if arrays is None else per_instance(kind, arrays, B, problem_dims(prob), dt)
+            self.modes[kind] = mode
+            setattr(self, kind, {f: np.ascontiguousarray(a) for f, a in abi_arrays.items()})
         self.sol_x = np.zeros((B, N, nx), dtype=dt)
         self.sol_u = np.zeros((B, N - 1, nu), dtype=dt)
         self.iter = np.zeros(B, dtype=np.int32)
@@ -185,17 +163,10 @@ class HostBatch:
         b.solved = self.solved.ctypes.data
         b.residuals = None if self.residuals is None else self.residuals.ctypes.data
         b.models = None if self.models is None else self.models.ctypes.data
-        b.bounds_per_instance = self.bounds_per_instance
-        for k, a in self.bounds.items():
-            setattr(b, k, a.ctypes.data)
-        if self.cones is not None:
-            b.cones_per_instance = 1
-            for k, a in self.cones.items():
-                setattr(b, "cone_" + k, a.ctypes.data)
-        if self.planes is not None:
-            b.planes_per_instance = 1
-            for k, a in self.planes.items():
-                setattr(b, k, a.ctypes.data)
+        for kind, spec in KINDS.items():
+            setattr(b, spec.mode_field, self.modes[kind])
+            for f, a in getattr(self, kind).items():
+                setattr(b, f, a.ctypes.data)
         b._owner = self
         return b
 

@@ -15,7 +15,7 @@ import ctypes as C
 
 from . import abi
 from ._lib import check
-from .batch import bounds_layout, cones_check, num_planes, planes_abi, planes_check
+from .batch import KINDS, per_instance, problem_dims
 from .solver import AdaptiveRho, BatchedTinySolver, pack_models
 
 # box-constrained warm start: slacks + duals (+ the previous-iteration slacks v, z, which only feed the dual residual of
@@ -62,40 +62,22 @@ class DeviceMPCLoop:
             cm = lambda a: torch.as_tensor(a, device=self.dev).to(self._tdt).transpose(1, 2).contiguous().transpose(1, 2)  # noqa: E731
             self.adaptive_rho = AdaptiveRho(cm(adaptive_rho.dKinf_drho), cm(adaptive_rho.dPinf_drho), adaptive_rho.rho_min,
                                             adaptive_rho.rho_max, adaptive_rho.enable_clipping)
-        self.bounds = None if bounds is None else self._device_bounds(bounds)
-        self.cones = None if cones is None else self._device_cones(cones)
-        self.planes = None if planes is None else self._device_planes(planes)
+        for kind, arrays in dict(bounds=bounds, cones=cones, planes=planes).items():
+            setattr(self, kind, None if arrays is None else self._device(kind, arrays))
         self.models = None
         if adaptive_rho is not None or models is not None:
             m = pack_models(p, self.B) if models is None else models
             self.models = torch.as_tensor(m, dtype=self._tdt, device=self.dev).reshape(self.B, -1).contiguous().clone()
 
-    def _device_bounds(self, bounds):
+    def _device(self, kind, arrays):
+        """one kind's per-instance arrays checked, each kept on the device in ABI layout (contiguous) and handed on as its view
+        in the user's layout, which make_device_batch uses in place"""
         import torch
 
         p = self.solver.problem
-        bounds_layout(bounds, self.B, p.N, p.nx, p.nu, p.dtype)
-        return {k: torch.as_tensor(v, device=self.dev).contiguous() for k, v in bounds.items() if v is not None}
-
-    def _device_cones(self, cones):
-        import torch
-
-        p = self.solver.problem
-        cones_check(cones, self.B, len(p.Acx), len(p.Acu), p.dtype)
-        return {k: torch.as_tensor(v, device=self.dev).contiguous() for k, v in cones.items() if v is not None}
-
-    def _device_planes(self, planes):
-        import torch
-
-        p = self.solver.problem
-        planes_check(planes, self.B, *num_planes(p), p.nx, p.nu, p.dtype)
-        # each matrix is kept column-major ([B, nx, n] contiguous) and handed on as its [B, n, nx] view, which
-        # make_device_batch uses in place
-        out = {}
-        for k, v in planes_abi(planes).items():
-            a = torch.as_tensor(v, device=self.dev).contiguous()
-            out[k] = a.swapaxes(1, 2) if k.startswith("Alin") else a
-        return out
+        per_instance(kind, arrays, self.B, problem_dims(p), p.dtype)
+        to_abi = KINDS[kind].to_abi
+        return {k: to_abi(k, to_abi(k, torch.as_tensor(v, device=self.dev)).contiguous()) for k, v in arrays.items() if v is not None}
 
     def step(self, Xref, Uref=None, stream=None, bounds=None, cones=None, planes=None):
         """One MPC step for every instance: solve (warm-started), then advance the plants.  Returns the output dict
@@ -111,8 +93,8 @@ class DeviceMPCLoop:
         het = self.models is not None and self.adaptive_rho is None
         batch, out = s.make_device_batch(self.x0, Xref, Uref, state=self.state, cold_start=self._first, want_state=self.fields,
                                          want_u0=True, want_solution=self.want_solution, models=self.models if het else None,
-                                         bounds=self.bounds if bounds is None else bounds, cones=self.cones if cones is None else cones,
-                                         planes=self.planes if planes is None else planes)
+                                         **{kind: getattr(self, kind) if over is None else over
+                                            for kind, over in dict(bounds=bounds, cones=cones, planes=planes).items()})
         if self.adaptive_rho is None:
             s.solve_device(batch, stream)
         else:
@@ -140,12 +122,9 @@ class DeviceMPCLoop:
 
         if self.adaptive_rho is not None:
             raise ValueError("rollout: adaptive rho is not available in a rollout; use step()")
-        if self.bounds is not None:
-            raise ValueError("rollout: per-instance bounds are not available in a rollout; use step()")
-        if self.cones is not None:
-            raise ValueError("rollout: per-instance cones are not available in a rollout; use step()")
-        if self.planes is not None:
-            raise ValueError("rollout: per-instance hyperplanes are not available in a rollout; use step()")
+        for kind in KINDS:
+            if getattr(self, kind) is not None:
+                raise ValueError(f"rollout: per-instance {kind} are not available in a rollout; use step()")
         if len(self.fields) != len(WARM_FIELDS if "v" in self.fields else WARM_FIELDS_FAST):
             raise ValueError("rollout: covers box constraints only (no extra_state); use step()")
         T = int(T)

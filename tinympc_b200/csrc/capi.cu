@@ -155,46 +155,103 @@ tmpc::Features features(const tinympc_b200_solver *s) {
     return f;
 }
 
-// the static hyperplane loops that run and read their coefficients (enabled, with rows): bit 0 state side, bit 1 input side
-int plane_sides(const tinympc_b200_solver *s) {
-    const tmpc::Features ft = features(s);
-    return (ft.lin_x && s->pd.nlx > 0 ? 1 : 0) | (ft.lin_u && s->pd.nlu > 0 ? 2 : 0);
+// The per-instance kinds of a batch besides models (tmpc::InstKind order): the mode field and its reserved neighbour, the
+// arrays with their side and elements per instance, when a side's loop runs and reads them, and the words of the errors.
+// check_solve, plan_solve, enqueue and the host path all work from this table.
+using BatchArray = const void *tinympc_batch_t::*;
+using BatchInt = int32_t tinympc_batch_t::*;
+struct KindArray {
+    BatchArray member;
+    int side;                                              // 0: state, 1: input
+    size_t (*elems)(const tmpc::ProblemDesc &, int mode);  // elements per instance
+};
+struct KindDesc {
+    BatchInt mode, reserved;
+    int max_mode;
+    KindArray arrays[4];
+    bool (*runs)(const tinympc_b200_solver *s, int side);  // the side's loop runs and reads its arrays
+    bool gps_only;      // served by the streamed kernel only; read only while a loop runs (else routed by the flag)
+    const char *mode_msg;
+    const char *pairs_msg;  // a side's arrays come together, whether its loop runs or not; null: no such rule
+    int missing_code;   // a side whose loop runs lacks an array
+    const char *missing_msg;
+    const char *handles, *noun, *field, *exclusive;  // "the handle's <handles>", "per-instance <noun>", the mode field, kinds it does not combine with
+};
+
+const KindDesc KINDS[tmpc::NKINDS] = {
+    {&tinympc_batch_t::bounds_per_instance, &tinympc_batch_t::reserved2, 2,
+     {{&tinympc_batch_t::x_min, 0, [](const tmpc::ProblemDesc &pd, int m) { return (size_t)pd.nx * (m == 2 ? pd.N : 1); }},
+      {&tinympc_batch_t::x_max, 0, [](const tmpc::ProblemDesc &pd, int m) { return (size_t)pd.nx * (m == 2 ? pd.N : 1); }},
+      {&tinympc_batch_t::u_min, 1, [](const tmpc::ProblemDesc &pd, int m) { return (size_t)pd.nu * (m == 2 ? pd.N - 1 : 1); }},
+      {&tinympc_batch_t::u_max, 1, [](const tmpc::ProblemDesc &pd, int m) { return (size_t)pd.nu * (m == 2 ? pd.N - 1 : 1); }}},
+     [](const tinympc_b200_solver *s, int side) { return (side ? s->settings.en_input_bound : s->settings.en_state_bound) != 0; },
+     false,
+     "bounds_per_instance must be 0 (the handle's bounds), 1 (one column per instance) or 2 (a horizon per instance), and "
+     "reserved2 must be 0",
+     "per-instance bounds: x_min / x_max and u_min / u_max are given in pairs",
+     TINYMPC_ERR_NO_BOUNDS,
+     "per-instance bounds: en_state_bound/en_input_bound set but the batch has no x_min/x_max or u_min/u_max",
+     "bounds", "bounds", "bounds_per_instance", "hyperplanes"},
+    {&tinympc_batch_t::cones_per_instance, &tinympc_batch_t::reserved3, 1,
+     {{&tinympc_batch_t::cone_x_mu, 0, [](const tmpc::ProblemDesc &pd, int) { return (size_t)pd.ncx; }},
+      {&tinympc_batch_t::cone_u_mu, 1, [](const tmpc::ProblemDesc &pd, int) { return (size_t)pd.ncu; }}},
+     [](const tinympc_b200_solver *s, int side) { return (bool)(side ? features(s).soc_u : features(s).soc_x); },
+     true,
+     "cones_per_instance must be 0 (the handle's cone coefficients) or 1 (cone_x_mu / cone_u_mu per instance), and reserved3 "
+     "must be 0",
+     nullptr,
+     TINYMPC_ERR_ARG,
+     "per-instance cones: en_state_soc / en_input_soc set on a side with cones but the batch has no cone_x_mu / cone_u_mu for it",
+     "cone coefficients", "cones", "cones_per_instance", "hyperplanes"},
+    {&tinympc_batch_t::planes_per_instance, &tinympc_batch_t::reserved4, 1,
+     {{&tinympc_batch_t::Alin_x, 0, [](const tmpc::ProblemDesc &pd, int) { return (size_t)pd.nx * pd.nlx; }},
+      {&tinympc_batch_t::blin_x, 0, [](const tmpc::ProblemDesc &pd, int) { return (size_t)pd.nlx; }},
+      {&tinympc_batch_t::Alin_u, 1, [](const tmpc::ProblemDesc &pd, int) { return (size_t)pd.nu * pd.nlu; }},
+      {&tinympc_batch_t::blin_u, 1, [](const tmpc::ProblemDesc &pd, int) { return (size_t)pd.nlu; }}},
+     [](const tinympc_b200_solver *s, int side) { return side ? features(s).lin_u && s->pd.nlu > 0 : features(s).lin_x && s->pd.nlx > 0; },
+     true,
+     "planes_per_instance must be 0 (the handle's hyperplanes) or 1 (Alin_x / blin_x / Alin_u / blin_u per instance), and "
+     "reserved4 must be 0",
+     nullptr,
+     TINYMPC_ERR_ARG,
+     "per-instance hyperplanes: en_state_linear / en_input_linear set on a side with rows but the batch has no Alin_x / blin_x "
+     "or Alin_u / blin_u for it",
+     "hyperplanes", "hyperplanes", "planes_per_instance", "bounds or cones"},
+};
+
+// what a batch brings per instance and what its solve's kernel reads (tmpc::PerInstance)
+tmpc::PerInstance per_instance(const tinympc_b200_solver *s, const tinympc_batch_t *io) {
+    tmpc::PerInstance pi;
+    pi.models = io->models != nullptr;
+    for (int k = 0; k < tmpc::NKINDS; ++k) {
+        const KindDesc &kd = KINDS[k];
+        pi.given[k] = io->*kd.mode;
+        pi.read[k] = pi.given[k] && (!kd.gps_only || kd.runs(s, 0) || kd.runs(s, 1)) ? pi.given[k] : 0;
+    }
+    return pi;
 }
 
 // The checks of a solve before it is planned: the handle's state, then the arguments (ar: adaptive rho, or null).  Their
 // order decides which error a caller sees.
 int check_solve(const tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_adaptive_rho_t *ar) {
     const tinympc_settings_t &st = s->settings;
-    const int bpi = io->bounds_per_instance;
-    if (bpi < 0 || bpi > 2 || io->reserved2 != 0)
-        return fail(TINYMPC_ERR_ARG, "bounds_per_instance must be 0 (the handle's bounds), 1 (one column per instance) or 2 "
-                                     "(a horizon per instance), and reserved2 must be 0");
-    if (bpi == 0) {
-        if ((st.en_state_bound && !s->pd.x_min) || (st.en_input_bound && !s->pd.u_min))
-            return fail(TINYMPC_ERR_NO_BOUNDS, "en_state_bound/en_input_bound set but bounds were never provided");
-    } else {  // the batch's bounds replace the handle's
-        if (!io->x_min != !io->x_max || !io->u_min != !io->u_max)
-            return fail(TINYMPC_ERR_ARG, "per-instance bounds: x_min / x_max and u_min / u_max are given in pairs");
-        if ((st.en_state_bound && !io->x_min) || (st.en_input_bound && !io->u_min))
-            return fail(TINYMPC_ERR_NO_BOUNDS, "per-instance bounds: en_state_bound/en_input_bound set but the batch has no x_min/x_max or u_min/u_max");
-    }
-    if ((io->cones_per_instance != 0 && io->cones_per_instance != 1) || io->reserved3 != 0)
-        return fail(TINYMPC_ERR_ARG, "cones_per_instance must be 0 (the handle's cone coefficients) or 1 (cone_x_mu / cone_u_mu per "
-                                     "instance), and reserved3 must be 0");
-    if (io->cones_per_instance) {  // a side whose cone loop runs needs its coefficients; the other side's pointer is never read
-        const tmpc::Features ft = features(s);
-        if ((ft.soc_x && !io->cone_x_mu) || (ft.soc_u && !io->cone_u_mu))
-            return fail(TINYMPC_ERR_ARG, "per-instance cones: en_state_soc / en_input_soc set on a side with cones but the batch has no "
-                                         "cone_x_mu / cone_u_mu for it");
-    }
-    if ((io->planes_per_instance != 0 && io->planes_per_instance != 1) || io->reserved4 != 0)
-        return fail(TINYMPC_ERR_ARG, "planes_per_instance must be 0 (the handle's hyperplanes) or 1 (Alin_x / blin_x / Alin_u / blin_u per "
-                                     "instance), and reserved4 must be 0");
-    if (io->planes_per_instance) {  // a side whose static hyperplane loop runs needs its pair; the other side's is never read
-        const int sides = plane_sides(s);
-        if (((sides & 1) && (!io->Alin_x || !io->blin_x)) || ((sides & 2) && (!io->Alin_u || !io->blin_u)))
-            return fail(TINYMPC_ERR_ARG, "per-instance hyperplanes: en_state_linear / en_input_linear set on a side with rows but the "
-                                         "batch has no Alin_x / blin_x or Alin_u / blin_u for it");
+    for (const KindDesc &kd : KINDS) {
+        const int mode = io->*kd.mode;
+        if (mode < 0 || mode > kd.max_mode || io->*kd.reserved != 0) return fail(TINYMPC_ERR_ARG, kd.mode_msg);
+        if (mode == 0) {  // the handle's arrays: only bounds can be missing from a handle
+            if (&kd == &KINDS[tmpc::KIND_BOUNDS] && ((st.en_state_bound && !s->pd.x_min) || (st.en_input_bound && !s->pd.u_min)))
+                return fail(TINYMPC_ERR_NO_BOUNDS, "en_state_bound/en_input_bound set but bounds were never provided");
+            continue;
+        }
+        // the batch's arrays replace the handle's; a side whose loop does not run is never read
+        int n[2] = {}, have[2] = {};  // arrays per side, and those of them the batch gives
+        for (const KindArray &a : kd.arrays)
+            if (a.member) {
+                ++n[a.side];
+                have[a.side] += io->*a.member != nullptr;
+            }
+        if (kd.pairs_msg && ((have[0] && have[0] != n[0]) || (have[1] && have[1] != n[1]))) return fail(TINYMPC_ERR_ARG, kd.pairs_msg);
+        if ((kd.runs(s, 0) && have[0] < n[0]) || (kd.runs(s, 1) && have[1] < n[1])) return fail(kd.missing_code, kd.missing_msg);
     }
     if (st.check_termination <= 0) return fail(TINYMPC_ERR_ARG, "check_termination must be >= 1");
     if (!io->x0 || !io->Xref) return fail(TINYMPC_ERR_ARG, "x0 and Xref are required");
@@ -217,36 +274,27 @@ struct SolvePlan {
 // shared memory the adaptive kernel adds per CTA for its tables
 size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->pd.nx, s->pd.nu, esize(s->pd.dtype)); }
 
-// The plan of a solve of B instances (models: per-instance models; bounds: per-instance box bounds; cones: per-instance cone
-// coefficients, cones_per_instance set; planes: per-instance static hyperplanes, planes_per_instance set; adapt: adaptive rho).
-// GPI = lane groups, state on chip (box constraints, horizon fits in shared memory); GPS = lane groups, state streamed
-// (everything else the lane mapping covers); TPI = one thread per instance.  Fails when an explicit request or a feature
-// cannot be served.
-int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cones, bool planes, bool adapt, int64_t B, SolvePlan *p,
-               bool rollout = false) {
+// The plan of a solve of B instances (pi: its per-instance data; adapt: adaptive rho).  GPI = lane groups, state on chip (box
+// constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane mapping covers);
+// TPI = one thread per instance.  Fails when an explicit request or a feature cannot be served.
+int plan_solve(const tinympc_b200_solver *s, const tmpc::PerInstance &pi, bool adapt, int64_t B, SolvePlan *p, bool rollout = false) {
     const tmpc::Features ft = features(s);
-    if (planes) {  // per-instance static hyperplanes have STRICT variants of the streamed kernel only, alone or with models
-        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's hyperplanes (planes_per_instance must be 0)");
-        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's hyperplanes (planes_per_instance must be 0)");
-        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes are available in STRICT mode only");
-        if (s->family == TINYMPC_KERNEL_TPI)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes run on the streamed lane-group kernel (GPS), not on one thread per instance");
-        if (bounds || cones)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes do not combine with per-instance bounds or cones in one batch");
-    }
-    const bool planes_run = planes && plane_sides(s) != 0;  // else the coefficients are never read: the plan without them
-    if (cones) {  // per-instance cone coefficients have STRICT variants of the streamed kernel only
-        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's cone coefficients (cones_per_instance must be 0)");
-        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's cone coefficients (cones_per_instance must be 0)");
-        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones are available in STRICT mode only");
-        if (s->family == TINYMPC_KERNEL_TPI)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones run on the streamed lane-group kernel (GPS), not on one thread per instance");
-    }
-    const bool cones_run = cones && (ft.soc_x || ft.soc_u);  // else the coefficients are never read: the plan without them
-    if (bounds) {  // per-instance bounds have STRICT solve variants only
-        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run with the handle's bounds (bounds_per_instance must be 0)");
-        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs with the handle's bounds (bounds_per_instance must be 0)");
-        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance bounds are available in STRICT mode only");
+    // per-instance kinds have STRICT solve variants only; the refusals look at the flags, planes first, then cones, then bounds
+    for (int k = tmpc::NKINDS - 1; k >= 0; --k) {
+        if (!pi.given[k]) continue;
+        const KindDesc &kd = KINDS[k];
+        if (rollout) return fail(TINYMPC_ERR_UNSUPPORTED, std::string("rollouts run with the handle's ") + kd.handles + " (" + kd.field + " must be 0)");
+        if (adapt) return fail(TINYMPC_ERR_UNSUPPORTED, std::string("adaptive rho runs with the handle's ") + kd.handles + " (" + kd.field + " must be 0)");
+        if (s->mode == TINYMPC_MODE_FAST)
+            return fail(TINYMPC_ERR_UNSUPPORTED, std::string("per-instance ") + kd.noun + " are available in STRICT mode only");
+        if (kd.gps_only && s->family == TINYMPC_KERNEL_TPI)
+            return fail(TINYMPC_ERR_UNSUPPORTED, std::string("per-instance ") + kd.noun +
+                                                     " run on the streamed lane-group kernel (GPS), not on one thread per instance");
+        bool compiled = false;  // some streamed kernel serves the kinds the batch gives together
+        for (int fam : {0, 1, 6, 7}) compiled |= tmpc::gps_compiled(fam, tmpc::gps_variant(pi.models, pi.given), false);
+        if (!compiled)
+            return fail(TINYMPC_ERR_UNSUPPORTED, std::string("per-instance ") + kd.noun + " do not combine with per-instance " +
+                                                     kd.exclusive + " in one batch");
     }
     if (rollout) {  // closed-loop rollout: the on-chip kernel's rollout variant, with the on-chip plan a solve would use
         if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts are available in STRICT mode only");
@@ -306,7 +354,7 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cone
     // rounds such chunks by the family a shared model would get).  Otherwise the streamed kernel's one-instance-per-lane-group
     // variant: explicit GPS, cones or hyperplanes, or a horizon that does not fit on chip.  One thread per instance has no
     // such variant.
-    if (models || bounds) {
+    if (pi.models || pi.given[tmpc::KIND_BOUNDS]) {
         if (s->family == TINYMPC_KERNEL_TPI)
             return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models and bounds run on the lane-group kernel families (GPI, GPS), not on one thread per instance");
         if (s->family != TINYMPC_KERNEL_GPS && !ft.ext && gpi_ok) {
@@ -314,17 +362,17 @@ int plan_solve(const tinympc_b200_solver *s, bool models, bool bounds, bool cone
         } else {
             if (!gps_ok) return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance models / bounds: this problem needs the streamed lane-group kernel, which does not cover this shape");
             p->family = TINYMPC_KERNEL_GPS;
-            p->per_cta = s->dim->gps_het_slots(s->pd.dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u, cones_run,
-                                               s->max_smem_optin);
+            p->per_cta = s->dim->gps_het_slots(s->pd.dtype, ft.soc_x || ft.soc_u, ft.lin_x || ft.lin_u || ft.tvl_x || ft.tvl_u,
+                                               pi.read[tmpc::KIND_CONES], s->max_smem_optin);
         }
     }
-    // A cone loop routes the solve to the streamed kernel when it covers the shape; its GPS_CONES variants keep the plan the
-    // rules above chose (alone: the shared solve's, whose chunks are not rounded; with models or bounds: gps_het_slots)
-    if (cones_run && p->family != TINYMPC_KERNEL_GPS)
-        return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance cones: this problem needs the streamed lane-group kernel, which does not cover this shape");
-    // likewise a static hyperplane loop: its GPS_PLANES variants keep the shared solve's plan, or gps_het_slots with models
-    if (planes_run && p->family != TINYMPC_KERNEL_GPS)
-        return fail(TINYMPC_ERR_UNSUPPORTED, "per-instance hyperplanes: this problem needs the streamed lane-group kernel, which does not cover this shape");
+    // A cone or static hyperplane loop routes the solve to the streamed kernel when it covers the shape; its GPS_CONES /
+    // GPS_PLANES variants keep the plan the rules above chose (alone: the shared solve's, whose chunks are not rounded; with
+    // models or bounds: gps_het_slots)
+    for (int k = 0; k < tmpc::NKINDS; ++k)
+        if (KINDS[k].gps_only && pi.read[k] && p->family != TINYMPC_KERNEL_GPS)
+            return fail(TINYMPC_ERR_UNSUPPORTED, std::string("per-instance ") + KINDS[k].noun +
+                                                     ": this problem needs the streamed lane-group kernel, which does not cover this shape");
     if (p->family < 0) return fail(TINYMPC_ERR_UNSUPPORTED, "the requested lane-group kernel does not cover this problem shape");
     return 0;
 }
@@ -404,10 +452,10 @@ int upload_rollout(tinympc_b200_solver *s, const tinympc_rollout_t *ro, cudaStre
 // the kernel reads, the per-instance models or, with ar (adaptive rho, else null), the blobs it adapts in place
 int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stream, bool timed,
             const tinympc_adaptive_rho_t *ar = nullptr, const tinympc_rollout_t *ro = nullptr) {
+    const tmpc::PerInstance pi = per_instance(s, io);
     SolvePlan plan;
     if (ar || ro || io->B > 0)  // an adaptive solve or a rollout is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0,
-                                io->planes_per_instance != 0, ar != nullptr, io->B, &plan, ro != nullptr))
+        if (int rc = plan_solve(s, pi, ar != nullptr, io->B, &plan, ro != nullptr))
             return rc;
     if (io->B <= 0 || (ro && ro->T == 0)) return TINYMPC_OK;
     const int family = plan.family;
@@ -422,9 +470,7 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
     d.fast = s->mode == TINYMPC_MODE_FAST;
     d.sm_count = s->sm_count;
     d.max_smem_optin = s->max_smem_optin;
-    d.bounds = io->bounds_per_instance;
-    d.cones = io->cones_per_instance && (d.ft.soc_x || d.ft.soc_u);
-    d.planes = io->planes_per_instance && plane_sides(s) != 0;
+    d.pi = pi;
     if (ar) {
         if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_adaptive<double>(s, ar, io->models, stream)
                                                 : upload_adaptive<float>(s, ar, io->models, stream))
@@ -947,8 +993,7 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     chunk = (chunk + 31) / 32 * 32;
     SolvePlan plan;  // of a chunk
     if (ar || B > 0)  // an adaptive solve is checked whole even when the batch is empty
-        if (int rc = plan_solve(s, io->models != nullptr, io->bounds_per_instance != 0, io->cones_per_instance != 0,
-                                io->planes_per_instance != 0, ar != nullptr, chunk, &plan))
+        if (int rc = plan_solve(s, per_instance(s, io), ar != nullptr, chunk, &plan))
             return rc;
     if (B <= 0) return TINYMPC_OK;
     const size_t es = esize(s->pd.dtype);
@@ -981,42 +1026,13 @@ int solve_host_impl(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const t
     if (io->models) fields.push_back({io->models, nullptr, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, false, (void **)&dev.models});
     // adaptive rho: the model blobs are in/out; they travel in dev.models (io->models is NULL), where the kernel adapts them
     if (ar) fields.push_back({ar->models, ar->models, es * (size_t)tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), true, true, (void **)&dev.models});
-    if (io->bounds_per_instance) {  // sliced per chunk like the models; a disabled side is never read
-        const size_t kx = io->bounds_per_instance == 2 ? s->pd.N : 1, ku = io->bounds_per_instance == 2 ? s->pd.N - 1 : 1;
-        if (s->settings.en_state_bound) {
-            fields.push_back({io->x_min, nullptr, es * s->pd.nx * kx, true, false, (void **)&dev.x_min});
-            fields.push_back({io->x_max, nullptr, es * s->pd.nx * kx, true, false, (void **)&dev.x_max});
-        } else {
-            dev.x_min = dev.x_max = nullptr;
-        }
-        if (s->settings.en_input_bound) {
-            fields.push_back({io->u_min, nullptr, es * s->pd.nu * ku, true, false, (void **)&dev.u_min});
-            fields.push_back({io->u_max, nullptr, es * s->pd.nu * ku, true, false, (void **)&dev.u_max});
-        } else {
-            dev.u_min = dev.u_max = nullptr;
-        }
-    }
-    if (io->cones_per_instance) {  // sliced per chunk like the bounds; a side whose cone loop does not run is never read
-        const tmpc::Features ft = features(s);
-        if (ft.soc_x) fields.push_back({io->cone_x_mu, nullptr, es * s->pd.ncx, true, false, (void **)&dev.cone_x_mu});
-        else dev.cone_x_mu = nullptr;
-        if (ft.soc_u) fields.push_back({io->cone_u_mu, nullptr, es * s->pd.ncu, true, false, (void **)&dev.cone_u_mu});
-        else dev.cone_u_mu = nullptr;
-    }
-    if (io->planes_per_instance) {  // sliced per chunk like the cones; a side whose static hyperplane loop does not run is never read
-        const int sides = plane_sides(s);
-        const size_t nlx = s->pd.nlx, nlu = s->pd.nlu;
-        if (sides & 1) {
-            fields.push_back({io->Alin_x, nullptr, es * s->pd.nx * nlx, true, false, (void **)&dev.Alin_x});
-            fields.push_back({io->blin_x, nullptr, es * nlx, true, false, (void **)&dev.blin_x});
-        } else {
-            dev.Alin_x = dev.blin_x = nullptr;
-        }
-        if (sides & 2) {
-            fields.push_back({io->Alin_u, nullptr, es * s->pd.nu * nlu, true, false, (void **)&dev.Alin_u});
-            fields.push_back({io->blin_u, nullptr, es * nlu, true, false, (void **)&dev.blin_u});
-        } else {
-            dev.Alin_u = dev.blin_u = nullptr;
+    for (const KindDesc &kd : KINDS) {  // sliced per chunk like the models; a side whose loop does not run is never read
+        const int mode = io->*kd.mode;
+        if (!mode) continue;
+        for (const KindArray &a : kd.arrays) {
+            if (!a.member) continue;
+            if (kd.runs(s, a.side)) fields.push_back({io->*a.member, nullptr, es * a.elems(s->pd, mode), true, false, (void **)&(dev.*a.member)});
+            else dev.*a.member = nullptr;
         }
     }
     if (ar && ar->tables_per_instance) {  // sliced per chunk like the models

@@ -33,6 +33,7 @@
 #pragma once
 #include <algorithm>
 #include <cstdlib>
+#include <utility>
 
 #include "common.cuh"
 #include "lanegroup.cuh"
@@ -194,31 +195,27 @@ __device__ __forceinline__ void stg_piece(T *p, const T (&v)[R], unsigned pr) {
     }
 }
 
+// Per-instance data: variant bits added to the family mask (FAMH); launch.h defines them and which variants are compiled.
 // Per-instance models (tinympc_batch_t.models): the kernel is instantiated with GPS_HET added to its family mask (FAMH).
 // Every instance then brings its own model / cache blob and rho.  A slot keeps a pointer to its instance's blob and the
 // sweeps read their matrix rows from it (ld.global.nc: the blobs are read-only for the launch) instead of from the CTA's
 // staged copy.  It runs one instance per lane group: the NI = 2 variant shares the matrix registers between the two
 // instances of a group, and two sets of rows do not fit.
-constexpr int GPS_HET = 8;
 // Per-instance box bounds (tinympc_batch_t.bounds_per_instance): GPS_BOUNDS added to the family mask.  P.x_min ... u_max point at
 // the batch's [B][nx] / [B][nu] columns (P.bounds_tv == 0) or [B][N][nx] / [B][N-1][nu] horizons (P.bounds_tv == 1); a slot loads
 // its instance's column 0 when it is loaded.  One instance per lane group, as GPS_HET: the bound registers are per lane, and
 // two instances with bounds of their own do not fit the NI = 2 budget.
-constexpr int GPS_BOUNDS = 16;
 // Per-instance cone coefficients (tinympc_batch_t.cones_per_instance): GPS_CONES added to a family mask with cones (1, 7).
 // P.w_vc / P.w_zc (thread-per-instance workspace pointers, which this kernel never reads otherwise) point at the batch's
 // [B][ncx] / [B][ncu] coefficients.  Each warp keeps a table [slot][side][MAX_CONES] in shared memory, after the rings of all
 // warps, which a slot's lanes fill when the slot is loaded.  In cones_xu lane l of a group always projects work item l, one
 // (instance, side) pair, so a lane reads the coefficients of one slot and one side only: they stay out of registers, and
 // the kernel keeps the NI of the shared solve (two instances per lane group where the shared model runs two).
-constexpr int GPS_CONES = 32;
 // Per-instance static hyperplanes (tinympc_batch_t.planes_per_instance): GPS_PLANES added to a family mask with static
 // hyperplanes (6, 7), alone or with GPS_HET.  P.Alin_x / blin_x / Alin_u / blin_u point at the batch's [B][nx][nlx] / [B][nlx] /
 // [B][nu][nlu] / [B][nlu] arrays, and planes_x / planes_u add the slot's instance offset.  project_rows reads the coefficients
 // from memory row by row and never holds them in registers, so the per-slot cost is a pointer and the kernel keeps the NI of
 // the shared solve.
-constexpr int GPS_PLANES = 64;
-constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS | GPS_CONES | GPS_PLANES;  // the family-mask bits that are not constraint families
 
 template <typename T, int NX, int NU, int L, int NI, int FAMH, bool FAST>
 __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
@@ -1234,90 +1231,38 @@ int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
 
 // family mask of the kernel that serves a feature set: 0 box only, 1 cones only, 6 hyperplanes only, 7 anything else
 inline int gps_family_mask(bool soc, bool lin) { return !soc && !lin ? 0 : (soc && !lin ? 1 : (!soc ? 6 : 7)); }
+constexpr int GPS_FAMILY_MASKS[4] = {0, 1, 6, 7};
 
+// case I of the walk over (family mask, variant bits): launch its kernel when it is compiled and (fam, var) selects it
+template <typename T, int NX, int NU, int L, int NI, bool FAST, int I>
+bool gps_launch_case(LaunchDesc *d, const KParams<T, NX, NU> &P0, int fam, int var, int *rc) {
+    constexpr int FF = GPS_FAMILY_MASKS[I / 16], VV = (I % 16) * GPS_HET;
+    if constexpr (gps_compiled(FF, VV, FAST)) {
+        if (fam == FF && var == VV) {
+            *rc = launch_gps_cfg<T, NX, NU, L, gps_variant_ni(VV, NI), FF | VV, FAST>(d, P0);
+            return true;
+        }
+    }
+    return false;
+}
+template <typename T, int NX, int NU, int L, int NI, bool FAST, int... I>
+int gps_launch_walk(LaunchDesc *d, const KParams<T, NX, NU> &P0, int fam, int var, std::integer_sequence<int, I...>) {
+    int rc = TINYMPC_ERR_UNSUPPORTED;
+    (gps_launch_case<T, NX, NU, L, NI, FAST, I>(d, P0, fam, var, &rc) || ...);
+    return rc;
+}
+
+// the streamed kernel of the solve's constraint families and per-instance data (launch.h: gps_compiled); a variant that is
+// not compiled is TINYMPC_ERR_UNSUPPORTED
 template <typename T, int NX, int NU, bool FAST>
 int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
     constexpr int L = gps_pick_L<T, NX, NU>();
     if constexpr (L == 0) {
         return TINYMPC_ERR_UNSUPPORTED;
     } else {
-        constexpr int NI = gps_pick_NI<T, NX, NU, L>();
         const int fam = gps_family_mask(d->ft.soc_x || d->ft.soc_u, d->ft.lin_x || d->ft.lin_u || d->ft.tvl_x || d->ft.tvl_u);
-        if (d->planes) {  // per-instance static hyperplanes (STRICT; a static hyperplane loop runs, so the mask is 6 or 7; no
-                          // per-instance bounds or cones): the shared solve's NI alone, one instance per lane group with models
-            if constexpr (FAST) {
-                return TINYMPC_ERR_UNSUPPORTED;
-            } else {
-                if (d->bounds || d->cones) return TINYMPC_ERR_UNSUPPORTED;
-                const bool het = d->io.models != nullptr;
-#define TM_GPS_PL_CASE(FF)                                                                        \
-    if (fam == FF) {                                                                              \
-        if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_PLANES | GPS_HET, false>(d, P0); \
-        return launch_gps_cfg<T, NX, NU, L, NI, FF | GPS_PLANES, false>(d, P0);                   \
-    }
-                TM_GPS_PL_CASE(6)
-                TM_GPS_PL_CASE(7)
-#undef TM_GPS_PL_CASE
-                return TINYMPC_ERR_UNSUPPORTED;
-            }
-        }
-        if (d->cones) {  // per-instance cone coefficients (STRICT; a cone loop runs, so the mask is 1 or 7): the shared solve's NI
-                         // on their own, one instance per lane group with per-instance models or bounds
-            if constexpr (FAST) {
-                return TINYMPC_ERR_UNSUPPORTED;
-            } else {
-                const bool het = d->io.models != nullptr;
-#define TM_GPS_CN_CASE(FF)                                                                                             \
-    if (fam == FF) {                                                                                                   \
-        if (d->bounds) {                                                                                               \
-            if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_CONES | GPS_BOUNDS | GPS_HET, false>(d, P0);      \
-            return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_CONES | GPS_BOUNDS, false>(d, P0);                         \
-        }                                                                                                              \
-        if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_CONES | GPS_HET, false>(d, P0);                       \
-        return launch_gps_cfg<T, NX, NU, L, NI, FF | GPS_CONES, false>(d, P0);                                         \
-    }
-                TM_GPS_CN_CASE(1)
-                TM_GPS_CN_CASE(7)
-#undef TM_GPS_CN_CASE
-                return TINYMPC_ERR_UNSUPPORTED;
-            }
-        }
-        if (d->bounds) {  // per-instance bounds (STRICT): one instance per lane group, with or without per-instance models
-            if constexpr (FAST) {
-                return TINYMPC_ERR_UNSUPPORTED;
-            } else {
-                const bool het = d->io.models != nullptr;
-#define TM_GPS_BND_CASE(FF)                                                                       \
-    if (fam == FF) {                                                                              \
-        if (het) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_BOUNDS | GPS_HET, false>(d, P0); \
-        return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_BOUNDS, false>(d, P0);                    \
-    }
-                TM_GPS_BND_CASE(0)
-                TM_GPS_BND_CASE(1)
-                TM_GPS_BND_CASE(6)
-                TM_GPS_BND_CASE(7)
-#undef TM_GPS_BND_CASE
-                return TINYMPC_ERR_UNSUPPORTED;
-            }
-        }
-        if (d->io.models) {  // per-instance models: one instance per lane group, the same family variants
-#define TM_GPS_HET_CASE(FF) \
-    if (fam == FF) return launch_gps_cfg<T, NX, NU, L, 1, FF | GPS_HET, FAST>(d, P0);
-            TM_GPS_HET_CASE(0)
-            TM_GPS_HET_CASE(1)
-            TM_GPS_HET_CASE(6)
-            TM_GPS_HET_CASE(7)
-#undef TM_GPS_HET_CASE
-            return TINYMPC_ERR_UNSUPPORTED;
-        }
-#define TM_GPS_CASE(FF) \
-    if (fam == FF) return launch_gps_cfg<T, NX, NU, L, NI, FF, FAST>(d, P0);
-        TM_GPS_CASE(0)
-        TM_GPS_CASE(1)
-        TM_GPS_CASE(6)
-        TM_GPS_CASE(7)
-#undef TM_GPS_CASE
-        return TINYMPC_ERR_UNSUPPORTED;
+        return gps_launch_walk<T, NX, NU, L, gps_pick_NI<T, NX, NU, L>(), FAST>(d, P0, fam, gps_variant(d->pi.models, d->pi.read),
+                                                                              std::make_integer_sequence<int, 4 * 16>());
     }
 }
 
@@ -1330,13 +1275,14 @@ int gps_het_slots(int fam, bool cones, int max_smem_optin) {
     if constexpr (L == 0) {
         return 0;
     } else {
+        constexpr int NI = gps_variant_ni(GPS_HET, gps_pick_NI<T, NX, NU, L>());
         int warps;
-        if (cones) warps = fam == 1 ? gps_warps_max<T, NX, NU, L, 1, 1 | GPS_CONES>(max_smem_optin)
-                                    : gps_warps_max<T, NX, NU, L, 1, 7 | GPS_CONES>(max_smem_optin);
-        else if (fam == 0) warps = gps_warps_max<T, NX, NU, L, 1, 0>(max_smem_optin);
-        else if (fam == 1) warps = gps_warps_max<T, NX, NU, L, 1, 1>(max_smem_optin);
-        else if (fam == 6) warps = gps_warps_max<T, NX, NU, L, 1, 6>(max_smem_optin);
-        else warps = gps_warps_max<T, NX, NU, L, 1, 7>(max_smem_optin);
+        if (cones) warps = fam == 1 ? gps_warps_max<T, NX, NU, L, NI, 1 | GPS_CONES>(max_smem_optin)
+                                    : gps_warps_max<T, NX, NU, L, NI, 7 | GPS_CONES>(max_smem_optin);
+        else if (fam == 0) warps = gps_warps_max<T, NX, NU, L, NI, 0>(max_smem_optin);
+        else if (fam == 1) warps = gps_warps_max<T, NX, NU, L, NI, 1>(max_smem_optin);
+        else if (fam == 6) warps = gps_warps_max<T, NX, NU, L, NI, 6>(max_smem_optin);
+        else warps = gps_warps_max<T, NX, NU, L, NI, 7>(max_smem_optin);
         return warps * (32 / L);
     }
 }

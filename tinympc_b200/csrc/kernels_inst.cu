@@ -47,7 +47,7 @@ int launch_tpi(LaunchDesc *d) {
 
 template <typename T>
 int launch_T(LaunchDesc *d) {
-    if (d->io.models || d->bounds || d->cones || d->planes) return TINYMPC_ERR_UNSUPPORTED;  // per-instance data: the lane-group kernels only
+    if (d->pi.any()) return TINYMPC_ERR_UNSUPPORTED;  // per-instance data: the lane-group kernels only
     if (d->ft.ext) return d->fast ? launch_tpi<T, true, true>(d) : launch_tpi<T, false, true>(d);
     return d->fast ? launch_tpi<T, true, false>(d) : launch_tpi<T, false, false>(d);
 }
@@ -105,10 +105,11 @@ template <typename T, int NX, int NU, bool FAST>
 int launch_gpi(LaunchDesc *d) {
     const int L = d->gpi.L;
     if (L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
-    const bool het = d->io.models != nullptr;  // heterogeneous batch: per-instance model blobs
+    const bool het = d->pi.models;  // heterogeneous batch: per-instance model blobs
     if (d->adapt && (FAST || !het || !d->adapt_args)) return TINYMPC_ERR_UNSUPPORTED;  // adaptive rho: heterogeneous STRICT batches
     if (d->rollout && (FAST || d->adapt || !d->roll_args)) return TINYMPC_ERR_UNSUPPORTED;  // rollouts: STRICT, no adaptive rho
-    if (d->bounds && (FAST || d->adapt || d->rollout)) return TINYMPC_ERR_UNSUPPORTED;  // per-instance bounds: STRICT solves
+    const int bounds = d->pi.read[KIND_BOUNDS];
+    if (bounds && (FAST || d->adapt || d->rollout)) return TINYMPC_ERR_UNSUPPORTED;  // per-instance bounds: STRICT solves
     KParams<T, NX, NU> P;
     fill_params<T, NX, NU>(P, *d);
     if (d->adapt) set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
@@ -128,7 +129,7 @@ int launch_gpi(LaunchDesc *d) {
             if (d->adapt == 2) /* per-instance tables */                                                                 \
                 return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT + GPI_ADAPT_TABLES, false, true>(d, P, gmat);              \
             if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                       \
-            if (d->bounds) /* before MM: the host cannot scan per-instance bounds for signed zeros */                   \
+            if (bounds) /* before MM: the host cannot scan per-instance bounds for signed zeros */                       \
                 return het ? launch_gpi_L<T, NX, NU, LL + GPI_BOUNDS, false, true>(d, P, gmat)                           \
                            : launch_gpi_L<T, NX, NU, LL + GPI_BOUNDS, false, false>(d, P, gmat);                         \
             if constexpr (sizeof(T) == 4)                                                                                \

@@ -92,9 +92,9 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
     P.uref_pi = io.uref_per_instance;
     P.x0 = (const T *)io.x0; P.Xref = (const T *)io.Xref; P.Uref = (const T *)io.Uref;
     P.x_min = (const T *)pd.x_min; P.x_max = (const T *)pd.x_max; P.u_min = (const T *)pd.u_min; P.u_max = (const T *)pd.u_max;
-    if (d.bounds) {  // per-instance bounds replace the problem's; the kernels derive an instance's offset from NX, NU, N and bounds_tv
+    if (d.pi.read[KIND_BOUNDS]) {  // per-instance bounds replace the problem's; the kernels derive an instance's offset from NX, NU, N and bounds_tv
         P.x_min = (const T *)io.x_min; P.x_max = (const T *)io.x_max; P.u_min = (const T *)io.u_min; P.u_max = (const T *)io.u_max;
-        P.bounds_tv = d.bounds == 2;
+        P.bounds_tv = d.pi.read[KIND_BOUNDS] == 2;
     }
     P.Alin_x = (const T *)pd.Alin_x; P.blin_x = (const T *)pd.blin_x; P.Alin_u = (const T *)pd.Alin_u; P.blin_u = (const T *)pd.blin_u;
     P.tv_Alin_x = (const T *)pd.tv_Alin_x; P.tv_blin_x = (const T *)pd.tv_blin_x;
@@ -116,11 +116,11 @@ inline void fill_params(KParams<T, NX, NU> &P, const LaunchDesc &d) {
         tpi_workspace(NX, NU, pd.N, pd.dtype, d.Bpad, ft, (char *)d.tpi_ws, w);
         std::memcpy((char *)&P + offsetof(KP, w_v), w, sizeof(w));
     }
-    if (d.cones) {  // per-instance cone coefficients ride in two workspace pointers the streamed kernel never reads (gps_kernel.cuh: GPS_CONES)
+    if (d.pi.read[KIND_CONES]) {  // per-instance cone coefficients ride in two workspace pointers the streamed kernel never reads (gps_kernel.cuh: GPS_CONES)
         P.w_vc = const_cast<void *>(d.io.cone_x_mu);
         P.w_zc = const_cast<void *>(d.io.cone_u_mu);
     }
-    if (d.planes) {  // per-instance static hyperplanes replace the problem's; the kernel adds the slot's instance offset
+    if (d.pi.read[KIND_PLANES]) {  // per-instance static hyperplanes replace the problem's; the kernel adds the slot's instance offset
         P.Alin_x = (const T *)io.Alin_x; P.blin_x = (const T *)io.blin_x; P.Alin_u = (const T *)io.Alin_u; P.blin_u = (const T *)io.blin_u;
     }
 }

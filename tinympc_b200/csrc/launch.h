@@ -42,6 +42,45 @@ struct Features {
     int soc_x, soc_u, lin_x, lin_u, tvl_x, tvl_u, ext;  // ext: any of them
 };
 
+// The kinds of per-instance data a batch can bring besides models, each with arrays in place of the handle's (capi.cu: KINDS)
+enum InstKind { KIND_BOUNDS, KIND_CONES, KIND_PLANES, NKINDS };
+
+// What a solve's batch brings per instance (given) and what its kernel reads (read).  given[k] is the batch's mode field
+// (bounds: 1 one column, 2 a horizon per instance).  Bounds are read whenever given; cones and hyperplanes only when a loop
+// of theirs runs, else the solve is the one without them.
+struct PerInstance {
+    bool models = false;  // io.models: per-instance models, or the blobs adaptive rho adapts
+    int given[NKINDS] = {}, read[NKINDS] = {};
+    bool any() const {  // does the kernel read any per-instance data?
+        for (int k = 0; k < NKINDS; ++k)
+            if (read[k]) return true;
+        return models;
+    }
+};
+
+// Variant bits of the streamed kernel (gps_kernel.cuh), added to its constraint-family mask (0 box only, 1 cones, 6
+// hyperplanes, 7 both): per-instance models, box bounds, cone coefficients and static hyperplanes
+constexpr int GPS_HET = 8, GPS_BOUNDS = 16, GPS_CONES = 32, GPS_PLANES = 64;
+constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS | GPS_CONES | GPS_PLANES;  // the family-mask bits that are not constraint families
+
+// Which streamed kernels are compiled, for a family mask, variant bits and mode.  FAST: the shared and the per-instance-model
+// solves only.  Per-instance cones with a cone family (1, 7), hyperplanes with a static hyperplane family (6, 7), never
+// with bounds or cones.
+constexpr bool gps_compiled(int fam, int var, bool fast) {
+    if (fast && var != 0 && var != GPS_HET) return false;
+    if ((var & GPS_CONES) && fam != 1 && fam != 7) return false;
+    if ((var & GPS_PLANES) && (fam < 6 || (var & (GPS_BOUNDS | GPS_CONES)))) return false;
+    return true;
+}
+// instances per lane group of a compiled variant: the shared solve's (ni) unless per-instance models or bounds hold a lane
+// group's registers
+constexpr int gps_variant_ni(int var, int ni) { return (var & (GPS_HET | GPS_BOUNDS)) ? 1 : ni; }
+// the variant bits of per-instance data (kinds: PerInstance::given or read)
+inline int gps_variant(bool models, const int (&kinds)[NKINDS]) {
+    return (models ? GPS_HET : 0) | (kinds[KIND_BOUNDS] ? GPS_BOUNDS : 0) | (kinds[KIND_CONES] ? GPS_CONES : 0) |
+           (kinds[KIND_PLANES] ? GPS_PLANES : 0);
+}
+
 struct LaunchDesc {
     const ProblemDesc *pd;
     tinympc_settings_t st;
@@ -66,15 +105,8 @@ struct LaunchDesc {
     // of GpiRoll<T> (rollout.h)
     int rollout;
     const void *roll_args;
-    // per-instance box bounds (io.bounds_per_instance): 0 = the problem's; 1 = io.x_min ... u_max hold one column per instance;
-    // 2 = they hold a horizon per instance.  The lane-group kernels' GPI_BOUNDS / GPS_BOUNDS variants read them.
-    int bounds;
-    // per-instance cone coefficients (io.cones_per_instance) with a cone loop that runs: io.cone_x_mu / cone_u_mu hold [B][ncx] /
-    // [B][ncu].  The streamed kernel's GPS_CONES variants read them.
-    int cones;
-    // per-instance static hyperplanes (io.planes_per_instance) with a static hyperplane loop that runs: io.Alin_x / blin_x /
-    // Alin_u / blin_u hold [B][nx][nlx] / [B][nlx] / [B][nu][nlu] / [B][nlu].  The streamed kernel's GPS_PLANES variants read them.
-    int planes;
+    // per-instance data: the lane-group kernels' GPI_BOUNDS and GPS_HET / BOUNDS / CONES / PLANES variants read io's arrays
+    PerInstance pi;
 
     cudaStream_t stream;
     int sm_count;

@@ -19,7 +19,7 @@ import numpy as np
 
 from . import abi
 from ._lib import check, load
-from .batch import BOUND_NAMES, CONE_NAMES, PLANE_NAMES, HostBatch, bounds_layout, cones_check, num_planes, planes_abi, planes_check
+from .batch import KINDS, HostBatch, per_instance, problem_dims
 from .problem import MPCProblem, copy_settings, default_settings, dtype_code
 from .workloads import ModelSpec
 
@@ -360,26 +360,13 @@ class BatchedTinySolver:
         models_t = None if models is None else t(models)
         tens["models"] = models_t
         b.models = None if models_t is None else models_t.data_ptr()
-        if bounds is not None:
-            b.bounds_per_instance = bounds_layout(bounds, B, p.N, p.nx, p.nu, p.dtype)
-            bt = {k: t(v) for k, v in bounds.items() if v is not None}
-            for k in BOUND_NAMES:
-                setattr(b, k, bt[k].data_ptr() if k in bt else None)
-            tens["bounds"] = bt
-        if cones is not None:
-            cones_check(cones, B, len(p.Acx), len(p.Acu), p.dtype)
-            ct = {k: t(v) for k, v in cones.items() if v is not None}
-            b.cones_per_instance = 1
-            for k in CONE_NAMES:
-                setattr(b, "cone_" + k, ct[k].data_ptr() if k in ct else None)
-            tens["cones"] = ct
-        if planes is not None:
-            planes_check(planes, B, *num_planes(p), p.nx, p.nu, p.dtype)
-            pt = {k: t(v) for k, v in planes_abi(planes).items()}
-            b.planes_per_instance = 1
-            for k in PLANE_NAMES:
-                setattr(b, k, pt[k].data_ptr() if k in pt else None)
-            tens["planes"] = pt
+        for kind, arrays in dict(bounds=bounds, cones=cones, planes=planes).items():
+            if arrays is not None:
+                mode, abi_arrays = per_instance(kind, arrays, B, problem_dims(p), p.dtype)
+                tens[kind] = {f: t(a) for f, a in abi_arrays.items()}
+                setattr(b, KINDS[kind].mode_field, mode)
+                for f in KINDS[kind].fields.values():
+                    setattr(b, f, tens[kind][f].data_ptr() if f in tens[kind] else None)
         b.iter, b.solved = out["iter"].data_ptr(), out["solved"].data_ptr()
         b.residuals = None if out["residuals"] is None else out["residuals"].data_ptr()
         res = dict(out)
