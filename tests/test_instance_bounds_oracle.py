@@ -1,38 +1,17 @@
-"""CPU checks of per-instance box bounds (tinympc_batch_t.bounds_per_instance): the ctypes mirror of the new batch fields
-matches the header, and the palette helper the GPU tests compare against (bounds_common.grouped_oracle) equals the unmodified
+"""CPU checks of per-instance box bounds (tinympc_batch_t.bounds_per_instance): the ctypes mirror of the batch fields matches
+the header, and the grouped helper the GPU tests compare against (instance_common.grouped_oracle) equals the unmodified
 reference run once per instance, each with its own tiny_set_bound_constraints, bit for bit."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
-
 import numpy as np
 import pytest
 
-import bounds_common as BC
 import helpers as H
+import instance_common as IC
 from oracle import oracle
-from tinympc_b200 import abi, workloads as wl
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-FIELDS = ["models", "x_min", "x_max", "u_min", "u_max", "bounds_per_instance", "reserved2"]
+from tinympc_b200 import workloads as wl
 
 
 def test_batch_bounds_fields_match_header():
-    src = "#include <stdio.h>\n#include <stddef.h>\n#include \"tinympc_b200.h\"\nint main(void){\n"
-    src += '  printf("%zu\\n", sizeof(tinympc_batch_t));\n'
-    src += "".join(f'  printf("%zu\\n", offsetof(tinympc_batch_t, {n}));\n' for n in FIELDS)
-    src += "  return 0; }\n"
-    with tempfile.TemporaryDirectory() as td:
-        c = os.path.join(td, "probe.c")
-        open(c, "w").write(src)
-        exe = os.path.join(td, "probe")
-        subprocess.check_call(["/usr/bin/gcc", "-std=c11", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
-        out = list(map(int, subprocess.check_output([exe], text=True).split()))
-    assert out[0] == C.sizeof(abi.Batch)
-    assert out[1:] == [getattr(abi.Batch, n).offset for n in FIELDS]
-    assert abi.Batch().bounds_per_instance == 0 and abi.Batch().reserved2 == 0  # a zero-initialised batch: the handle's bounds
+    IC.assert_batch_fields_match_header("bounds")
 
 
 OUT = H.OUT_KEYS + H.BOX_STATE
@@ -52,14 +31,14 @@ def test_palette_helper_equals_reference_per_instance(dt, layout):
     st.max_iter = 40
     inst = wl.tracking_instances(12, N=spec.N, seed=11, dtype=dt)
     x0, Xref = inst["x0"], inst["Xref"]
-    pal = BC.palette(prob, 6, layout, seed=3, scale=0.5, tight=0.9) + BC.palette(prob, 6, layout, seed=4, scale=0.3, zeros=True)
-    which = BC.deal(12, 12, stride=5)
-    helper = BC.grouped_oracle(prob, st, pal, which, nthreads=4)
+    pal = IC.palette(prob, 6, layout, seed=3, scale=0.5, tight=0.9) + IC.palette(prob, 6, layout, seed=4, scale=0.3, zeros=True)
+    which = IC.deal(12, 12, stride=5)
+    helper = IC.grouped_oracle(prob, st, bounds=IC.batch_bounds(pal, which), nthreads=4)
 
     def reference(x0_, state, cold):
         outs = []
         for b in range(12):
-            p = BC.with_bounds(prob, pal[which[b]])
+            p = IC.with_instance(prob, "bounds", pal[which[b]])
             sub = None if state is None else {n: np.array(a[b:b + 1], copy=True) for n, a in state.items()}
             xr = Xref[b:b + 1] if Xref.ndim == 3 else Xref
             outs.append(oracle.solve_batch(p, st, x0_[b:b + 1], xr, None, state=sub, cold_start=cold,

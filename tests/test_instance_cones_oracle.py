@@ -1,42 +1,17 @@
-"""CPU checks of per-instance cone coefficients (tinympc_batch_t.cones_per_instance): the ctypes mirror of the new batch fields
-matches the header, and the helper the GPU tests compare against (cones_common.grouped_oracle) equals the unmodified
-reference run once per instance, each with its own tiny_set_cone_constraints, bit for bit."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
-
+"""CPU checks of per-instance cone coefficients (tinympc_batch_t.cones_per_instance): the ctypes mirror of the batch fields
+matches the header, and the grouped helper the GPU tests compare against (instance_common.grouped_oracle) equals the
+unmodified reference run once per instance, each with its own tiny_set_cone_constraints, bit for bit."""
 import numpy as np
 import pytest
 
-import cones_common as CC
 import helpers as H
+import instance_common as IC
 from oracle import oracle
-from tinympc_b200 import abi, workloads as wl
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-FIELDS = ["cone_x_mu", "cone_u_mu", "cones_per_instance", "reserved3"]
+from tinympc_b200 import workloads as wl
 
 
 def test_batch_cones_fields_match_header():
-    src = "#include <stdio.h>\n#include <stddef.h>\n#include \"tinympc_b200.h\"\nint main(void){\n"
-    src += '  printf("%zu\\n", sizeof(tinympc_batch_t));\n'
-    src += "".join(f'  printf("%zu\\n", offsetof(tinympc_batch_t, {n}));\n' for n in FIELDS)
-    src += "  return 0; }\n"
-    with tempfile.TemporaryDirectory() as td:
-        c = os.path.join(td, "probe.c")
-        open(c, "w").write(src)
-        exe = os.path.join(td, "probe")
-        subprocess.check_call(["/usr/bin/gcc", "-std=c11", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
-        out = list(map(int, subprocess.check_output([exe], text=True).split()))
-    assert out[0] == C.sizeof(abi.Batch)
-    assert out[1:] == [getattr(abi.Batch, n).offset for n in FIELDS]
-    # the new fields come after every field of the previous layout
-    assert abi.Batch.cone_x_mu.offset >= abi.Batch.reserved2.offset + 4
-    b = abi.Batch()
-    assert b.cones_per_instance == 0 and b.reserved3 == 0  # a zero-initialised batch: the handle's cx / cu
-    assert b.cone_x_mu is None and b.cone_u_mu is None
+    IC.assert_batch_fields_match_header("cones")
 
 
 OUT = H.OUT_KEYS + H.SOC_STATE
@@ -64,17 +39,17 @@ def test_cone_helper_equals_reference_per_instance(dt):
     x0, Xref, Uref = inst["x0"], inst["Xref"], inst["Uref"]
     x0[::3, 2] = -np.abs(x0[::3, 2]) - 1.0  # below the landing plane: the state cone's apex branch
     extra = [(0.3, 0.55), (0.55, 0.3)] if dt == np.float64 else [(0.3, 0.55)]
-    pal = CC.mu_palette(prob, 8, seed=2, scale=(0.2, 1.0)) + CC.mu_palette(prob, 8 - len(extra), seed=3, scale=(2.0, 12.0), extra=extra)
+    pal = IC.mu_palette(prob, 8, seed=2, scale=(0.2, 1.0)) + IC.mu_palette(prob, 8 - len(extra), seed=3, scale=(2.0, 12.0), extra=extra)
     which = (np.arange(B) * 5) % B
-    cones = CC.batch_cones(pal, which)
+    cones = IC.batch_cones(pal, which)
     if dt == np.float64:
         assert np.any(cones["x_mu"] == 0.3) and np.float64(np.float32(0.3)) != 0.3
-    helper = CC.grouped_oracle(prob, st, cones, nthreads=4)
+    helper = IC.grouped_oracle(prob, st, cones=cones, nthreads=4)
 
     def reference(x0_, state, cold):
         outs = []
         for b in range(B):
-            p = CC.with_cones(prob, cones["x_mu"][b], cones["u_mu"][b])
+            p = IC.with_instance(prob, "cones", {k: a[b] for k, a in cones.items()})
             sub = None if state is None else {n: np.array(a[b:b + 1], copy=True) for n, a in state.items()}
             outs.append(oracle.solve_batch(p, st, x0_[b:b + 1], Xref[b:b + 1], Uref[b:b + 1], state=sub, cold_start=cold,
                                            want_state=tuple(H.SOC_STATE), impl="reference"))
@@ -84,12 +59,12 @@ def test_cone_helper_equals_reference_per_instance(dt):
     r1 = reference(x0, None, True)
     H.assert_bits_per_instance(h1, r1, OUT, "cold")
     # the projections bite: instances land in each of project_soc's three branches, on the state or the input side
-    bx = CC.soc_branches(h1["vcnew"], prob.Acx, cones["x_mu"])
-    bu = CC.soc_branches(h1["zcnew"], prob.Acu, cones["u_mu"])
+    bx = IC.soc_branches(h1["vcnew"], prob.Acx, cones["x_mu"])
+    bu = IC.soc_branches(h1["zcnew"], prob.Acu, cones["u_mu"])
     counts = [int(np.sum(a | b)) for a, b in zip(bx, bu)]
     assert all(c >= 2 for c in counts), f"instances per branch (below, inside, projected): {counts}"
     # the coefficients matter: the same batch with the problem's own mu differs for most instances
-    shared = CC.grouped_oracle(prob, st, {"x_mu": np.tile(prob.cx, (B, 1)), "u_mu": np.tile(prob.cu, (B, 1))}, nthreads=4)
+    shared = IC.grouped_oracle(prob, st, cones={"x_mu": np.tile(prob.cx, (B, 1)), "u_mu": np.tile(prob.cu, (B, 1))}, nthreads=4)
     s1 = shared(x0, Xref, Uref, None, True, H.SOC_STATE)
     differ = [not np.array_equal(s1["sol_u"][b], h1["sol_u"][b]) for b in range(B)]
     assert sum(differ) >= B // 2, differ
@@ -110,20 +85,6 @@ def test_cone_helper_groups_by_distinct_mu(monkeypatch):
     st.max_iter = 20
     B = 9
     inst = wl.rocket_instances(B, N=spec.N, seed=1, dtype=dt)
-    pal = [dict(x_mu=prob.cx.copy(), u_mu=prob.cu.copy())] + CC.mu_palette(prob, 2, seed=9)
+    pal = [dict(x_mu=prob.cx.copy(), u_mu=prob.cu.copy())] + IC.mu_palette(prob, 2, seed=9)
     which = np.arange(B) % 3
-    cones = CC.batch_cones(pal, which)
-    calls = []
-    real = oracle.solve_batch
-
-    def counting(*a, **k):
-        calls.append(len(a[2]))
-        return real(*a, **k)
-
-    monkeypatch.setattr(oracle, "solve_batch", counting)
-    got = CC.grouped_oracle(prob, st, cones, nthreads=2)(inst["x0"], inst["Xref"], inst["Uref"], None, True, ())
-    monkeypatch.undo()
-    assert sorted(calls) == [3, 3, 3]
-    ref = oracle.solve_batch(prob, st, inst["x0"], inst["Xref"], inst["Uref"], cold_start=True, nthreads=2)
-    for k in H.OUT_KEYS:
-        assert H.bits_equal(got[k][which == 0], ref[k][which == 0]), k
+    IC.assert_one_run_per_set(monkeypatch, prob, st, inst["x0"], inst["Xref"], inst["Uref"], which, cones=IC.batch_cones(pal, which))

@@ -1,43 +1,19 @@
-"""CPU checks of per-instance static hyperplanes (tinympc_batch_t.planes_per_instance): the ctypes mirror of the new batch
-fields matches the header, and the helper the GPU tests compare against (planes_common.grouped_oracle) equals the unmodified
-reference run once per instance, each with its own tiny_set_linear_constraints, bit for bit."""
-import ctypes as C
-import os
-import subprocess
-import tempfile
-
+"""CPU checks of per-instance static hyperplanes (tinympc_batch_t.planes_per_instance): the ctypes mirror of the batch fields
+matches the header, the check and layout of the arrays, and the grouped helper the GPU tests compare against
+(instance_common.grouped_oracle) equals the unmodified reference run once per instance, each with its own
+tiny_set_linear_constraints, bit for bit."""
 import numpy as np
 import pytest
 
 import helpers as H
-import planes_common as PC
+import instance_common as IC
 from oracle import oracle
-from tinympc_b200 import abi, workloads as wl
+from tinympc_b200 import workloads as wl
 from tinympc_b200.batch import planes_abi, planes_check
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-FIELDS = ["Alin_x", "blin_x", "Alin_u", "blin_u", "planes_per_instance", "reserved4"]
 
 
 def test_batch_planes_fields_match_header():
-    src = "#include <stdio.h>\n#include <stddef.h>\n#include \"tinympc_b200.h\"\nint main(void){\n"
-    src += '  printf("%zu\\n", sizeof(tinympc_batch_t));\n'
-    src += "".join(f'  printf("%zu\\n", offsetof(tinympc_batch_t, {n}));\n' for n in FIELDS)
-    src += "  return 0; }\n"
-    with tempfile.TemporaryDirectory() as td:
-        c = os.path.join(td, "probe.c")
-        open(c, "w").write(src)
-        exe = os.path.join(td, "probe")
-        subprocess.check_call(["/usr/bin/gcc", "-std=c11", "-I", os.path.join(ROOT, "include"), c, "-o", exe])
-        out = list(map(int, subprocess.check_output([exe], text=True).split()))
-    assert out[0] == C.sizeof(abi.Batch)
-    assert out[1:] == [getattr(abi.Batch, n).offset for n in FIELDS]
-    # the new fields come after every field of the previous layout
-    assert abi.Batch.Alin_x.offset >= abi.Batch.reserved3.offset + 4
-    b = abi.Batch()
-    assert b.planes_per_instance == 0 and b.reserved4 == 0  # a zero-initialised batch: the handle's hyperplanes
-    assert b.Alin_x is None and b.blin_x is None and b.Alin_u is None and b.blin_u is None
+    IC.assert_batch_fields_match_header("planes")
 
 
 def test_planes_check_and_layout():
@@ -81,15 +57,15 @@ def test_plane_helper_equals_reference_per_instance(dt):
     st = spec.settings
     B = 16
     x0, Xref = _instances(spec, B, dt)
-    pal = PC.plane_palette(prob, 12, seed=2)
+    pal = IC.plane_palette(prob, 12, seed=2)
     which = (np.arange(B) * 5) % 12
-    planes = PC.batch_planes(pal, which)
-    helper = PC.grouped_oracle(prob, st, planes, nthreads=4)
+    planes = IC.batch_planes(pal, which)
+    helper = IC.grouped_oracle(prob, st, planes=planes, nthreads=4)
 
     def reference(x0_, state, cold):
         outs = []
         for b in range(B):
-            p = PC.with_planes(prob, {k: v[b] for k, v in planes.items()})
+            p = IC.with_instance(prob, "planes", {k: v[b] for k, v in planes.items()})
             sub = None if state is None else {n: np.array(a[b:b + 1], copy=True) for n, a in state.items()}
             outs.append(oracle.solve_batch(p, st, x0_[b:b + 1], Xref[b:b + 1], None, state=sub, cold_start=cold,
                                            want_state=tuple(H.LIN_STATE), impl="reference"))
@@ -99,7 +75,7 @@ def test_plane_helper_equals_reference_per_instance(dt):
     r1 = reference(x0, None, True)
     H.assert_bits_per_instance(h1, r1, OUT, "cold")
     # the planes bite: most instances end with a slack on one of their planes
-    act = PC.active_rows(planes, h1["vlnew"], h1["zlnew"])
+    act = IC.active_rows(planes, h1["vlnew"], h1["zlnew"])
     assert act.sum() >= (3 * B) // 4, act
     # and they matter: the same batch with the problem's own planes differs for at least half of the instances
     shared = oracle.solve_batch(prob, st, x0, Xref, None, cold_start=True, nthreads=4)
@@ -121,7 +97,7 @@ def test_padding_rows_are_inert(dt):
     st = spec.settings
     B = 8
     x0, Xref = _instances(spec, B, dt)
-    pset = PC.plane_palette(prob, 1, seed=7)[0]
+    pset = IC.plane_palette(prob, 1, seed=7)[0]
     # the problem with one extra state row and one extra input row, which this robot pads with zeros
     cons = dict(spec0.constraints)
     cons["Alin_x"] = np.vstack([pset["Alin_x"], np.zeros((1, prob.nx))])
@@ -130,7 +106,7 @@ def test_padding_rows_are_inert(dt):
     cons["blin_u"] = np.concatenate([pset["blin_u"], [0.0]])
     spec0.constraints = cons
     padded = H.problem_from_spec(spec0, dt, oracle.port_setup)
-    plain = PC.with_planes(padded, pset)
+    plain = IC.with_instance(padded, "planes", pset)
     assert padded.Alin_x.shape[0] == plain.Alin_x.shape[0] + 1
     a = oracle.solve_batch(padded, st, x0, Xref, None, cold_start=True, want_state=tuple(H.LIN_STATE), nthreads=4)
     b = oracle.solve_batch(plain, st, x0, Xref, None, cold_start=True, want_state=tuple(H.LIN_STATE), nthreads=4)
@@ -146,23 +122,9 @@ def test_plane_helper_groups_by_distinct_set(monkeypatch):
     st = spec.settings
     B = 9
     x0, Xref = _instances(spec, B, dt, seed=1)
-    pal = [PC.own_planes(prob)] + PC.plane_palette(prob, 2, seed=9)
+    pal = [IC.own_planes(prob)] + IC.plane_palette(prob, 2, seed=9)
     which = np.arange(B) % 3
-    planes = PC.batch_planes(pal, which)
-    calls = []
-    real = oracle.solve_batch
-
-    def counting(*a, **k):
-        calls.append(len(a[2]))
-        return real(*a, **k)
-
-    monkeypatch.setattr(oracle, "solve_batch", counting)
-    got = PC.grouped_oracle(prob, st, planes, nthreads=2)(x0, Xref, None, None, True, ())
-    monkeypatch.undo()
-    assert sorted(calls) == [3, 3, 3]
-    ref = oracle.solve_batch(prob, st, x0, Xref, None, cold_start=True, nthreads=2)
-    for k in H.OUT_KEYS:
-        assert H.bits_equal(got[k][which == 0], ref[k][which == 0]), k
+    IC.assert_one_run_per_set(monkeypatch, prob, st, x0, Xref, None, which, planes=IC.batch_planes(pal, which))
 
 
 def test_plane_fleet_is_seeded_and_keeps_structure():
