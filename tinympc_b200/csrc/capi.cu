@@ -274,6 +274,17 @@ struct SolvePlan {
 // shared memory the adaptive kernel adds per CTA for its tables
 size_t adapt_smem(const tinympc_b200_solver *s) { return tmpc::gpi_adapt_bytes(s->pd.nx, s->pd.nu, esize(s->pd.dtype)); }
 
+// The entry points only an on-chip kernel variant serves (rollouts, adaptive rho): the variant bits, and plan_solve's
+// refusals in the order it checks them (mode, constraint families, kernel family, horizon)
+struct OnChipOnly {
+    int bits;
+    const char *strict, *box, *family, *fit;
+} const ONCHIP_ONLY[2] = {
+    {tmpc::GPI_ROLLOUT, "rollouts are available in STRICT mode only", "rollouts cover box constraints only (no cones or hyperplanes)",
+     "rollouts run on the on-chip (GPI) kernel family only", "rollout: the horizon does not fit the on-chip kernel"},
+    {tmpc::GPI_ADAPT, "adaptive rho is available in STRICT mode only", "adaptive rho covers box constraints only (no cones or hyperplanes)",
+     "adaptive rho runs on the on-chip (GPI) kernel family only", "adaptive rho: the horizon does not fit the on-chip kernel"}};
+
 // The plan of a solve of B instances (pi: its per-instance data; adapt: adaptive rho).  GPI = lane groups, state on chip (box
 // constraints, horizon fits in shared memory); GPS = lane groups, state streamed (everything else the lane mapping covers);
 // TPI = one thread per instance.  Fails when an explicit request or a feature cannot be served.
@@ -296,25 +307,17 @@ int plan_solve(const tinympc_b200_solver *s, const tmpc::PerInstance &pi, bool a
             return fail(TINYMPC_ERR_UNSUPPORTED, std::string("per-instance ") + kd.noun + " do not combine with per-instance " +
                                                      kd.exclusive + " in one batch");
     }
-    if (rollout) {  // closed-loop rollout: the on-chip kernel's rollout variant, with the on-chip plan a solve would use
-        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts are available in STRICT mode only");
-        if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts cover box constraints only (no cones or hyperplanes)");
-        if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "rollouts run on the on-chip (GPI) kernel family only");
-        p->gpi = s->dim->gpi_plan(s->pd.dtype, s->pd.N, s->max_smem_optin);
-        if (p->gpi.smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "rollout: the horizon does not fit the on-chip kernel");
-        p->family = TINYMPC_KERNEL_GPI;
-        p->per_cta = p->gpi.instances_per_cta;
-        return 0;
-    }
-    if (adapt) {  // adaptive rho: the on-chip kernel's adaptive variant, whose tables take shared memory
-        if (s->mode == TINYMPC_MODE_FAST) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho is available in STRICT mode only");
-        if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho covers box constraints only (no cones or hyperplanes)");
-        if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS)
-            return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho runs on the on-chip (GPI) kernel family only");
-        const size_t tables = adapt_smem(s);
+    if (rollout || adapt) {  // the on-chip kernel's variant, with the on-chip plan a solve would use less the adaptive tables
+        const OnChipOnly &oc = ONCHIP_ONLY[rollout ? 0 : 1];
+        bool compiled = false;  // some on-chip kernel serves the variant in this mode (adaptive rho adapts per-instance blobs)
+        for (int L : {4, 8, 16})
+            compiled |= tmpc::gpi_compiled(L, oc.bits, adapt || pi.models, false, s->mode == TINYMPC_MODE_FAST, s->pd.dtype == TINYMPC_F64);
+        if (!compiled) return fail(TINYMPC_ERR_UNSUPPORTED, oc.strict);
+        if (ft.ext) return fail(TINYMPC_ERR_UNSUPPORTED, oc.box);
+        if (s->family == TINYMPC_KERNEL_TPI || s->family == TINYMPC_KERNEL_GPS) return fail(TINYMPC_ERR_UNSUPPORTED, oc.family);
+        const size_t tables = oc.bits == tmpc::GPI_ADAPT ? adapt_smem(s) : 0;
         p->gpi = s->dim->gpi_plan(s->pd.dtype, s->pd.N, s->max_smem_optin - (int)tables);
-        if (p->gpi.smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, "adaptive rho: the horizon does not fit the on-chip kernel");
+        if (p->gpi.smem <= 0) return fail(TINYMPC_ERR_UNSUPPORTED, oc.fit);
         p->gpi.smem += tables;
         p->family = TINYMPC_KERNEL_GPI;
         p->per_cta = p->gpi.instances_per_cta;

@@ -65,25 +65,7 @@ __host__ __device__ constexpr bool gpi_feasible() {
 
 constexpr int GPI_MAX_WARPS = 8;
 
-// Adaptive rho (tinympc_b200_solve_adaptive): the kernel is instantiated with GPI_ADAPT added to its lane count; it then
-// runs heterogeneous STRICT batches and reads its GpiAdapt arguments (adapt.h: gpi_adapt_args).  (A separate template
-// parameter or kernel argument would rename the existing kernels, a shared __device__ body or a larger KParams changes their
-// machine code.)
-constexpr int GPI_ADAPT = 64;
-// ... with per-instance sensitivity tables (tinympc_adaptive_rho_t.tables_per_instance): added on top of GPI_ADAPT.  A variant of
-// its own, so that the shared-table adaptive kernel keeps its machine code (a run-time choice between the staged and the
-// per-instance tables cost it 2-3 %, DESIGN.md §5.5).
-constexpr int GPI_ADAPT_TABLES = 128;
-// Closed-loop rollout (tinympc_b200_rollout): the kernel runs GpiRoll::steps warm-started MPC steps per instance and reads its
-// GpiRoll arguments (rollout.h: gpi_roll_args).  Encoded in the lane parameter for the same reason as GPI_ADAPT; never combined
-// with it.
-constexpr int GPI_ROLLOUT = 256;
-// Per-instance box bounds (tinympc_batch_t.bounds_per_instance): P.x_min ... u_max point at the batch's [B][nx] / [B][nu] columns
-// (P.bounds_tv == 0) or [B][N][nx] / [B][N-1][nu] horizons (P.bounds_tv == 1), and every slot loads its instance's column 0 when it
-// is refilled.  Encoded in the lane parameter for the same reason as GPI_ADAPT; STRICT only, never with MM, GPI_ADAPT or
-// GPI_ROLLOUT (the host cannot tell whether a per-instance bound is a signed zero, so the clamp stays compare-select).
-constexpr int GPI_BOUNDS = 512;
-
+// LA: the lane count plus the variant bits (launch.h: GPI_ADAPT ... GPI_BOUNDS).
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
 template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
@@ -94,11 +76,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     constexpr bool ROLL = (LA & GPI_ROLLOUT) != 0;        // closed-loop rollout
     constexpr bool BND = (LA & GPI_BOUNDS) != 0;          // per-instance box bounds
     constexpr int L = LA % GPI_ADAPT;
-    static_assert(LA < 2 * GPI_BOUNDS && L > 0 && (ADAPT || !PERTAB) && !(ADAPT && ROLL),
-                  "lane count: 4, 8 or 16, plus GPI_ADAPT (and GPI_ADAPT_TABLES) for the adaptive variants, GPI_ROLLOUT or GPI_BOUNDS");
-    static_assert(!ADAPT || (HET && !FAST && !MM), "adaptive rho runs on heterogeneous STRICT batches");
-    static_assert(!ROLL || !FAST, "rollouts run in STRICT mode");
-    static_assert(!BND || (!FAST && !MM && !ADAPT && !ROLL), "per-instance bounds run in STRICT mode, alone");
+    static_assert(gpi_compiled(L, LA - L, HET, MM, FAST, sizeof(T) == 8), "a variant gpi_compiled does not admit");
     GpiAdapt<T> AP{};
     if constexpr (ADAPT) AP = *gpi_adapt_args<T>(P);
     const GpiRoll<T> *RP = nullptr;
@@ -1373,8 +1351,8 @@ inline GpiPlan gpi_plan(int N, int max_smem) {
     return p;
 }
 
-// launch the kernel of lane parameter LA (the lane count L, plus GPI_ADAPT [+ GPI_ADAPT_TABLES] for adaptive rho) with the plan d->gpi (d->gpi.L == L;
-// for adaptive rho its smem includes gpi_adapt_bytes)
+// launch the kernel of lane parameter LA (the lane count L plus its variant bits) with the plan d->gpi (d->gpi.L == L; for
+// adaptive rho its smem includes gpi_adapt_bytes)
 template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
 int launch_gpi_L(LaunchDesc *d, const KParams<T, NX, NU> &P, const T *gmat) {
     constexpr int L = LA % GPI_ADAPT;

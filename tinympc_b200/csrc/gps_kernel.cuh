@@ -225,11 +225,8 @@ __global__ void __launch_bounds__(gps_max_warps(NI) * 32, 1)
     constexpr bool CN = (FAMH & GPS_CONES) != 0;    // per-instance cone coefficients
     constexpr bool PL = (FAMH & GPS_PLANES) != 0;   // per-instance static hyperplanes
     constexpr int FAM = FAMH & ~GPS_VARIANTS;       // constraint families compiled in
-    static_assert(!HET || NI == 1, "per-instance models run one instance per lane group");
-    static_assert(!BND || (NI == 1 && !FAST), "per-instance bounds run one instance per lane group, in STRICT mode");
-    static_assert(!CN || ((FAM & 1) != 0 && !FAST), "per-instance cone coefficients need the cone family, in STRICT mode");
-    static_assert(!PL || ((FAM & 2) != 0 && !FAST && !BND && !CN),
-                  "per-instance hyperplanes need the static hyperplane family, in STRICT mode, without per-instance bounds or cones");
+    static_assert(gps_compiled(FAM, FAMH & GPS_VARIANTS, FAST) && gps_variant_ni(FAMH & GPS_VARIANTS, NI) == NI,
+                  "a variant gps_compiled does not admit, or NI > 1 where per-instance models or bounds hold a lane group");
     using Cfg = GpsCfg<NX, NU, L, (int)sizeof(T), NI, FAM>;
     using REC = GpsRec<NX, NU, Cfg::SPW, (int)sizeof(T), FAM>;
     constexpr int RX = Cfg::RX, RU = Cfg::RU, IPW = Cfg::IPW, W = Cfg::W, NXP = Cfg::NXP, NUP = Cfg::NUP;
@@ -1233,25 +1230,6 @@ int launch_gps_cfg(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
 inline int gps_family_mask(bool soc, bool lin) { return !soc && !lin ? 0 : (soc && !lin ? 1 : (!soc ? 6 : 7)); }
 constexpr int GPS_FAMILY_MASKS[4] = {0, 1, 6, 7};
 
-// case I of the walk over (family mask, variant bits): launch its kernel when it is compiled and (fam, var) selects it
-template <typename T, int NX, int NU, int L, int NI, bool FAST, int I>
-bool gps_launch_case(LaunchDesc *d, const KParams<T, NX, NU> &P0, int fam, int var, int *rc) {
-    constexpr int FF = GPS_FAMILY_MASKS[I / 16], VV = (I % 16) * GPS_HET;
-    if constexpr (gps_compiled(FF, VV, FAST)) {
-        if (fam == FF && var == VV) {
-            *rc = launch_gps_cfg<T, NX, NU, L, gps_variant_ni(VV, NI), FF | VV, FAST>(d, P0);
-            return true;
-        }
-    }
-    return false;
-}
-template <typename T, int NX, int NU, int L, int NI, bool FAST, int... I>
-int gps_launch_walk(LaunchDesc *d, const KParams<T, NX, NU> &P0, int fam, int var, std::integer_sequence<int, I...>) {
-    int rc = TINYMPC_ERR_UNSUPPORTED;
-    (gps_launch_case<T, NX, NU, L, NI, FAST, I>(d, P0, fam, var, &rc) || ...);
-    return rc;
-}
-
 // the streamed kernel of the solve's constraint families and per-instance data (launch.h: gps_compiled); a variant that is
 // not compiled is TINYMPC_ERR_UNSUPPORTED
 template <typename T, int NX, int NU, bool FAST>
@@ -1261,8 +1239,16 @@ int launch_gps(LaunchDesc *d, const KParams<T, NX, NU> &P0) {
         return TINYMPC_ERR_UNSUPPORTED;
     } else {
         const int fam = gps_family_mask(d->ft.soc_x || d->ft.soc_u, d->ft.lin_x || d->ft.lin_u || d->ft.tvl_x || d->ft.tvl_u);
-        return gps_launch_walk<T, NX, NU, L, gps_pick_NI<T, NX, NU, L>(), FAST>(d, P0, fam, gps_variant(d->pi.models, d->pi.read),
-                                                                              std::make_integer_sequence<int, 4 * 16>());
+        const int var = gps_variant(d->pi.models, d->pi.read);
+        constexpr int NI = gps_pick_NI<T, NX, NU, L>();
+        int rc = TINYMPC_ERR_UNSUPPORTED;
+        walk_cases([&](auto i) {  // case i: family mask, variant bits
+            constexpr int FF = GPS_FAMILY_MASKS[decltype(i)::value / 16], VV = decltype(i)::value % 16 * GPS_HET;
+            if constexpr (gps_compiled(FF, VV, FAST))
+                if (fam == FF && var == VV)
+                    rc = launch_gps_cfg<T, NX, NU, L, gps_variant_ni(VV, NI), FF | VV, FAST>(d, P0);
+        }, std::make_integer_sequence<int, 4 * 16>());
+        return rc;
     }
 }
 
@@ -1276,13 +1262,12 @@ int gps_het_slots(int fam, bool cones, int max_smem_optin) {
         return 0;
     } else {
         constexpr int NI = gps_variant_ni(GPS_HET, gps_pick_NI<T, NX, NU, L>());
-        int warps;
-        if (cones) warps = fam == 1 ? gps_warps_max<T, NX, NU, L, NI, 1 | GPS_CONES>(max_smem_optin)
-                                    : gps_warps_max<T, NX, NU, L, NI, 7 | GPS_CONES>(max_smem_optin);
-        else if (fam == 0) warps = gps_warps_max<T, NX, NU, L, NI, 0>(max_smem_optin);
-        else if (fam == 1) warps = gps_warps_max<T, NX, NU, L, NI, 1>(max_smem_optin);
-        else if (fam == 6) warps = gps_warps_max<T, NX, NU, L, NI, 6>(max_smem_optin);
-        else warps = gps_warps_max<T, NX, NU, L, NI, 7>(max_smem_optin);
+        int warps = 0;
+        walk_cases([&](auto i) {  // case i: family mask, per-instance cone coefficients
+            constexpr int FF = GPS_FAMILY_MASKS[decltype(i)::value / 2], CC = decltype(i)::value % 2 * GPS_CONES;
+            if constexpr (gps_compiled(FF, CC, false))
+                if (fam == FF && cones == (CC != 0)) warps = gps_warps_max<T, NX, NU, L, NI, FF | CC>(max_smem_optin);
+        }, std::make_integer_sequence<int, 4 * 2>());
         return warps * (32 / L);
     }
 }

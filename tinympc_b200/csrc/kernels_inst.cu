@@ -100,51 +100,25 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
 namespace tmpc {
 namespace {
 
-// the plan d->gpi comes from the caller (capi.cu: plan_solve, through the DimEntry's gpi_plan)
+// the on-chip kernel of the solve's variant (launch.h: gpi_variant, gpi_compiled) with the plan d->gpi, which comes from the
+// caller (capi.cu: plan_solve, through the DimEntry's gpi_plan); a variant that is not compiled is TINYMPC_ERR_UNSUPPORTED
 template <typename T, int NX, int NU, bool FAST>
 int launch_gpi(LaunchDesc *d) {
-    const int L = d->gpi.L;
-    if (L == 0 || !d->work_queue) return TINYMPC_ERR_UNSUPPORTED;
-    const bool het = d->pi.models;  // heterogeneous batch: per-instance model blobs
-    if (d->adapt && (FAST || !het || !d->adapt_args)) return TINYMPC_ERR_UNSUPPORTED;  // adaptive rho: heterogeneous STRICT batches
-    if (d->rollout && (FAST || d->adapt || !d->roll_args)) return TINYMPC_ERR_UNSUPPORTED;  // rollouts: STRICT, no adaptive rho
-    const int bounds = d->pi.read[KIND_BOUNDS];
-    if (bounds && (FAST || d->adapt || d->rollout)) return TINYMPC_ERR_UNSUPPORTED;  // per-instance bounds: STRICT solves
+    if (d->gpi.L == 0 || !d->work_queue || (d->adapt && !d->adapt_args) || (d->rollout && !d->roll_args)) return TINYMPC_ERR_UNSUPPORTED;
     KParams<T, NX, NU> P;
     fill_params<T, NX, NU>(P, *d);
     if (d->adapt) set_gpi_adapt_args<T>(P, d->adapt_args);  // GpiAdapt<T> + tables, uploaded by the caller (capi.cu: upload_adaptive)
     if (d->rollout) set_gpi_roll_args<T>(P, d->roll_args);  // GpiRoll<T>, uploaded by the caller (capi.cu: upload_rollout)
-    const T *gmat = (const T *)d->pd->blob;
-    // STRICT: adaptive rho, the rollout and per-instance bounds have variants of their own; fp32 with a shared model (the
-    // headline path) clamps with min / max when no bound of the problem is a signed zero
-#define TM_GPI_CASE(LL)                                                                                                  \
-    if (L == LL) {                                                                                                       \
-        if constexpr (!FAST) {                                                                                           \
-            if (d->rollout) {                                                                                            \
-                if (het) return launch_gpi_L<T, NX, NU, LL + GPI_ROLLOUT, false, true>(d, P, gmat);                      \
-                if constexpr (sizeof(T) == 4)                                                                            \
-                    if (d->pd->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL + GPI_ROLLOUT, false, false, true>(d, P, gmat); \
-                return launch_gpi_L<T, NX, NU, LL + GPI_ROLLOUT, false, false>(d, P, gmat);                              \
-            }                                                                                                            \
-            if (d->adapt == 2) /* per-instance tables */                                                                 \
-                return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT + GPI_ADAPT_TABLES, false, true>(d, P, gmat);              \
-            if (d->adapt) return launch_gpi_L<T, NX, NU, LL + GPI_ADAPT, false, true>(d, P, gmat);                       \
-            if (bounds) /* before MM: the host cannot scan per-instance bounds for signed zeros */                       \
-                return het ? launch_gpi_L<T, NX, NU, LL + GPI_BOUNDS, false, true>(d, P, gmat)                           \
-                           : launch_gpi_L<T, NX, NU, LL + GPI_BOUNDS, false, false>(d, P, gmat);                         \
-            if constexpr (sizeof(T) == 4)                                                                                \
-                if (!het && d->pd->bounds_zero_free) return launch_gpi_L<T, NX, NU, LL, false, false, true>(d, P, gmat); \
-        }                                                                                                                \
-        if (het) return launch_gpi_L<T, NX, NU, LL, FAST, true>(d, P, gmat);                                             \
-        return launch_gpi_L<T, NX, NU, LL, FAST, false>(d, P, gmat);                                                     \
-    }
-    TM_GPI_CASE(4)
-    TM_GPI_CASE(8)
-    if constexpr (sizeof(T) == 8) {  // fp64 may need L = 16 for the widest states (see gpi_plan)
-        TM_GPI_CASE(16)
-    }
-#undef TM_GPI_CASE
-    return TINYMPC_ERR_UNSUPPORTED;
+    const GpiVariant v = gpi_variant(*d);
+    int rc = TINYMPC_ERR_UNSUPPORTED;
+    walk_cases([&](auto i) {  // case i: L = 4, 8, 16; variant bits; het; mm
+        constexpr int I = decltype(i)::value, LL = 4 << (I / 64), BB = I / 4 % 16 * GPI_ADAPT;
+        constexpr bool HH = I / 2 % 2, MM = I % 2;
+        if constexpr (gpi_compiled(LL, BB, HH, MM, FAST, sizeof(T) == 8))
+            if (d->gpi.L == LL && v.bits == BB && v.het == HH && v.mm == MM)
+                rc = launch_gpi_L<T, NX, NU, LL + BB, FAST, HH, MM>(d, P, (const T *)d->pd->blob);
+    }, std::make_integer_sequence<int, 3 * 64>());
+    return rc;
 }
 
 template <typename T>

@@ -5,6 +5,8 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/tinympc_b200.h"
@@ -66,7 +68,7 @@ constexpr int GPS_VARIANTS = GPS_HET | GPS_BOUNDS | GPS_CONES | GPS_PLANES;  // 
 // Which streamed kernels are compiled, for a family mask, variant bits and mode.  FAST: the shared and the per-instance-model
 // solves only.  Per-instance cones with a cone family (1, 7), hyperplanes with a static hyperplane family (6, 7), never
 // with bounds or cones.
-constexpr bool gps_compiled(int fam, int var, bool fast) {
+__host__ __device__ constexpr bool gps_compiled(int fam, int var, bool fast) {
     if (fast && var != 0 && var != GPS_HET) return false;
     if ((var & GPS_CONES) && fam != 1 && fam != 7) return false;
     if ((var & GPS_PLANES) && (fam < 6 || (var & (GPS_BOUNDS | GPS_CONES)))) return false;
@@ -74,11 +76,41 @@ constexpr bool gps_compiled(int fam, int var, bool fast) {
 }
 // instances per lane group of a compiled variant: the shared solve's (ni) unless per-instance models or bounds hold a lane
 // group's registers
-constexpr int gps_variant_ni(int var, int ni) { return (var & (GPS_HET | GPS_BOUNDS)) ? 1 : ni; }
+__host__ __device__ constexpr int gps_variant_ni(int var, int ni) { return (var & (GPS_HET | GPS_BOUNDS)) ? 1 : ni; }
 // the variant bits of per-instance data (kinds: PerInstance::given or read)
 inline int gps_variant(bool models, const int (&kinds)[NKINDS]) {
     return (models ? GPS_HET : 0) | (kinds[KIND_BOUNDS] ? GPS_BOUNDS : 0) | (kinds[KIND_CONES] ? GPS_CONES : 0) |
            (kinds[KIND_PLANES] ? GPS_PLANES : 0);
+}
+
+// Variant bits of the on-chip kernel (gpi_kernel.cuh), added to its lane count L (its lane parameter LA; L = LA % GPI_ADAPT):
+// a separate template parameter or kernel argument would rename the existing kernels, a shared __device__ body or a larger
+// KParams changes their machine code.  GPI_ADAPT: adaptive rho (tinympc_b200_solve_adaptive), GpiAdapt arguments (adapt.h);
+// GPI_ADAPT_TABLES on top: its per-instance sensitivity tables, a variant of its own because a run-time choice between staged
+// and per-instance tables cost the shared-table kernel 2-3 % (DESIGN.md §5.5).  GPI_ROLLOUT: closed-loop rollouts
+// (tinympc_b200_rollout), GpiRoll arguments (rollout.h).  GPI_BOUNDS: per-instance box bounds (bounds_per_instance), P.x_min ...
+// u_max at the batch's columns or horizons (P.bounds_tv), each slot's column 0 loaded at its refill.
+constexpr int GPI_ADAPT = 64, GPI_ADAPT_TABLES = 128, GPI_ROLLOUT = 256, GPI_BOUNDS = 512;
+
+// Which on-chip kernels are compiled, for a lane count, variant bits, per-instance models (het), the min / max clamp (mm),
+// mode and dtype.  FAST: the plain solves only.  MM: fp32 with a shared model, plain or rollout.  Adaptive rho (with or
+// without its tables): per-instance models only.  Rollouts and bounds: never with each other or with adaptive rho.  L = 16:
+// fp64 only.
+__host__ __device__ constexpr bool gpi_compiled(int L, int bits, bool het, bool mm, bool fast, bool fp64) {
+    if (L != 4 && L != 8 && !(L == 16 && fp64)) return false;
+    if (bits & ~(GPI_ADAPT | GPI_ADAPT_TABLES | GPI_ROLLOUT | GPI_BOUNDS)) return false;
+    if (fast && (bits != 0 || mm)) return false;
+    if (mm && (fp64 || het || (bits != 0 && bits != GPI_ROLLOUT))) return false;
+    if ((bits & GPI_ADAPT) && !het) return false;
+    if ((bits & GPI_ADAPT_TABLES) && !(bits & GPI_ADAPT)) return false;
+    return !!(bits & GPI_ADAPT) + !!(bits & GPI_ROLLOUT) + !!(bits & GPI_BOUNDS) <= 1;
+}
+
+// the walks over kernel variants: f(std::integral_constant<int, i>()) for every case i, which f decodes and checks against
+// gps_compiled or gpi_compiled with if constexpr, so that only compiled variants are instantiated
+template <typename F, int... I>
+inline void walk_cases(F &&f, std::integer_sequence<int, I...>) {
+    (f(std::integral_constant<int, I>()), ...);
 }
 
 struct LaunchDesc {
@@ -116,6 +148,17 @@ struct LaunchDesc {
     int out_threads, out_ctas, out_smem, out_lanes_per_instance, out_instances_per_cta;
     size_t out_ws_need;  // GPS: workspace bytes this launch needs (set when the launcher returns TM_ERR_WORKSPACE)
 };
+
+// The on-chip kernel a launch wants (launch_gpi runs it when gpi_compiled admits it): variant bits, per-instance models and
+// the min / max clamp, which fp32 STRICT solves with a shared model use when no bound of the problem is a signed zero (the
+// host cannot scan per-instance bounds, so they rule it out)
+struct GpiVariant { int bits; bool het, mm; };
+inline GpiVariant gpi_variant(const LaunchDesc &d) {
+    const bool bounds = d.pi.read[KIND_BOUNDS] != 0;
+    const int bits = (d.adapt ? GPI_ADAPT : 0) | (d.adapt == 2 ? GPI_ADAPT_TABLES : 0) | (d.rollout ? GPI_ROLLOUT : 0) |
+                     (bounds ? GPI_BOUNDS : 0);
+    return {bits, d.pi.models, !d.fast && d.pd->dtype == TINYMPC_F32 && !d.pi.models && !bounds && d.pd->bounds_zero_free};
+}
 
 // launch epilogue of every kernel family: record the launch geometry in the descriptor, return the launch status
 inline int launch_done(LaunchDesc *d, int threads, int ctas, size_t smem, int lanes, int instances_per_cta) {
