@@ -429,6 +429,18 @@ typedef struct tinympc_rollout {
     int32_t *solved_traj; /* [B][T] */
     void *residuals_traj; /* [B][T][4] */
     int64_t reserved1[2]; /* must be 0 */
+    /*
+     * A plant of their own and measurement noise (a robustness study: every robot heavier, lighter or pushed by wind, seeing its
+     * state through a noisy sensor).  Instance b's plant P_b = (A_p, B_p, f_p) is the controller's model (the handle's, or
+     * io->models[b]) when plant is NULL, else the record `plant` (plant_per_instance = 0) or plant[b] (= 1).  Step t then runs
+     *     x^_t = x_t + noise[b][t]  (no add at all when noise is NULL);  solve from x^_t;  u0 = work->u.col(0);
+     *     x_{t+1} = (A_p x_t + B_p u0) + f_p  (tinympc_b200_advance_plant);  x_{t+1} = x_{t+1} + w[b][t]
+     * and x_traj records the true states x_t.  plant == NULL with noise == NULL is the rollout above.
+     */
+    const void *plant;          /* A | B | f column-major, nx*nx + nx*nu + nx elements (the start of a model blob), or [B][record] */
+    int32_t plant_per_instance; /* 0: one record for the batch; 1: one per instance (plant required) */
+    int32_t reserved2;          /* must be 0 */
+    const void *noise;          /* [B][T][nx] measurement noise, or NULL */
 } tinympc_rollout_t;
 
 int tinympc_b200_rollout(tinympc_b200_solver_t *s, const tinympc_batch_t *io, const tinympc_rollout_t *ro, void *cuda_stream);
@@ -449,6 +461,14 @@ int tinympc_b200_advance(tinympc_b200_solver_t *s, int64_t B, void *x0, const vo
  */
 int tinympc_b200_advance_models(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *models,
                                 void *cuda_stream);
+
+/*
+ * The same step against plants that are not the controller's model: instance b is advanced with the plant record `plant`
+ * (plant_per_instance = 0) or plant[b] (= 1), each A | B | f column-major, nx*nx + nx*nu + nx elements of the handle's dtype
+ * (the first pieces of a model blob), DEVICE pointer; same arithmetic.  The plant step of tinympc_rollout_t.plant.
+ */
+int tinympc_b200_advance_plant(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *plant,
+                               int32_t plant_per_instance, void *cuda_stream);
 
 /* 1 if a kernel is compiled for (dtype,nx,nu); used by callers to fail early */
 int tinympc_b200_supported(int32_t dtype, int32_t nx, int32_t nu);

@@ -54,6 +54,7 @@ def load():
     lib.tinympc_b200_get_stats.argtypes = [vp, C.POINTER(abi.Stats)]
     lib.tinympc_b200_advance.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp]
     lib.tinympc_b200_advance_models.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, vp]
+    lib.tinympc_b200_advance_plant.argtypes = [vp, C.c_int64, vp, vp, C.c_int64, vp, C.c_int32, vp]
     lib.tinympc_b200_supported.argtypes = [C.c_int32, C.c_int32, C.c_int32]
     for n in abi.EXPORTS:
         if n not in ("tinympc_b200_last_error", "tinympc_b200_version"):

@@ -103,7 +103,8 @@ class AdaptiveRho(C.Structure):
 
 
 class Rollout(C.Structure):
-    """tinympc_rollout_t: T closed-loop steps per instance, their reference trajectories, disturbance and per-step outputs."""
+    """tinympc_rollout_t: T closed-loop steps per instance, their reference trajectories, disturbance and per-step outputs, and the
+    plants they run against with their measurement noise."""
     _fields_ = [
         ("T", C.c_int32), ("reset_duals", C.c_int32), ("carry_v", C.c_int32), ("xref_per_instance", C.c_int32),
         ("Xref", vp), ("Uref", vp),
@@ -111,6 +112,8 @@ class Rollout(C.Structure):
         ("w", vp),
         ("x_traj", vp), ("u_traj", vp), ("iter_traj", vp), ("solved_traj", vp), ("residuals_traj", vp),
         ("reserved1", C.c_int64 * 2),
+        ("plant", vp), ("plant_per_instance", C.c_int32), ("reserved2", C.c_int32),
+        ("noise", vp),
     ]
 
 
@@ -136,6 +139,7 @@ EXPORTS = [
     "tinympc_b200_get_stats",
     "tinympc_b200_advance",
     "tinympc_b200_advance_models",
+    "tinympc_b200_advance_plant",
     "tinympc_b200_supported",
     "tinympc_b200_last_error",
     "tinympc_b200_version",

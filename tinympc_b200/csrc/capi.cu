@@ -117,6 +117,7 @@ struct tinympc_b200_solver {
     DevBuf ws;
     DevBuf queue;
     DevBuf vscratch;
+    DevBuf xtrue;  // rollout with measurement noise: the true plant states [B][nx] (GpiRoll::xtrue)
     DevBuf gps_ws;
     DevBuf shared_ref;  // host path: references shared by the whole batch
     DevBuf d_args;      // adaptive rho: GpiAdapt arguments + the shared dKinf_drho + dPinf_drho (adapt.h); rollout: GpiRoll (rollout.h)
@@ -434,9 +435,16 @@ int upload_adaptive(tinympc_b200_solver *s, const tinympc_adaptive_rho_t *ar, co
     });
 }
 
-// the rollout kernel's arguments (GpiRoll<T>)
+// elements of a plant record (A | B | f): the first three pieces of a model blob
+int64_t plant_elems(const tinympc_b200_solver *s) { return tmpc::model_blob<int64_t>(s->pd.nx, s->pd.nu).Qd; }
+
+// does a rollout need the GPI_PLANT variant (a plant of its own or measurement noise)?
+bool rollout_plant(const tinympc_rollout_t *ro) { return ro->plant || ro->noise; }
+
+// the rollout kernel's arguments (GpiRoll<T>).  Without a plant of their own, the instances' plant is the controller's model:
+// the handle's blob or the batch's model blobs, whose first pieces are a plant record.
 template <typename T>
-int upload_rollout(tinympc_b200_solver *s, const tinympc_rollout_t *ro, cudaStream_t stream) {
+int upload_rollout(tinympc_b200_solver *s, const tinympc_batch_t *io, const tinympc_rollout_t *ro, cudaStream_t stream) {
     return upload_args(s, sizeof(tmpc::GpiRoll<T>), stream, "rollout", [&](char *h) {
         tmpc::GpiRoll<T> r{};
         r.steps = ro->T;
@@ -447,6 +455,19 @@ int upload_rollout(tinympc_b200_solver *s, const tinympc_rollout_t *ro, cudaStre
         r.res_traj = (T *)ro->residuals_traj;
         r.iter_traj = ro->iter_traj;
         r.solved_traj = ro->solved_traj;
+        if (rollout_plant(ro)) {
+            if (ro->plant) {
+                r.plant = (const T *)ro->plant;
+                r.plant_stride = ro->plant_per_instance ? plant_elems(s) : 0;
+            } else if (io->models) {
+                r.plant = (const T *)io->models;
+                r.plant_stride = tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu);
+            } else {
+                r.plant = (const T *)s->pd.blob;
+            }
+            r.noise = (const T *)ro->noise;
+            r.xtrue = ro->noise ? (T *)s->xtrue.p : nullptr;
+        }
         std::memcpy(h, &r, sizeof(r));
     });
 }
@@ -482,8 +503,11 @@ int enqueue(tinympc_b200_solver *s, const tinympc_batch_t *io, cudaStream_t stre
         d.adapt_args = s->d_args.p;
     }
     if (ro) {
-        if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_rollout<double>(s, ro, stream) : upload_rollout<float>(s, ro, stream)) return rc;
-        d.rollout = 1;
+        if (ro->noise && s->xtrue.ensure((size_t)io->B * s->pd.nx * esize(s->pd.dtype) + 256))
+            return fail(TINYMPC_ERR_CUDA, "rollout true-state allocation failed");
+        if (int rc = s->pd.dtype == TINYMPC_F64 ? upload_rollout<double>(s, io, ro, stream) : upload_rollout<float>(s, io, ro, stream))
+            return rc;
+        d.rollout = rollout_plant(ro) ? 2 : 1;
         d.roll_args = s->d_args.p;
     }
     if (timed) CUDA_TRY(cudaEventRecord(s->ev0, stream));
@@ -899,6 +923,9 @@ int tinympc_b200_rollout(tinympc_b200_solver_t *s, const tinympc_batch_t *io, co
     if (ro->reserved != 0 || ro->reserved1[0] != 0 || ro->reserved1[1] != 0) return fail(TINYMPC_ERR_ARG, "rollout: reserved fields must be 0");
     if (!ro->carry_v && (io->state.v || io->state.z))
         return fail(TINYMPC_ERR_ARG, "rollout: io->state.v / state.z need carry_v = 1 (without it work->v / work->z read as zeros)");
+    if ((ro->plant_per_instance != 0 && ro->plant_per_instance != 1) || ro->reserved2 != 0)
+        return fail(TINYMPC_ERR_ARG, "rollout: plant_per_instance must be 0 or 1 and reserved2 must be 0");
+    if (ro->plant_per_instance && !ro->plant) return fail(TINYMPC_ERR_ARG, "rollout: plant_per_instance = 1 needs a plant");
     CUDA_TRY(cudaSetDevice(s->device));
     tinympc_batch_t b = *io;  // the first step's window is the trajectory's start: the kernel reads the trajectories in its place
     b.Xref = ro->Xref;
@@ -938,6 +965,13 @@ int tinympc_b200_advance_models(tinympc_b200_solver_t *s, int64_t B, void *x0, c
                                 void *cuda_stream) {
     if (!s || !x0 || !u || !models) return fail(TINYMPC_ERR_ARG, "null argument");
     return advance_impl(s, B, x0, u, u_stride, models, tinympc_b200_model_blob_elems(s->pd.nx, s->pd.nu), cuda_stream);
+}
+
+int tinympc_b200_advance_plant(tinympc_b200_solver_t *s, int64_t B, void *x0, const void *u, int64_t u_stride, const void *plant,
+                               int32_t plant_per_instance, void *cuda_stream) {
+    if (!s || !x0 || !u || !plant) return fail(TINYMPC_ERR_ARG, "null argument");
+    if (plant_per_instance != 0 && plant_per_instance != 1) return fail(TINYMPC_ERR_ARG, "advance_plant: plant_per_instance must be 0 or 1");
+    return advance_impl(s, B, x0, u, u_stride, plant, plant_per_instance ? plant_elems(s) : 0, cuda_stream);
 }
 
 int tinympc_b200_get_stats(const tinympc_b200_solver_t *s, tinympc_b200_stats_t *out) {

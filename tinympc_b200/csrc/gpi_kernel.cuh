@@ -65,7 +65,7 @@ __host__ __device__ constexpr bool gpi_feasible() {
 
 constexpr int GPI_MAX_WARPS = 8;
 
-// LA: the lane count plus the variant bits (launch.h: GPI_ADAPT ... GPI_BOUNDS).
+// LA: the lane count plus the variant bits (launch.h: GPI_ADAPT ... GPI_PLANT).
 // MM (STRICT only): the box clamp as min / max instructions.  Identical to Eigen's compare-select form for every input
 // (NaN included: both return the bound) except when a bound is a signed zero - the host sets MM only when no bound is +-0.
 template <typename T, int NX, int NU, int LA, bool FAST, bool HET, bool MM = false>
@@ -74,6 +74,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     constexpr bool ADAPT = (LA & GPI_ADAPT) != 0;       // adaptive rho
     constexpr bool PERTAB = (LA & GPI_ADAPT_TABLES) != 0;  // ... with per-instance tables
     constexpr bool ROLL = (LA & GPI_ROLLOUT) != 0;        // closed-loop rollout
+    constexpr bool PLT = (LA & GPI_PLANT) != 0;           // ... against plants of their own, with measurement noise
     constexpr bool BND = (LA & GPI_BOUNDS) != 0;          // per-instance box bounds
     constexpr int L = LA % GPI_ADAPT;
     static_assert(gpi_compiled(L, LA - L, HET, MM, FAST, sizeof(T) == 8), "a variant gpi_compiled does not admit");
@@ -1115,9 +1116,44 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             if (s_it == 0) u0v[b] = T(0);  // no iteration ran: work->u of a loop state without work->u
         }
         gather_u(u0v, Uf0);
-        dots<FAST>(mB, Uf0, bu0);
+        if constexpr (!PLT) dots<FAST>(mB, Uf0, bu0);
         T *xt = RP->x_traj;
         const T *w = RP->w;
+        if constexpr (PLT) {
+            // the plant steps from the true state (the slot's x0 unless noise is given) with its own rows, read from the plant
+            // record: x <- (A_p x + B_p u0) + f_p (+ w), then the next step solves from x + n[b][t+1]
+            const T *nz = RP->noise;
+            T xs[RX], Xs[NX];
+#pragma unroll
+            for (int a = 0; a < RX; ++a) xs[a] = (nz && slot == s && xv[a]) ? RP->xtrue[ib * NX + l * RX + a] : x0o[a];
+            gather_x(xs, Xs);
+            if (slot == s) {
+                const T *pA = RP->plant + ib * RP->plant_stride, *pB = pA + NX * NX, *pf = pB + NX * NU;
+                const int64_t ox = (ib * (steps + 1) + s_t) * NX;
+#pragma unroll
+                for (int a = 0; a < RX; ++a) {
+                    const int ii = xv[a] ? l * RX + a : 0;
+                    T ax = __ldg(pA + ii) * Xs[0];
+#pragma unroll
+                    for (int m = 1; m < NX; ++m) ax = ax + __ldg(pA + ii + NX * m) * Xs[m];
+                    T bu = __ldg(pB + ii) * Uf0[0];
+#pragma unroll
+                    for (int j = 1; j < NU; ++j) bu = bu + __ldg(pB + ii + NX * j) * Uf0[j];
+                    T xn = (ax + bu) + __ldg(pf + ii);
+                    if (w && xv[a]) xn = xn + w[bt * NX + l * RX + a];
+                    if (xt && xv[a]) xt[ox + l * RX + a] = xs[a];
+                    if (xt && xv[a] && last) xt[ox + NX + l * RX + a] = xn;
+                    if (nz && xv[a]) {
+                        RP->xtrue[ib * NX + l * RX + a] = xn;
+                        if (!last) xn = xn + nz[(bt + 1) * NX + l * RX + a];
+                    }
+                    x0o[a] = xv[a] ? xn : T(0);
+                }
+#pragma unroll
+                for (int b = 0; b < RU; ++b)
+                    if (RP->u_traj && uv[b]) RP->u_traj[bt * NU + l * RU + b] = u0v[b];
+            }
+        } else {
         if (slot == s) {
             const int64_t ox = (ib * (steps + 1) + s_t) * NX;
 #pragma unroll
@@ -1131,6 +1167,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
 #pragma unroll
             for (int b = 0; b < RU; ++b)
                 if (RP->u_traj && uv[b]) RP->u_traj[bt * NU + l * RU + b] = u0v[b];
+        }
         }
         __syncwarp();
         if (last) return false;
@@ -1208,6 +1245,18 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 if constexpr (ROLL) {
                     if (slot == s) tstep = 0;
                     roll_window(s);
+                }
+                if constexpr (PLT) {  // noise: the first step solves from x0 + n[b][0]; x0 waits in the true-state scratch
+                    const T *nz = RP->noise;
+                    if (nz && slot == s) {
+                        const int64_t ib = (int64_t)nxt;
+#pragma unroll
+                        for (int a = 0; a < RX; ++a)
+                            if (xv[a]) {
+                                RP->xtrue[ib * NX + l * RX + a] = x0o[a];
+                                x0o[a] = x0o[a] + nz[ib * RP->steps * NX + l * RX + a];
+                            }
+                    }
                 }
             } else if (slot == s) {
                 busy = false;

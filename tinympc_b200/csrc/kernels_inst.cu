@@ -1,8 +1,10 @@
-// kernels_inst.cu — compiled three times per supported (nx, nu) with -DTM_NX=.. -DTM_NU=.. -DTM_PART=0|1|2 (see Makefile):
+// kernels_inst.cu — compiled four times per supported (nx, nu) with -DTM_NX=.. -DTM_NU=.. -DTM_PART=0|1|2|3 (see Makefile):
 //   part 0: thread-per-instance kernels (tpi_kernel.cuh), device precompute, and the type-erased DimEntry
-//   part 1: on-chip lane-group kernels (gpi_kernel.cuh)
+//   part 1: on-chip lane-group kernels (gpi_kernel.cuh), all but the GPI_PLANT variants
 //   part 2: streamed lane-group kernels (gps_kernel.cuh)
-// Three objects per dimension pair keep `make -j` busy and an edit of one kernel family from recompiling the others.
+//   part 3: the on-chip GPI_PLANT variants (rollouts against plants of their own), reached through part 1's launcher
+// Four objects per dimension pair keep `make -j` busy and an edit of one kernel family from recompiling the others; the
+// plant variants have an object of their own so that the on-chip objects, the longest compiles, take no longer than without them.
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
@@ -12,7 +14,7 @@
 #include "launch.h"
 
 #if !defined(TM_NX) || !defined(TM_NU) || !defined(TM_PART)
-#error "compile with -DTM_NX=<nx> -DTM_NU=<nu> -DTM_PART=<0|1|2>"
+#error "compile with -DTM_NX=<nx> -DTM_NU=<nu> -DTM_PART=<0|1|2|3>"
 #endif
 
 #define TM_CAT3(a, b, c) a##b##_##c
@@ -21,6 +23,7 @@
 
 // cross-part entry points of this dimension pair
 extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d);
+extern "C" int TM_SYM(tm_gpi_plant_launch_)(tmpc::LaunchDesc *d);
 extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_optin);
 extern "C" int TM_SYM(tm_gps_launch_)(tmpc::LaunchDesc *d);
 extern "C" int TM_SYM(tm_gps_lanes_)(int dtype);
@@ -93,7 +96,7 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
     return &e;
 }
 
-#elif TM_PART == 1
+#elif TM_PART == 1 || TM_PART == 3
 // =========================================================================================================
 #include "gpi_kernel.cuh"
 
@@ -101,7 +104,8 @@ namespace tmpc {
 namespace {
 
 // the on-chip kernel of the solve's variant (launch.h: gpi_variant, gpi_compiled) with the plan d->gpi, which comes from the
-// caller (capi.cu: plan_solve, through the DimEntry's gpi_plan); a variant that is not compiled is TINYMPC_ERR_UNSUPPORTED
+// caller (capi.cu: plan_solve, through the DimEntry's gpi_plan); a variant that is not compiled is TINYMPC_ERR_UNSUPPORTED.
+// Part 1 instantiates the variants without GPI_PLANT, part 3 those with it.
 template <typename T, int NX, int NU, bool FAST>
 int launch_gpi(LaunchDesc *d) {
     if (d->gpi.L == 0 || !d->work_queue || (d->adapt && !d->adapt_args) || (d->rollout && !d->roll_args)) return TINYMPC_ERR_UNSUPPORTED;
@@ -112,12 +116,12 @@ int launch_gpi(LaunchDesc *d) {
     const GpiVariant v = gpi_variant(*d);
     int rc = TINYMPC_ERR_UNSUPPORTED;
     walk_cases([&](auto i) {  // case i: L = 4, 8, 16; variant bits; het; mm
-        constexpr int I = decltype(i)::value, LL = 4 << (I / 64), BB = I / 4 % 16 * GPI_ADAPT;
+        constexpr int I = decltype(i)::value, LL = 4 << (I / 128), BB = I / 4 % 32 * GPI_ADAPT;
         constexpr bool HH = I / 2 % 2, MM = I % 2;
-        if constexpr (gpi_compiled(LL, BB, HH, MM, FAST, sizeof(T) == 8))
+        if constexpr (gpi_compiled(LL, BB, HH, MM, FAST, sizeof(T) == 8) && ((BB & GPI_PLANT) != 0) == (TM_PART == 3))
             if (d->gpi.L == LL && v.bits == BB && v.het == HH && v.mm == MM)
                 rc = launch_gpi_L<T, NX, NU, LL + BB, FAST, HH, MM>(d, P, (const T *)d->pd->blob);
-    }, std::make_integer_sequence<int, 3 * 64>());
+    }, std::make_integer_sequence<int, 3 * 128>());
     return rc;
 }
 
@@ -130,7 +134,9 @@ int launch_T(LaunchDesc *d) {
 }  // namespace
 }  // namespace tmpc
 
+#if TM_PART == 1
 extern "C" int TM_SYM(tm_gpi_launch_)(tmpc::LaunchDesc *d) {
+    if (tmpc::gpi_variant(*d).bits & tmpc::GPI_PLANT) return TM_SYM(tm_gpi_plant_launch_)(d);
     if (d->pd->dtype == TINYMPC_F32) return tmpc::launch_T<float>(d);
     if (d->pd->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
     return TINYMPC_ERR_ARG;
@@ -140,6 +146,13 @@ extern "C" tmpc::GpiPlan TM_SYM(tm_gpi_plan_)(int dtype, int N, int max_smem_opt
     auto plan = [&](auto t) { return tmpc::gpi_plan<decltype(t), TM_NX, TM_NU>(N, max_smem_optin - 64); };
     return dtype == TINYMPC_F32 ? plan(0.f) : (dtype == TINYMPC_F64 ? plan(0.0) : tmpc::GpiPlan{});
 }
+#else
+extern "C" int TM_SYM(tm_gpi_plant_launch_)(tmpc::LaunchDesc *d) {
+    if (d->pd->dtype == TINYMPC_F32) return tmpc::launch_T<float>(d);
+    if (d->pd->dtype == TINYMPC_F64) return tmpc::launch_T<double>(d);
+    return TINYMPC_ERR_ARG;
+}
+#endif
 
 #else
 // =========================================================================================================

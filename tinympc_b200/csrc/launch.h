@@ -89,18 +89,20 @@ inline int gps_variant(bool models, const int (&kinds)[NKINDS]) {
 // GPI_ADAPT_TABLES on top: its per-instance sensitivity tables, a variant of its own because a run-time choice between staged
 // and per-instance tables cost the shared-table kernel 2-3 % (DESIGN.md §5.5).  GPI_ROLLOUT: closed-loop rollouts
 // (tinympc_b200_rollout), GpiRoll arguments (rollout.h).  GPI_BOUNDS: per-instance box bounds (bounds_per_instance), P.x_min ...
-// u_max at the batch's columns or horizons (P.bounds_tv), each slot's column 0 loaded at its refill.
-constexpr int GPI_ADAPT = 64, GPI_ADAPT_TABLES = 128, GPI_ROLLOUT = 256, GPI_BOUNDS = 512;
+// u_max at the batch's columns or horizons (P.bounds_tv), each slot's column 0 loaded at its refill.  GPI_PLANT on top of
+// GPI_ROLLOUT: a rollout against a plant of each instance's own and / or with measurement noise (GpiRoll's plant fields).
+constexpr int GPI_ADAPT = 64, GPI_ADAPT_TABLES = 128, GPI_ROLLOUT = 256, GPI_BOUNDS = 512, GPI_PLANT = 1024;
 
 // Which on-chip kernels are compiled, for a lane count, variant bits, per-instance models (het), the min / max clamp (mm),
-// mode and dtype.  FAST: the plain solves only.  MM: fp32 with a shared model, plain or rollout.  Adaptive rho (with or
-// without its tables): per-instance models only.  Rollouts and bounds: never with each other or with adaptive rho.  L = 16:
-// fp64 only.
+// mode and dtype.  FAST: the plain solves only.  MM: fp32 with a shared model, plain or rollout (with or without a plant).
+// Adaptive rho (with or without its tables): per-instance models only.  Rollouts and bounds: never with each other or with
+// adaptive rho.  A plant: rollouts only.  L = 16: fp64 only.
 __host__ __device__ constexpr bool gpi_compiled(int L, int bits, bool het, bool mm, bool fast, bool fp64) {
     if (L != 4 && L != 8 && !(L == 16 && fp64)) return false;
-    if (bits & ~(GPI_ADAPT | GPI_ADAPT_TABLES | GPI_ROLLOUT | GPI_BOUNDS)) return false;
+    if (bits & ~(GPI_ADAPT | GPI_ADAPT_TABLES | GPI_ROLLOUT | GPI_BOUNDS | GPI_PLANT)) return false;
     if (fast && (bits != 0 || mm)) return false;
-    if (mm && (fp64 || het || (bits != 0 && bits != GPI_ROLLOUT))) return false;
+    if (mm && (fp64 || het || (bits != 0 && (bits & ~GPI_PLANT) != GPI_ROLLOUT))) return false;
+    if ((bits & GPI_PLANT) && !(bits & GPI_ROLLOUT)) return false;
     if ((bits & GPI_ADAPT) && !het) return false;
     if ((bits & GPI_ADAPT_TABLES) && !(bits & GPI_ADAPT)) return false;
     return !!(bits & GPI_ADAPT) + !!(bits & GPI_ROLLOUT) + !!(bits & GPI_BOUNDS) <= 1;
@@ -134,7 +136,7 @@ struct LaunchDesc {
     int adapt;  // 0: no; 1: one shared table pair; 2: per-instance tables
     const void *adapt_args;
     // closed-loop rollout (tinympc_b200_rollout): io.Xref / io.Uref are then the reference trajectories, roll_args = device copy
-    // of GpiRoll<T> (rollout.h)
+    // of GpiRoll<T> (rollout.h); 1: against the controller's model, 2: against plants of their own or with measurement noise
     int rollout;
     const void *roll_args;
     // per-instance data: the lane-group kernels' GPI_BOUNDS and GPS_HET / BOUNDS / CONES / PLANES variants read io's arrays
@@ -156,7 +158,7 @@ struct GpiVariant { int bits; bool het, mm; };
 inline GpiVariant gpi_variant(const LaunchDesc &d) {
     const bool bounds = d.pi.read[KIND_BOUNDS] != 0;
     const int bits = (d.adapt ? GPI_ADAPT : 0) | (d.adapt == 2 ? GPI_ADAPT_TABLES : 0) | (d.rollout ? GPI_ROLLOUT : 0) |
-                     (bounds ? GPI_BOUNDS : 0);
+                     (d.rollout == 2 ? GPI_PLANT : 0) | (bounds ? GPI_BOUNDS : 0);
     return {bits, d.pi.models, !d.fast && d.pd->dtype == TINYMPC_F32 && !d.pi.models && !bounds && d.pd->bounds_zero_free};
 }
 

@@ -91,6 +91,18 @@ def rocket_fleet(B, N=100, seed=0, mass_spread=0.2) -> dict:
                 Rdiag=tile(spec.Rdiag), rho=np.full(B, spec.rho), m=m, spec=spec)
 
 
+def plant_fleet(spec: ModelSpec, B, seed=0, mass_spread=0.2, drift=0.0) -> dict:
+    """The real robots behind one controller: robot b's plant is the spec's model with its input matrix scaled by 1/m_b,
+    m_b = 1 + mass_spread * U(-1, 1) (the convention of rocket_fleet), and its f plus a constant drift drift * N(0, 1) per state
+    (a steady wind).  -> dict(A [B,nx,nx], B [B,nx,nu], f [B,nx], m [B]) in float64, the `plant=` argument of DeviceMPCLoop."""
+    rng = np.random.default_rng(seed)
+    m = 1.0 + mass_spread * rng.uniform(-1.0, 1.0, size=B)
+    A = np.tile(np.asarray(spec.A, dtype=np.float64)[None], (B, 1, 1))
+    Bm = np.asarray(spec.B, dtype=np.float64)[None] / m[:, None, None]
+    f = np.asarray(spec.f, dtype=np.float64).reshape(1, -1) + drift * rng.standard_normal((B, spec.nx))
+    return dict(A=A, B=Bm, f=f, m=m)
+
+
 def cone_fleet(spec: ModelSpec, B, seed=0, scale=(0.6, 1.0), dtype=np.float64) -> dict:
     """Per-robot cone coefficients for a fleet of B robots of `spec` (e.g. rocket(), or rocket_fleet's spec): robot b's mu
     of every state and input cone is the spec's cx / cu times its own factor drawn from U(scale), e.g. a tighter glide
