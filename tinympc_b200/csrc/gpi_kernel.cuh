@@ -296,6 +296,14 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         }
     };
 
+    // one row of dots(): the same ascending-k operations
+    auto rowdot = [](const T (&m)[NX], const T (&v)[NX]) {
+        T acc = m[0] * v[0];
+#pragma unroll
+        for (int c = 1; c < NX; ++c) acc = mac<FAST>(acc, m[c], v[c]);
+        return acc;
+    };
+
     const bool cold = P.cold != 0;
     const bool tvb = P.bounds_tv != 0;
     const bool enx = P.en_state_bound != 0, enu = P.en_input_bound != 0;
@@ -375,24 +383,27 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
     };
 
     // forward pass fused with slack / dual update / residuals.  SLOW = some slot is in the first iteration of a
-    // warm start (work->v / work->z come from the caller) or work->v / work->z are being persisted.
-    auto forward = [&](auto tag, const bool vin, T &rpx, T &rdx, T &rpu, T &rdu) {
-        constexpr bool SLOW = decltype(tag)::value;
+    // warm start (work->v / work->z come from the caller) or work->v / work->z are being persisted.  TV = the bounds may vary
+    // along the horizon (P.bounds_tv): column k reloads them if they do.  A compile-time flag, so that the sweep of static
+    // bounds carries no reload branch, which would split its loop body in two blocks that the scheduler cannot interleave.
+    auto forward = [&](auto tag, auto tv, const bool vin, T &rpx, T &rdx, T &rpu, T &rdu) {
+        constexpr bool SLOW = decltype(tag)::value, TV = decltype(tv)::value;
         if constexpr (PS) load_fwd_rows(rowsrc);
         T xo[RX], Xf[NX];
 #pragma unroll
         for (int a = 0; a < RX; ++a) xo[a] = x0o[a];
         gather_x(xo, Xf);
-        // one column: slack + dual update of this lane's rows, residual maxima; HASU = the column has inputs
-        auto column = [&](int k, const bool HASU, const T (&u)[RU], const T (&vprev)[PVP], const T (&pb)[PVP]) {  // always inlined with a literal HASU
-            T pa[PVP], na[PVP], nb[PVP];
+        // one column: slack + dual update of this lane's rows (the new packs na / nb, from the primal pack pa it loads),
+        // residual maxima; HASU = the column has inputs.  put() stores the column.
+        auto column = [&](int k, const bool HASU, const T (&u)[RU], const T (&vprev)[PVP], const T (&pb)[PVP], T (&pa)[PVP],
+                          T (&na)[PVP], T (&nb)[PVP]) {  // always inlined with a literal HASU
             load_pack(aPA, k, pa);
 #pragma unroll
             for (int e = 0; e < PVP; ++e) {
                 na[e] = pa[e];
                 nb[e] = pb[e];
             }
-            if constexpr (!BND) {  // per-instance horizons are loaded at the top of the step (bounds_at below)
+            if constexpr (!BND && TV) {  // per-instance horizons are loaded at the top of the step (bounds_at below)
                 if (tvb) box_bounds<false>(P, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
             }
             if constexpr (FAST) {
@@ -474,6 +485,8 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                     }
                 }
             }
+        };
+        auto put = [&](int k, const T (&pa)[PVP], const T (&na)[PVP], const T (&nb)[PVP]) {
             if (busy) {
                 store_pack(aPA, k, na);
                 store_pb(k, nb);
@@ -515,7 +528,7 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         // BND, layout 2: column k of the slot's instance (laid out like Xref / Uref; a slot without an instance reads instance
         // 0), issued at the top of step k so that its latency hides behind the step's mat-vec and gathers
         auto bounds_at = [&](int k, const bool HASU) {
-            if constexpr (BND) {
+            if constexpr (BND && TV) {
                 const int64_t bi = inst < 0 ? 0 : inst;
                 if (tvb) box_bounds_at<false>(P, bi * N * NX, bi * (N - 1) * NU, l, k, HASU, enx, enu, xok, uok, loX, hiX, loU, hiU);
             }
@@ -526,11 +539,16 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
             load_vprev(k, vprev);
             load_pb(k, pbk);
             load_d(k, dk);
-            dots<FAST>(mS1f, Xf, t1);  // [A x_k ; Kinf x_k]
+            // [A x_k ; Kinf x_k], the recurrence first: u_k needs only the Kinf rows, and the A rows fill its exchange
+#pragma unroll
+            for (int b = 0; b < RU; ++b) t1[RX + b] = rowdot(mS1f[RX + b], Xf);
 #pragma unroll
             for (int b = 0; b < RU; ++b) u[b] = (-t1[RX + b]) - dk[b];  // u_k = -(Kinf x_k) - d_k
             gather_u(u, Uf);
-            column(k, true, u, vprev, pbk);
+#pragma unroll
+            for (int a = 0; a < RX; ++a) t1[a] = rowdot(mS1f[a], Xf);
+            T pa[PVP], na[PVP], nb[PVP];
+            column(k, true, u, vprev, pbk, pa, na, nb);
             dots<FAST>(mB, Uf, bu);
             {   // x_{k+1} = (A x_k + B u_k) + f
                 T ax[RX], tx[RX];
@@ -540,15 +558,19 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
                 vadd<T, RX>(tx, vf, xo);
             }
             gather_x(xo, Xf);
+            // the column's stores follow the exchange of x_{k+1}: stores ahead of it would pin the column's arithmetic in
+            // front of it, and with one warp per scheduler nothing else would fill the exchange's latency
+            put(k, pa, na, nb);
         }
         {
-            T udummy[RU], vprev[PVP], pbk[PVP];
+            T udummy[RU], vprev[PVP], pbk[PVP], pa[PVP], na[PVP], nb[PVP];
 #pragma unroll
             for (int b = 0; b < RU; ++b) udummy[b] = T(0);
             bounds_at(N - 1, false);
             load_vprev(N - 1, vprev);
             load_pb(N - 1, pbk);
-            column(N - 1, false, udummy, vprev, pbk);
+            column(N - 1, false, udummy, vprev, pbk, pa, na, nb);
+            put(N - 1, pa, na, nb);
         }
     };
 
@@ -1334,8 +1356,13 @@ __global__ void __launch_bounds__(GPI_MAX_WARPS * 32, 1)
         T rpx = T(0), rdx = T(0), rpu = T(0), rdu = T(0);
         bool vin = busy && (!cold) && it == 0;  // work->v / work->z come from the caller on the first iteration
         if constexpr (ROLL) vin = busy && (!cold || tstep > 0) && it == 0;  // ... or from the previous step after the first
-        if (keep_v || __any_sync(0xffffffffu, vin)) forward(BoolTag<true>{}, vin, rpx, rdx, rpu, rdu);
-        else forward(BoolTag<false>{}, false, rpx, rdx, rpu, rdu);
+        // fp64 keeps one sweep that tests P.bounds_tv per column: the second copy made its L = 16 rollout kernel 5 % slower
+        auto sweep = [&](auto slow, const bool vin_) {
+            if (PS || tvb) forward(slow, BoolTag<true>{}, vin_, rpx, rdx, rpu, rdu);
+            else forward(slow, BoolTag<false>{}, vin_, rpx, rdx, rpu, rdu);
+        };
+        if (keep_v || __any_sync(0xffffffffu, vin)) sweep(BoolTag<true>{}, vin);
+        else sweep(BoolTag<false>{}, false);
         __syncwarp();
         // ---- termination_condition (admm.cpp:310-328), per instance ----
         rpx = group_max<T, L>(rpx);
