@@ -284,7 +284,7 @@ int tinympc_b200_precompute_cache_batch(int32_t dtype, int32_t nx, int32_t nu, i
                                         void *models_out, int32_t nthreads);
 
 /*
- * The same computation ON THE DEVICE of handle `h` (one warp per instance, precompute_kernel.cuh), for batches whose
+ * The same computation ON THE DEVICE of handle `h` (one warp per instance, riccati.cuh: riccati_kernel), for batches whose
  * models change often (per-instance re-linearisation): all pointers are device pointers of the handle's dtype, layouts
  * as above; nx, nu are the handle's.  Asynchronous on `stream`.  The blobs are bit-identical to the host routine's.
  * sweeps_out (optional, [B]): Riccati sweeps used per instance, -1 where a matrix was singular (that blob's cache is
@@ -316,7 +316,7 @@ int tinympc_b200_precompute_sensitivity_batch(int32_t dtype, int32_t nx, int32_t
                                               void *dP_out, int32_t nthreads);
 
 /*
- * The same tables ON THE DEVICE of handle `h` (one warp per instance, precompute_kernel.cuh): device pointers of the
+ * The same tables ON THE DEVICE of handle `h` (one warp per instance, riccati.cuh: riccati_kernel): device pointers of the
  * handle's dtype, nx, nu are the handle's, asynchronous on `stream`.  Bit-identical to the host routine's.  sweeps_out
  * (optional, [B]): sweeps used per instance, -1 where a matrix was singular (the same instances as in
  * tinympc_b200_precompute_cache_batch_device; their tables are not written).  dK_out / dP_out can be passed straight to

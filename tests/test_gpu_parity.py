@@ -439,7 +439,11 @@ def test_heterogeneous_models_per_instance(dt):
     assert e.value.code == abi.ERR_UNSUPPORTED
 
 
-@pytest.mark.parametrize("dims", [(4, 1), (12, 4), (16, 8)])
+# every compiled (nx, nu) (csrc/launch.h: TM_DIMS)
+ALL_DIMS = [(4, 1), (6, 3), (12, 4), (4, 2), (4, 4), (4, 8), (8, 2), (8, 4), (8, 8), (12, 2), (12, 8), (16, 2), (16, 4), (16, 8)]
+
+
+@pytest.mark.parametrize("dims", ALL_DIMS)
 @pytest.mark.parametrize("dt", [np.float32, np.float64])
 def test_device_precompute_bit_identical_to_host_precompute(dt, dims):
     """SURVEY §8f-2: the batched cache precompute on the device (one warp per model) produces exactly the blobs of the
@@ -467,7 +471,6 @@ def test_device_precompute_bit_identical_to_host_precompute(dt, dims):
 # launch plans of the on-chip kernel: every compiled (nx, nu) at the horizons of the BASELINE sweep (N = 50, 100), so that
 # each distinct (lanes per instance, instances per SM) plan of the planner (227 KB of shared memory per CTA) meets the oracle
 # ---------------------------------------------------------------------------------------------------------------------
-ALL_DIMS = [(4, 1), (6, 3), (12, 4), (4, 2), (4, 4), (4, 8), (8, 2), (8, 4), (8, 8), (12, 2), (12, 8), (16, 2), (16, 4), (16, 8)]
 # fp32 plans: (lanes per instance, instances per SM)
 _P50 = {(4, 2): (4, 32), (4, 4): (4, 32), (8, 2): (4, 32), (8, 4): (4, 32), (12, 2): (4, 32), (12, 4): (4, 32), (4, 8): (8, 16),
         (8, 8): (8, 16), (12, 8): (8, 16), (16, 2): (8, 16), (16, 4): (8, 16), (16, 8): (8, 16)}

@@ -31,7 +31,7 @@ extern "C" int TM_SYM(tm_gps_het_slots_)(int dtype, bool soc, bool lin, bool con
 
 #if TM_PART == 0
 // =========================================================================================================
-#include "precompute_kernel.cuh"
+#include "riccati.cuh"
 #include "tpi_kernel.cuh"
 
 namespace tmpc {
@@ -63,21 +63,15 @@ int launch(LaunchDesc *d) {
     return TINYMPC_ERR_ARG;
 }
 
-int precompute_batch(int dtype, int64_t B, const void *A, const void *Bm, const void *f, const void *Qdiag, const void *Rdiag,
-                     const void *rho, void *models_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream) {
-    if (dtype == TINYMPC_F32)
-        return launch_precompute_T<float, TM_NX, TM_NU>(B, A, Bm, f, Qdiag, Rdiag, rho, models_out, sweeps_out, sm_count, stream);
-    if (dtype == TINYMPC_F64)
-        return launch_precompute_T<double, TM_NX, TM_NU>(B, A, Bm, f, Qdiag, Rdiag, rho, models_out, sweeps_out, sm_count, stream);
-    return TINYMPC_ERR_ARG;
-}
-
-int sensitivity_batch(int dtype, int64_t B, const void *A, const void *Bm, const void *Qdiag, const void *Rdiag, const void *rho,
-                      void *dK_out, void *dP_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream) {
-    if (dtype == TINYMPC_F32)
-        return launch_sensitivity_T<float, TM_NX, TM_NU>(B, A, Bm, Qdiag, Rdiag, rho, dK_out, dP_out, sweeps_out, sm_count, stream);
-    if (dtype == TINYMPC_F64)
-        return launch_sensitivity_T<double, TM_NX, TM_NU>(B, A, Bm, Qdiag, Rdiag, rho, dK_out, dP_out, sweeps_out, sm_count, stream);
+int riccati_batch(int dtype, bool tangent, int64_t B, const RiccatiBatch<void> &a, int32_t *sweeps_out, int sm_count,
+                  cudaStream_t stream) {
+    auto go = [&](auto t) {
+        using T = decltype(t);
+        return tangent ? launch_riccati<T, TM_NX, TM_NU, true>(B, a.as<T>(), sweeps_out, sm_count, stream)
+                       : launch_riccati<T, TM_NX, TM_NU, false>(B, a.as<T>(), sweeps_out, sm_count, stream);
+    };
+    if (dtype == TINYMPC_F32) return go(0.f);
+    if (dtype == TINYMPC_F64) return go(0.0);
     return TINYMPC_ERR_ARG;
 }
 
@@ -89,8 +83,7 @@ extern "C" const tmpc::DimEntry *TM_SYM(tm_dim_entry_)() {
                                      TM_NU,
                                      &tmpc::launch,
                                      &TM_SYM(tm_gpi_plan_),
-                                     &tmpc::precompute_batch,
-                                     &tmpc::sensitivity_batch,
+                                     &tmpc::riccati_batch,
                                      &TM_SYM(tm_gps_lanes_),
                                      &TM_SYM(tm_gps_het_slots_)};
     return &e;

@@ -179,6 +179,19 @@ inline bool set_dynamic_smem(K kern, size_t smem) {
 // internal: the launcher needs a larger gps_ws (size in out_ws_need); never leaves the library
 constexpr int TM_ERR_WORKSPACE = -100;
 
+// A batch of the Riccati precompute (riccati.cuh), host or device pointers, instance after instance and column-major:
+// A [B][nx*nx], B [B][nx*nu], f [B][nx], the user's diagonals Qd [B][nx] and Rd [B][nu], rho [B].  Without the tangent the
+// results are one model blob per instance (models, model_blob.h), with it the tables dK [B][nu*nx] and dP [B][nx*nx].
+template <typename T>
+struct RiccatiBatch {
+    const T *A, *B, *f, *Qd, *Rd, *rho;
+    T *models, *dK, *dP;
+    template <typename U>
+    RiccatiBatch<U> as() const {
+        return {(const U *)A, (const U *)B, (const U *)f, (const U *)Qd, (const U *)Rd, (const U *)rho, (U *)models, (U *)dK, (U *)dP};
+    }
+};
+
 // per-(nx,nu) entry: returns 0 on success, TINYMPC_ERR_UNSUPPORTED when (dtype,family,...) is not compiled
 typedef int (*launch_fn)(LaunchDesc *);
 
@@ -187,12 +200,9 @@ struct DimEntry {
     launch_fn launch;
     // GPI capability query: the on-chip kernel's launch plan for (dtype, N)
     GpiPlan (*gpi_plan)(int dtype, int N, int max_smem_optin);
-    // batched cache precompute on the device (precompute_kernel.cuh): device pointers, one model blob per instance
-    int (*precompute_batch)(int dtype, int64_t B, const void *A, const void *Bm, const void *f, const void *Qdiag, const void *Rdiag,
-                            const void *rho, void *models_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);
-    // batched sensitivity tables on the device (precompute_kernel.cuh): device pointers, dK [B][nu*nx], dP [B][nx*nx]
-    int (*sensitivity_batch)(int dtype, int64_t B, const void *A, const void *Bm, const void *Qdiag, const void *Rdiag, const void *rho,
-                             void *dK_out, void *dP_out, int32_t *sweeps_out, int sm_count, cudaStream_t stream);
+    // batched Riccati precompute on the device (riccati.cuh: riccati_kernel), the cache or with the tangent the tables
+    int (*riccati_batch)(int dtype, bool tangent, int64_t B, const RiccatiBatch<void> &a, int32_t *sweeps_out, int sm_count,
+                         cudaStream_t stream);
     // streamed lane-group kernel (gps_kernel.cuh): lanes per instance; 0 = shape not available
     int (*gps_lanes)(int dtype);
     // its per-instance-model variant (io.models): instances per CTA when the batch fills every SM, for the shape and the

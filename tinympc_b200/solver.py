@@ -56,14 +56,9 @@ def setup_problem(spec: ModelSpec, dtype=np.float32) -> MPCProblem:
     return p
 
 
-def setup_models(nx, nu, A, B, f, Qdiag, Rdiag, rho, dtype=np.float32, nthreads=0):
-    """tiny_setup's arithmetic for a heterogeneous batch: per-instance A [Bn,nx,nx], B [Bn,nx,nu] (row index first, like the
-    reference's examples), f [Bn,nx], user diagonals Qdiag [Bn,nx], Rdiag [Bn,nu], rho [Bn]  ->  packed model blobs
-    [Bn, blob] for BatchedTinySolver.solve(..., models=...)  (tinympc_batch_t.models, SURVEY §8f-2)."""
-    import os
-
-    lib = load()
-    dt = np.dtype(dtype).type
+def _batch_inputs(nx, nu, A, B, f, Qdiag, Rdiag, rho, dt):
+    """numpy inputs of the batched precompute: A [Bn,nx,nx], B [Bn,nx,nu] (row index first), f, Qdiag, Rdiag, rho ->
+    contiguous arrays of dtype dt, A and B column-major per instance"""
     A = np.asarray(A, dtype=dt)
     Bn = A.shape[0]
     A_ = np.ascontiguousarray(np.transpose(A.reshape(Bn, nx, nx), (0, 2, 1)))          # column-major per instance
@@ -72,11 +67,22 @@ def setup_models(nx, nu, A, B, f, Qdiag, Rdiag, rho, dtype=np.float32, nthreads=
     Q_ = np.ascontiguousarray(np.asarray(Qdiag, dtype=dt).reshape(Bn, nx))
     R_ = np.ascontiguousarray(np.asarray(Rdiag, dtype=dt).reshape(Bn, nu))
     r_ = np.ascontiguousarray(np.broadcast_to(np.asarray(rho, dtype=dt), (Bn,)))
-    M = int(lib.tinympc_b200_model_blob_elems(nx, nu))
-    out = np.zeros((Bn, M), dtype=dt)
+    return A_, B_, f_, Q_, R_, r_
+
+
+def setup_models(nx, nu, A, B, f, Qdiag, Rdiag, rho, dtype=np.float32, nthreads=0):
+    """tiny_setup's arithmetic for a heterogeneous batch: per-instance A [Bn,nx,nx], B [Bn,nx,nu] (row index first, like the
+    reference's examples), f [Bn,nx], user diagonals Qdiag [Bn,nx], Rdiag [Bn,nu], rho [Bn]  ->  packed model blobs
+    [Bn, blob] for BatchedTinySolver.solve(..., models=...)  (tinympc_batch_t.models, SURVEY §8f-2)."""
+    import os
+
+    lib = load()
+    dt = np.dtype(dtype).type
+    ins = _batch_inputs(nx, nu, A, B, f, Qdiag, Rdiag, rho, dt)
+    Bn = len(ins[0])
+    out = np.zeros((Bn, int(lib.tinympc_b200_model_blob_elems(nx, nu))), dtype=dt)
     vp = lambda a: C.c_void_p(a.ctypes.data)  # noqa: E731
-    check(lib.tinympc_b200_precompute_cache_batch(dtype_code(dt), nx, nu, Bn, vp(A_), vp(B_), vp(f_), vp(Q_), vp(R_), vp(r_),
-                                                  vp(out), nthreads or (os.cpu_count() or 1)))
+    check(lib.tinympc_b200_precompute_cache_batch(dtype_code(dt), nx, nu, Bn, *map(vp, ins), vp(out), nthreads or (os.cpu_count() or 1)))
     return out
 
 
@@ -88,18 +94,12 @@ def setup_sensitivity(nx, nu, A, B, f, Qdiag, Rdiag, rho, dtype=np.float32, nthr
 
     lib = load()
     dt = np.dtype(dtype).type
-    A = np.asarray(A, dtype=dt)
-    Bn = A.shape[0]
-    A_ = np.ascontiguousarray(np.transpose(A.reshape(Bn, nx, nx), (0, 2, 1)))          # column-major per instance
-    B_ = np.ascontiguousarray(np.transpose(np.asarray(B, dtype=dt).reshape(Bn, nx, nu), (0, 2, 1)))
-    f_ = np.ascontiguousarray(np.asarray(f, dtype=dt).reshape(Bn, nx))
-    Q_ = np.ascontiguousarray(np.asarray(Qdiag, dtype=dt).reshape(Bn, nx))
-    R_ = np.ascontiguousarray(np.asarray(Rdiag, dtype=dt).reshape(Bn, nu))
-    r_ = np.ascontiguousarray(np.broadcast_to(np.asarray(rho, dtype=dt), (Bn,)))
+    ins = _batch_inputs(nx, nu, A, B, f, Qdiag, Rdiag, rho, dt)
+    Bn = len(ins[0])
     dK, dP = np.zeros((Bn, nx, nu), dtype=dt), np.zeros((Bn, nx, nx), dtype=dt)  # column-major per instance
     vp = lambda a: C.c_void_p(a.ctypes.data)  # noqa: E731
-    check(lib.tinympc_b200_precompute_sensitivity_batch(dtype_code(dt), nx, nu, Bn, vp(A_), vp(B_), vp(f_), vp(Q_), vp(R_), vp(r_),
-                                                        vp(dK), vp(dP), nthreads or (os.cpu_count() or 1)))
+    check(lib.tinympc_b200_precompute_sensitivity_batch(dtype_code(dt), nx, nu, Bn, *map(vp, ins), vp(dK), vp(dP),
+                                                        nthreads or (os.cpu_count() or 1)))
     return np.transpose(dK, (0, 2, 1)), np.transpose(dP, (0, 2, 1))
 
 
@@ -254,28 +254,36 @@ class BatchedTinySolver:
         check(self._lib.tinympc_b200_solve_host(self._h, C.byref(cb)))
         return hb
 
+    def _device_precompute(self, entry, outputs, A, B, f, Qdiag, Rdiag, rho, want_sweeps):
+        """One batched precompute on the GPU through the C entry point `entry`, on the current stream.  Inputs as in
+        setup_models (numpy or torch, A [Bn,nx,nx] / B [Bn,nx,nu] row index first); outputs(Bn, dtype=, device=) makes the
+        zeroed output tensors.  Returns them and the sweeps [Bn] (int32, None unless want_sweeps)."""
+        import torch
+
+        p = self.problem
+        like = dict(dtype=torch.float32 if p.dtype == np.float32 else torch.float64, device=torch.device("cuda", self.device))
+        t = lambda a: torch.as_tensor(a, device=like["device"]).to(like["dtype"])  # noqa: E731
+        A_ = t(A).reshape(-1, p.nx, p.nx).transpose(1, 2).contiguous()  # column-major per instance
+        Bn = A_.shape[0]
+        B_ = t(B).reshape(Bn, p.nx, p.nu).transpose(1, 2).contiguous()
+        f_, Q_, R_ = t(f).reshape(Bn, p.nx).contiguous(), t(Qdiag).reshape(Bn, p.nx).contiguous(), t(Rdiag).reshape(Bn, p.nu).contiguous()
+        r_ = t(rho).reshape(-1).expand(Bn).contiguous()
+        outs = outputs(Bn, **like)
+        sweeps = torch.zeros(Bn, dtype=torch.int32, device=like["device"]) if want_sweeps else None
+        stream = torch.cuda.current_stream(like["device"]).cuda_stream
+        check(getattr(self._lib, entry)(self._h, Bn, *(a.data_ptr() for a in (A_, B_, f_, Q_, R_, r_)), *(o.data_ptr() for o in outs),
+                                        None if sweeps is None else sweeps.data_ptr(), C.c_void_p(stream)))
+        return outs, sweeps
+
     def setup_models_device(self, A, B, f, Qdiag, Rdiag, rho, want_sweeps=False):
         """setup_models on the GPU (tinympc_b200_precompute_cache_batch_device): inputs as in setup_models (numpy or torch,
         A [Bn,nx,nx] / B [Bn,nx,nu] row index first), result = torch CUDA tensor [Bn, blob] usable as `models=` of
         make_device_batch.  Bit-identical to the host routine."""
         import torch
 
-        p = self.problem
-        tdt = torch.float32 if p.dtype == np.float32 else torch.float64
-        dev = torch.device("cuda", self.device)
-        t = lambda a: torch.as_tensor(a, device=dev).to(tdt)  # noqa: E731
-        A_ = t(A).reshape(-1, p.nx, p.nx).transpose(1, 2).contiguous()  # column-major per instance
-        Bn = A_.shape[0]
-        B_ = t(B).reshape(Bn, p.nx, p.nu).transpose(1, 2).contiguous()
-        f_, Q_, R_ = t(f).reshape(Bn, p.nx).contiguous(), t(Qdiag).reshape(Bn, p.nx).contiguous(), t(Rdiag).reshape(Bn, p.nu).contiguous()
-        r_ = t(rho).reshape(-1).expand(Bn).contiguous()
-        M = int(self._lib.tinympc_b200_model_blob_elems(p.nx, p.nu))
-        out = torch.zeros((Bn, M), dtype=tdt, device=dev)
-        sweeps = torch.zeros(Bn, dtype=torch.int32, device=dev) if want_sweeps else None
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        check(self._lib.tinympc_b200_precompute_cache_batch_device(
-            self._h, Bn, A_.data_ptr(), B_.data_ptr(), f_.data_ptr(), Q_.data_ptr(), R_.data_ptr(), r_.data_ptr(), out.data_ptr(),
-            None if sweeps is None else sweeps.data_ptr(), C.c_void_p(stream)))
+        M = int(self._lib.tinympc_b200_model_blob_elems(self.problem.nx, self.problem.nu))
+        (out,), sweeps = self._device_precompute("tinympc_b200_precompute_cache_batch_device",
+                                                 lambda Bn, **like: (torch.zeros((Bn, M), **like),), A, B, f, Qdiag, Rdiag, rho, want_sweeps)
         return (out, sweeps) if want_sweeps else out
 
     def setup_sensitivity_device(self, A, B, f, Qdiag, Rdiag, rho, want_sweeps=False):
@@ -285,22 +293,11 @@ class BatchedTinySolver:
         routine."""
         import torch
 
-        p = self.problem
-        tdt = torch.float32 if p.dtype == np.float32 else torch.float64
-        dev = torch.device("cuda", self.device)
-        t = lambda a: torch.as_tensor(a, device=dev).to(tdt)  # noqa: E731
-        A_ = t(A).reshape(-1, p.nx, p.nx).transpose(1, 2).contiguous()  # column-major per instance
-        Bn = A_.shape[0]
-        B_ = t(B).reshape(Bn, p.nx, p.nu).transpose(1, 2).contiguous()
-        f_, Q_, R_ = t(f).reshape(Bn, p.nx).contiguous(), t(Qdiag).reshape(Bn, p.nx).contiguous(), t(Rdiag).reshape(Bn, p.nu).contiguous()
-        r_ = t(rho).reshape(-1).expand(Bn).contiguous()
-        dK = torch.zeros((Bn, p.nx, p.nu), dtype=tdt, device=dev)
-        dP = torch.zeros((Bn, p.nx, p.nx), dtype=tdt, device=dev)
-        sweeps = torch.zeros(Bn, dtype=torch.int32, device=dev) if want_sweeps else None
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        check(self._lib.tinympc_b200_precompute_sensitivity_batch_device(
-            self._h, Bn, A_.data_ptr(), B_.data_ptr(), f_.data_ptr(), Q_.data_ptr(), R_.data_ptr(), r_.data_ptr(), dK.data_ptr(),
-            dP.data_ptr(), None if sweeps is None else sweeps.data_ptr(), C.c_void_p(stream)))
+        nx, nu = self.problem.nx, self.problem.nu
+        (dK, dP), sweeps = self._device_precompute(
+            "tinympc_b200_precompute_sensitivity_batch_device",
+            lambda Bn, **like: (torch.zeros((Bn, nx, nu), **like), torch.zeros((Bn, nx, nx), **like)),  # column-major per instance
+            A, B, f, Qdiag, Rdiag, rho, want_sweeps)
         dK, dP = dK.transpose(1, 2), dP.transpose(1, 2)
         return (dK, dP, sweeps) if want_sweeps else (dK, dP)
 
